@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py - end-to-end FPS of the SMAP inference hot path (backbone + association + 3D lift) on B200.
+"""bench.py - end-to-end FPS of the SMAP inference hot path (backbone + association + 3D lift) on H100.
 
-Contract (driver): `python bench.py --gpus N --steps K --warmup W [--impl reference]`, under torchrun for
+Usage: `python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]`, under torchrun for
 N > 1; one JSON line on stdout from rank 0.
 
 A "step" = one pass of the whole hot path over one batch of B synthetic 832x512 frames per GPU
-(BASELINE.json configs[1]: batch=8, 1xB200, full backbone + GPU association; for N > 1 each rank owns its own
+(BASELINE.json configs[1]: batch=8 per GPU, full backbone + GPU association; for N > 1 each rank owns its own
 B frames and the per-image skeleton records are exchanged with ONE NCCL all-gather per step - weak scaling).
 
   value : frames/s with the input batch already resident in HBM (smapb_infer_device + all-gather)
@@ -13,13 +13,14 @@ B frames and the per-image skeleton records are exchanged with ONE NCCL all-gath
           memory, the whole path, D2H of the skeleton records) + all-gather
   roofline : the tensor-core convolution kernel (conv_tc_kernel, the dominant kernel): algorithmic conv FLOPs of
           one step / (its share of the step, from per-launch CUDA events, x the timed ms_per_step), against
-          MEASURED_PEAKS.json bf16_tflops_sustained.
+          MEASURED_PEAKS.json bf16_tflops_sustained when present, else the H100 SXM data-sheet dense bf16 rate.
           In bf16x3 mode every algorithmic FLOP is issued as 3 tensor-core FLOPs, so the tensor pipe runs at
           3 x frac of the bf16 peak.
   cpu_baseline : the CPU oracle of the same path (oracle/: PyTorch fp32 backbone on all cores + C++ association
           + numpy lift) on a bounded sample of the same workload.
-`--impl reference` times that CPU oracle alone (the reference has no GPU-free path of its own for the association
-and /root/reference does not exist on the GPU box; see DESIGN.md).
+`--impl reference` times that CPU oracle alone (the reference has no GPU-free path of its own for the association;
+see DESIGN.md).
+--dump-outputs DIR : the records of the last timed step as DIR/<field>.npy (inputs are seeded: compare two builds).
 """
 import argparse
 import json
@@ -52,21 +53,26 @@ def parse():
     ap.add_argument("--engines", type=int, default=int(os.environ.get("SMAPB_BENCH_ENGINES", "2")),
                     help="handles per GPU: >1 keeps that many batches in flight on independent streams")
     ap.add_argument("--profile-csv", default="")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the records of the last timed step as DIR/<field>.npy")
     ap.add_argument("--ncu-one-step", action="store_true",
                     help="bracket exactly one device-resident step with cudaProfilerStart/Stop and exit (for ncu --profile-from-start off)")
     return ap.parse_args()
+
+
+H100_SXM_BF16_TFLOPS, H100_SXM_HBM_GBS = 989.0, 3350.0  # NVIDIA H100 SXM data sheet: dense bf16, HBM3 bandwidth
 
 
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", H100_SXM_BF16_TFLOPS), d.get("hbm_gbs", H100_SXM_HBM_GBS), "measured"
+    return H100_SXM_BF16_TFLOPS, H100_SXM_HBM_GBS, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
-    """SM clock / throttle reasons during the timed region (B200_PROFILING.md recipe).  NVML in-process (a sample every
+    """SM clock / throttle reasons during the timed region.  NVML in-process (a sample every
     few ms, so that even a 0.2 s timed region gets tens of samples); `nvidia-smi` polling (~0.15 s per sample) only when
     the NVML binding is missing."""
 
@@ -222,22 +228,6 @@ class CpuOracle:
         return time.perf_counter() - t0, done, persons
 
 
-def ref_gpu_path_note():
-    """The reference's own single-GPU path (eager PyTorch/cuDNN backbone + unmodified dapalib per image + numpy lift) is
-    measured builder-side by tests/ref_gpu_compare.py on the same kind of box; bench.py only quotes the committed numbers."""
-    p = os.path.join(ROOT, "profiles", "r02_reference_gpu_path.json")
-    if not os.path.exists(p):
-        return None
-    d = json.load(open(p))
-    bb, e2e = d.get("backbone_only", {}), d.get("whole_gpu_path", {})
-    return {"value": d.get("value"), "unit": "frames/s", "what": d.get("what"),
-            "config4_15_persons_frames_per_s": e2e.get("reference_config4_15_persons", {}).get("frames_per_s"),
-            "backbone_only_ms_per_batch8": {"cudnn_tf32": bb.get("eager_cudnn_tf32_True_benchmark_False", {}).get("ms_per_batch"),
-                                            "cudnn_fp32": bb.get("eager_cudnn_tf32_False_benchmark_False", {}).get("ms_per_batch"),
-                                            "smap_b200_bf16x3": bb.get("smap_b200_bf16x3", {}).get("ms_per_batch")},
-            "source": "profiles/r02_reference_gpu_path.json (tests/ref_gpu_compare.py, builder-side run on a B200)"}
-
-
 def run_reference(args):
     """Reference arm: the CPU port of the whole path (oracle/) on the box's host cores; each step = a bounded sample of
     the workload (1 frame of the 8-frame batch).  Only the per-frame work is inside the timed region."""
@@ -260,16 +250,12 @@ def run_reference(args):
         "ms_per_step": 1e3 * total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "fp32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "frames_per_step": frames_per_step,
-                   "arm": "cpu port of the reference path (oracle/); the reference has no GPU-free association of its own "
-                          "and /root/reference does not travel to the GPU box"},
+                   "arm": "cpu port of the reference path (oracle/); the reference has no GPU-free association of its own"},
         "cpu_baseline": {"value": value, "unit": "frames/s", "cores": oracle.threads, "kind": "port",
                          "sample": "%d frame(s) per step x %d steps, whole path on host cores; weights/input/library set up "
                                    "outside the timed region" % (frames_per_step, args.steps)},
         "e2e": {"value": value, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
-    g = ref_gpu_path_note()
-    if g:
-        line["reference_gpu_path"] = g
     print(json.dumps(line))
 
 
@@ -280,7 +266,7 @@ def run_ours(args):
 
     from smap_b200 import dist as sdist
     from smap_b200 import schema
-    from smap_b200.engine import RECORD_BYTES, Engine, scale_row
+    from smap_b200.engine import RECORD_BYTES, Engine, records_to_numpy, scale_row
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -412,6 +398,14 @@ def run_ours(args):
     ms_dev, wall_dev = timed(run_device, args.steps)
     per_rank_ms = timed.per_rank
     launches = sum(e.launch_count() for e in engines) - l0
+    if args.dump_outputs and rank == 0:
+        # the records of the last timed step (index steps - 1), before any later run reuses its buffer
+        last = dev_outs[(args.steps - 1) % NE][:B]
+        rec = records_to_numpy(last)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name in ("pred3d", "root_depth", "pred2d", "count"):
+            a = rec[name]
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
     run_host(max(DEPTH, args.warmup))  # slot buffers + graphs for the slot pointers, then the host warm-up
     torch.cuda.synchronize()
@@ -444,13 +438,6 @@ def run_ours(args):
         share = conv_ms_serial / total_prof_ms
         conv_ms_per_step = share * ms_per_step  # in the timed (graph, NE handles) mode
         achieved = conv_flops * fwd / (conv_ms_per_step * 1e-3) * 1e-12 if conv_ms_per_step > 0 else 0.0
-        traffic, traffic_src = None, None
-        for name in ("r02_conv_traffic.json", "r01_conv_traffic.json"):
-            tp = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(tp):  # committed ncu capture of the same command (tools/gpu_profile.sh)
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj["mean_dram_bytes_per_launch"], "profiles/" + name
-                break
         # association (nms + paf + group) against the HBM roofline: algorithmic bytes per frame (SURVEY 8(d)) = heat-maps
         # read once 43*128*208*4 + root-depth map 128*208*4 + skeleton records written
         assoc_ms = prof["assoc"][0] / prof_steps
@@ -463,7 +450,7 @@ def run_ours(args):
             "dtype": "bf16x3 (split-bf16 operands, fp32 accumulate; fp32-faithful)" if args.precision == "bf16x3" else "bf16",
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "frames_per_gpu_per_step": B, "flip_tta": int(args.flip),
-                       "l2": "inputs rotate over %d distinct batches (%.0f MB) and every step streams >2 GB of activations (> 126 MB L2)"
+                       "l2": "inputs rotate over %d distinct batches (%.0f MB) and every step streams >2 GB of activations (> 50 MB L2)"
                              % (NROT, NROT * B * 3 * IN_H * IN_W * 4 / 1e6),
                        "parallelism": "dp%d, one ncclAllGather of skeleton records per step (handle-owned communicator, gather stream behind an event)" % world,
                        "batches_in_flight_per_gpu": NE,
@@ -482,19 +469,13 @@ def run_ours(args):
                          "tensor_pipe_flop_multiplier": 3 if args.precision == "bf16x3" else 1,
                          "kernel_ms_per_step": conv_ms_per_step, "share_of_step": share,
                          "how": "share (per-launch CUDA events, one handle, eager) x timed ms_per_step (graph replay, %d handles)" % NE,
-                         "kernel_ms_per_step_serialised_eager": conv_ms_serial,
-                         "traffic": traffic, "traffic_unit": "bytes per launch (dram read+write, ncu)",
-                         "traffic_source": traffic_src},
+                         "kernel_ms_per_step_serialised_eager": conv_ms_serial},
             "roofline_assoc": {"bound": "hbm", "kernel": "nms_kernel + paf_kernel + group_kernel",
                                "achieved": assoc_gbs, "peak": peak_bw, "unit": "GB/s", "frac": assoc_gbs / peak_bw,
                                "algorithmic_bytes_per_step": assoc_bytes, "kernel_ms_per_step": assoc_ms,
-                               "note": "batch 8: 3 launches of 120 / 112 / 8 CTAs - latency bound, not bandwidth bound; the "
-                                       "B=64 ncu capture in profiles/ is the bandwidth number"},
+                               "note": "batch 8: 3 launches of 120 / 112 / 8 CTAs - latency bound, not bandwidth bound"},
             "breakdown_ms_per_step": {k: v[0] / prof_steps for k, v in prof.items() if v[1]},
         }
-        g = ref_gpu_path_note()
-        if g:
-            line["reference_gpu_path"] = dict(g, ratio_value=value / g["value"] if g.get("value") else None)
         if not args.no_cpu_baseline:
             oracle = CpuOracle()
             x = oracle.make_frames(8)

@@ -1,5 +1,5 @@
 /*
- * smap_b200 - C ABI of the B200-native SMAP inference hot path.
+ * smap_b200 - C ABI of the H100-native SMAP inference hot path.
  *
  * Plain C: opaque handle, raw pointers, sizes, int error codes (0 = ok, < 0 = error; the text is
  * available from smapb_last_error()).  Nothing throws across this boundary, no torch types appear in
@@ -166,7 +166,7 @@ int smapb_submit_host_gather(smapb_handle* h, int slot, const float* imgs_nchw_h
                              int do_flip, smapb_record* all_records_host);
 /* Decoupled form for streams of batches (what bench.py times at N > 1): the whole path is enqueued on `stream`, the all-gather
  * on the handle's own gather stream behind an event - `stream` is ordered after the COMPUTE only, so a rank's compute stream
- * never waits for its peers (measured on 2 x B200: the stream-ordered form above costs 0.4 ms per 9.1 ms step - not in the
+ * never waits for its peers (the stream-ordered form above locks the ranks into step with each other - not in the
  * 14 us collective but in the lock-step it imposes on the ranks' two batches in flight; this form costs nothing).
  * all_records_dev is valid once smapb_gather_sync(h, s) has made a stream s wait for the outstanding exchanges.  The records
  * are double-buffered inside the handle: a call waits at most for the exchange issued two calls earlier.
@@ -216,10 +216,10 @@ int64_t smapb_launch_count(const smapb_handle* h);
  * 6-element arrays and, if csv_path is not NULL, writes one line per launch. */
 int smapb_profile_begin(smapb_handle* h);
 int smapb_profile_end(smapb_handle* h, double* ms_by_kind, int* launches_by_kind, const char* csv_path);
-/* Tile shapes of the tensor-core convolutions (process-wide): one line per layer geometry, "key<TAB>BLOCK_N<TAB>cta_group"
- * (cta_group: 1 = one CTA per 128-row tile, 2 = CTA pair (cta_group::2) per 256-row tile, 3 = CTA pair over halo strips - the
- * 3x3 stride-1 64->64 variant).  Whatever shape computes a layer, the result bits are the same.
- * Geometries found in the table use its entry; others are autotuned once per process (SMAPB_NO_AUTOTUNE=1: cost model)
+/* Tile shapes of the tensor-core convolutions (process-wide): one line per layer geometry, "key<TAB>BLOCK_N<TAB>variant"
+ * (BLOCK_N: 32, 64 or 128 output channels per 128-row tile; variant: 1 = one CTA per tile, the only one the sm_90a kernel has;
+ * entries it cannot run are stored but measured again).  Whatever shape computes a layer, the result bits are the same.
+ * Geometries found in the table with a shape the kernel has use its entry; others are autotuned once per process (SMAPB_NO_AUTOTUNE=1: cost model)
  * and added to it.  Loading the same table in every process makes tile selection - and with it every result bit -
  * independent of the handle, the process and the rank.  smapb_get_tile_table returns the bytes needed (incl. the
  * terminating 0) and fills buf up to cap. */

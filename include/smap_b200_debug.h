@@ -26,17 +26,15 @@ int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dim
 /* Environment switches read when a handle / plan is built (never on the per-call path):
  *   SMAPB_DEBUG_STOP=n        run only the first n ops of the plan
  *   SMAPB_DEBUG_SYNC=1        synchronise the stream after every launch
- *   SMAPB_DEBUG_ONEGROUP=fpro one epilogue group for fp32-out / post-add / residual / other layers
- *   SMAPB_FORCE_TILE=bn,cg    force a tile shape wherever it is valid;  SMAPB_NO_AUTOTUNE=1  cost model only
- *   SMAPB_PAIR=0|1|2          CTA pairs off / model / always;  SMAPB_NO_BN256=1  no one-CTA 128x256 tiles;  SMAPB_NO_HALO=1  no halo strips
+ *   SMAPB_FORCE_TILE=bn[,1]   force a tile width (32, 64, 128) wherever it is valid;  SMAPB_NO_AUTOTUNE=1  cost model only
  *   SMAPB_ONE_STREAM=1        no side stream;  SMAPB_NO_GRAPH=1  no CUDA graph replay;  SMAPB_PDL=1  programmatic dependent launch
  *   SMAPB_STEM=cuda           CUDA-core stem;  SMAPB_NO_FUSE_DS=1 / SMAPB_NO_FUSE_UP=1  unfused downsample / up-residual
  *   SMAPB_ROLES=1             per-role wait-cycle counters in smapb_conv_test
  *   SMAPB_ROLES_PLAN=file.csv the same counters for every conv launch of a profiled (smapb_profile_begin/end) run, i.e. inside the
  *                             real step (tools/roles_plan.py)
- *   SMAPB_TIMELINE=1          clock64 time line of CTA 0 of one launch in smapb_conv_test (set-up, first operands, main loop end,
- *                             chunk ends, exit)
- *   SMAPB_LIB=path (Python)   load another build of the library (A/B runs: tools/gpu_ab.sh, tools/ab_hash.py) */
+ *   SMAPB_TIMELINE=1          clock64 time line of CTA 0 of one launch in smapb_conv_test (set-up, first operands, last main loop end,
+ *                             epilogue done, exit)
+ *   SMAPB_LIB=path (Python)   load another build of the library (A/B runs: tools/ab_hash.py) */
 
 #ifdef __cplusplus
 }

@@ -14,7 +14,7 @@
  *   oracle_group    <- extensions/association.cpp:123-233 (findConnectedJoints)
  *   oracle_connect  <- extensions/association.cpp:34-120 + 123-233 composed
  *
- * FMA placement follows the sm_100 SASS of the unmodified reference build
+ * FMA placement follows the SASS of the unmodified reference build
  * (nvcc default -fmad=true): see SURVEY.md section 8(a) rows B3/B4.  Compile
  * with -ffp-contract=off so that gcc adds no contraction of its own; every
  * fused op below is an explicit fmaf().

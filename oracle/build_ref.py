@@ -41,7 +41,7 @@ def build(verbose=False):
     if not os.path.isdir(ext):
         return built_path()
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     from torch.utils.cpp_extension import load
 
     load(

@@ -121,7 +121,7 @@ def flip_merge(o2d, o2d_flip):
 
 def rescale_reference_cuda(hm):
     """exps/stage3_root2/test.py:111-112 as the reference actually executes it: `hmsIn` is a CUDA tensor and ATen's
-    CUDA true-divide by a Python scalar multiplies by the fp32 reciprocal (measured on B200, tools/diag_assoc.py);
+    CUDA true-divide by a Python scalar multiplies by the fp32 reciprocal (tools/diag_assoc.py);
     a CPU tensor would get an IEEE division.  In place on hm [B,43,h,w]; works on CPU and CUDA tensors alike."""
     r255 = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(255.0, dtype=torch.float32)
     r127 = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(127.0, dtype=torch.float32)

@@ -3,7 +3,7 @@ import ctypes
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# SMAPB_LIB: load another build of the same library (A/B comparisons of kernel changes, tools/gpu_ab.sh); the default is
+# SMAPB_LIB: load another build of the same library (A/B comparisons of kernel changes, tools/ab_hash.py); the default is
 # the in-tree build
 LIB_PATH = os.environ.get("SMAPB_LIB") or os.path.join(HERE, "lib", "libsmap_b200.so")
 
@@ -38,7 +38,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise SmapB200Error(
             "libsmap_b200.so is not built (%s). Run `python -m smap_b200.build` "
-            "(needs nvcc with sm_100a support). There is no CPU fallback." % LIB_PATH)
+            "(needs nvcc with sm_90a support). There is no CPU fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     c = ctypes
     vp, i32, i64 = c.c_void_p, c.c_int, c.c_int64

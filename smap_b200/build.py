@@ -1,4 +1,4 @@
-"""Build libsmap_b200.so (sm_100a only) in-tree with nvcc.  `python -m smap_b200.build [-f]`."""
+"""Build libsmap_b200.so (sm_90a only) in-tree with nvcc.  `python -m smap_b200.build [-f]`."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsmap_b200.so")
 SOURCES = ["engine.cu", "assoc.cu", "elementwise.cu", "refine.cu", "preprocess.cu", "json_out.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 
@@ -25,7 +25,7 @@ def build_variant(name, defines):
         objs.append(obj)
         subprocess.check_call(["nvcc"] + NVCC_FLAGS + ["-D" + d for d in defines] + ["-c", os.path.join(CSRC, s), "-o", obj])
     lib = os.path.join(LIBDIR, "libsmap_b200_%s.so" % name)
-    subprocess.check_call(["nvcc", "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call(["nvcc", "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return lib
 
 
@@ -44,7 +44,7 @@ def build(force=False, verbose=False):
                 print(" ".join(cmd))
             subprocess.check_call(cmd)
     if force or not os.path.exists(LIB) or any(_newer(o, LIB) for o in objs):
-        cmd = ["nvcc", "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = ["nvcc", "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         if verbose:
             print(" ".join(cmd))
         subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// Depth-aware part association on sm_100a: batched, device-resident, bit-exact with the reference.
+// Depth-aware part association on sm_90a: batched, device-resident, bit-exact with the reference.
 //
 //   nms_kernel    <- extensions/gpu/nmsBase.cu:10-135 (register + thrust scan + write, fused)
 //   paf_kernel    <- extensions/gpu/bodyPartConnectorBase.cu:11-63,104-150
@@ -8,7 +8,7 @@
 // Data movement: every heat-map / PAF plane is staged ONCE into shared memory with 1-D bulk async copies
 // (cp.async.bulk -> UBLKCP, completion on an mbarrier); all neighbourhood / line-integral gathers then hit
 // shared memory.  Floating-point expressions whose rounding feeds a comparison are pinned with explicit
-// __f*_rn intrinsics in the contraction pattern of the reference's sm_100 binary (SURVEY.md 8(a) B3/B4).
+// __f*_rn intrinsics in the contraction pattern of the reference's binary (SURVEY.md 8(a) B3/B4).
 #include "assoc.h"
 #include "common.cuh"
 
@@ -316,13 +316,13 @@ struct PafSamplerPlanes {  // both planes behind ordinary pointers (shared or gl
 };
 // STAGED: both planes fit in shared memory (the parity configuration 128x208: 213 KB) and are staged once; otherwise
 // (larger maps, e.g. 256x256 at a 1024x1024 input) the line integrals gather straight from global memory / L2.
-// Two restructurings were built, measured on B200 at B = 64 crowded scenes and dropped (this kernel: 55.6 us, 3.46 TB/s):
+// Two restructurings were built and dropped (timed at B = 64 crowded scenes on the GPU this kernel was first written for):
 //  * a cluster of two CTAs per item, one plane each, the other component read through distributed shared memory, so that
 //    two CTAs fit on an SM and one's copy overlaps the other's scoring: 78.5 us - 25 dependent DSMEM loads per pair;
 //  * a persistent CTA with the x and y planes in separate buffers and the scoring split in an x pass and a y pass, so that
 //    a plane is refilled while the other is in use: 57 - 60 us - the scoring of an item (IEEE sqrt / divisions of the
-//    reference, a <= 25-sample chain per pair, CTA barriers) takes ~6 us, longer than the 4.5 us its planes need at 7 TB/s
-//    (tools/probes/bw_probe.cu), so the copy engine was never the bottleneck of this kernel at 15 persons per frame.
+//    reference, a <= 25-sample chain per pair, CTA barriers) takes longer than its planes
+//    need to arrive, so the copy engine was never the bottleneck of this kernel at 15 persons per frame.
 template <bool STAGED>
 __global__ void __launch_bounds__(PAF_THREADS, 1)
 paf_kernel(const float* __restrict__ hms, int nchan, int h, int w, const float* __restrict__ peaks,
@@ -345,7 +345,7 @@ paf_kernel(const float* __restrict__ hms, int nchan, int h, int w, const float* 
     // two peak lists (dependent global loads, ~1 us each) then arrive while the copy engine streams the 213 KB.  An item with
     // an empty peak list has staged its planes for nothing - on a frame that contains people every limb has candidates -
     // but the critical path of an item shrinks from  counts -> planes -> peak lists -> scores  to  planes -> scores
-    // (B = 64 crowded scenes, round 2: 56 us before; profiles/ holds the capture of this form).
+    // (B = 64 crowded scenes).
     if (STAGED) {
         if (threadIdx.x == 0) {
             mbar_init(bar, 1);
@@ -1020,7 +1020,7 @@ cudaError_t launch_nms(const float* hms, int nchan, int B, int h, int w, float t
     const bool vec = (h * w) % 128 == 0;
     const long long warps_needed = vec ? (words + 15) / 16 : words;  // 16 words (VEC, 4 groups) or 1 word per warp step
     long long blocks = (warps_needed * 32 + NMSF_THREADS - 1) / NMSF_THREADS;
-    const long long cap = vec ? 148LL * 4 : 148LL * 8 * 4;  // VEC: one persistent wave; scalar: the warps stride over the rest
+    const long long cap = vec ? 132LL * 4 : 132LL * 8 * 4;  // VEC: one persistent wave; scalar: the warps stride over the rest
     if (blocks > cap) blocks = cap;
     if (vec)
         nms_flag_kernel<true><<<(unsigned)blocks, NMSF_THREADS, 0, st>>>(hms, nchan, B, h, w, thr, masks);

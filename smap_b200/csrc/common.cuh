@@ -1,12 +1,12 @@
-// Shared device helpers for the smap_b200 kernels (sm_100a only).
+// Shared device helpers for the smap_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
 
-#ifndef __CUDA_ARCH_FEAT_SM100_ALL
+#ifndef __CUDA_ARCH_FEAT_SM90_ALL
 #if defined(__CUDA_ARCH__)
-#error "smap_b200 kernels must be compiled with -gencode arch=compute_100a,code=sm_100a"
+#error "smap_b200 kernels must be compiled with -gencode arch=compute_90a,code=sm_90a"
 #endif
 #endif
 
@@ -22,7 +22,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
-// make mbarrier.init visible to the async proxy (TMA / tcgen05.commit)
+// make mbarrier.init visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }

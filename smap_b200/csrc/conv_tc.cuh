@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   y[n, oy, ox, co] = epilogue( sum_{ky,kx,ci} x[n, oy*s+ky-p, ox*s+kx-p, ci] * w[co, ci, ky, kx] )
 //
@@ -9,24 +9,20 @@
 //      offset, zero padding is TMA out-of-bounds fill, conv stride is the map's elementStrides.
 //   B: 4-D tensor map (Cin, Cout, tap, term) over the repacked (BN-folded) weights.
 // Precision: "bf16x3" - every fp32 value v is carried as two bf16 planes (hi = bf16(v), lo = bf16(v - hi));
-// a product a*b is issued as 3 MMAs  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  into the same fp32 TMEM accumulator
+// a product a*b is issued as 3 MMAs  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  into the same fp32 accumulator
 // (dropped terms are O(2^-16) relative) - fp32-faithful results at 3x the bf16 MMA count.  NTERMS = 1 is the
 // plain bf16 fast mode.
 //
 // Warp roles (384 threads, persistent CTA, static tile schedule):
-//   warp 0 : operand TMA producer (one lane)        warp 1 : MMA issuer (one lane)
-//   warp 2 : TMEM allocator                         warp 3 : residual TMA producer (one lane)
-//   warps 4-11 : epilogue, two groups of 4 warps taking alternate 32-column chunks:
-//                TMEM -> regs (+bias +residual, ReLU, hi/lo split) -> swizzled smem -> TMA store
-// Pipelines: operand full/empty ring (TMA <-> MMA), double-buffered TMEM accumulators (MMA <-> epilogue),
-// residual full/empty ring (TMA <-> epilogue), bulk-async store groups (epilogue <-> TMA store).
-// The epilogue never touches global memory with per-thread loads/stores on the main path: the residual tile
-// arrives by TMA ahead of time and the output leaves by TMA in 32-channel x 128-pixel boxes.  It is latency bound (one
-// dependent chain per 32-column chunk, two warps per scheduler), so it is written for few instructions - packed fp32
-// adds and mixed bf16/fp32 adds and fmas of sm_100 - and for overlap: the next chunk's accumulators are requested from
-// TMEM while the current chunk is converted, and the accumulator buffer is handed back after the tile's last read.
-// Taps of a k x k filter are visited kx-major; all variants (tile widths, CTA pairs, halo strips) accumulate every output
-// element in the same order, i.e. produce the same bits.
+//   warp 0 : operand TMA producer (one lane)        warp 1 : epilogue-input TMA producer (one lane)
+//   warpgroups 1-2 (warps 4-11) : consumers; warpgroup g owns rows [64 g, 64 g + 64) of the 128-row tile and all BLOCK_N
+//                columns: wgmma m64nBLOCK_Nk16 into registers, then the epilogue from those registers in 32-column
+//                chunks: (+bias +residual, ReLU, +skips, hi/lo split) -> swizzled smem -> one TMA store per chunk
+// Pipelines: operand full/empty ring (TMA <-> wgmma), epilogue-input full/empty ring (TMA <-> epilogue), bulk-async store
+// groups (epilogue <-> TMA store).  The producer runs ahead into the next tile's operands while the consumers run the
+// epilogue of the current one.
+// Taps of a k x k filter are visited kx-major and every tile width issues the same MMAs per output element in the same
+// order, i.e. all tile shapes produce the same bits.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -57,7 +53,6 @@ struct alignas(64) ConvParams {
     float* out_f32;      // fp32 NHWC (heads), or null
     long long plane_stride;  // elements between the hi and lo planes (= N*H*W*Cout)
     int relu;
-    int one_group;  // debug: epilogue group 0 takes every chunk
     int reverse;    // walk the tile list back to front (the consumer of a tensor starts with the rows its producer wrote
                     // last, which are the ones still resident in L2)
     // fused bilinear residual (Upsample_unit, model/smap.py:211-217): tmR[0] is a low-resolution tensor [N,Hi,Wi,C];
@@ -68,7 +63,7 @@ struct alignas(64) ConvParams {
     long long* dbg_tl;  // optional: clock64 time line of CTA 0 (SMAPB_TIMELINE, smapb_conv_test only), null in production
 };
 
-// ---- tcgen05 / TMA PTX wrappers -----------------------------------------------------------------
+// ---- TMA / wgmma PTX wrappers -------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                             int c2, int c3, int c4) {
     asm volatile(
@@ -88,50 +83,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_128B operand descriptor: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;  // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
-    uint4 r;
-    asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-    return r;
-}
-
-
 __device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3,
                                              int c4) {
     asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(map),
@@ -144,123 +95,95 @@ __device__ __forceinline__ void bulk_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ uint4 lds_v4(uint32_t addr) {
-    uint4 r;
-    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
+// named barrier of the two consumer warpgroups
+__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+    uint32_t r;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(addr));
     return r;
 }
-__device__ __forceinline__ void sts_v4(uint32_t addr, uint4 v) {
-    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-                 : "memory");
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-// byte offset of 16-byte chunk j (0..3) of row r in a [128 rows x 64 B] SWIZZLE_64B box
+// byte offset of 16-byte chunk j (0..3) of row r in a [rows x 64 B] SWIZZLE_64B box
 __device__ __forceinline__ uint32_t sw64_off(int r, int j) { return (uint32_t)(r * 64 + ((j ^ ((r >> 1) & 3)) << 4)); }
 
 // ATen bilinear, align_corners=True: src = dst * (in-1)/(out-1) in fp32; i0 = (int)src
 __device__ __forceinline__ float up_scale(int in, int out) { return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f; }
 __device__ __forceinline__ int up_src_index(int dst, int in, int out) { return (int)(up_scale(in, out) * (float)dst); }
 
-__device__ __forceinline__ uint4 ldg_v4(const void* p) {
-    uint4 r;
-    asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
-    return r;
-}
-
-
-
-// ---- epilogue arithmetic: packed fp32 (FADD2) and mixed bf16 -> fp32 (FHADD / FHFMA) instructions of sm_100 -------------
-// All of them are IEEE round-to-nearest single operations, i.e. bit-identical to the scalar fp32 sequences they replace
-// (bf16 -> fp32 widening is exact): the point is the instruction count of the epilogue, which is latency bound.
-// (a0, a1) += (b0, b1)
-__device__ __forceinline__ void fadd2(float& a0, float& a1, float b0, float b1) {
-    asm("{\n\t.reg .b64 ra, rb;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tadd.rn.f32x2 ra, ra, rb;\n\t"
-        "mov.b64 {%0, %1}, ra;\n\t}"
-        : "+f"(a0), "+f"(a1)
-        : "f"(b0), "f"(b1));
-}
-// fp32(low / high bf16 half of w) + c
-__device__ __forceinline__ float add_bf16lo(uint32_t w, float c) {
-    float d;
-    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %1;\n\tadd.rn.f32.bf16 %0, l, %2;\n\t}" : "=f"(d) : "r"(w), "f"(c));
-    return d;
-}
-__device__ __forceinline__ float add_bf16hi(uint32_t w, float c) {
-    float d;
-    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %1;\n\tadd.rn.f32.bf16 %0, h, %2;\n\t}" : "=f"(d) : "r"(w), "f"(c));
-    return d;
-}
-// c - fp32(low / high bf16 half of w), as one fma with the bf16 constant -1 (the product is exact)
-__device__ __forceinline__ float sub_bf16lo(float c, uint32_t w) {
-    float d;
-    asm("{\n\t.reg .b16 l, h, m;\n\tmov.b32 {l, h}, %1;\n\tmov.b16 m, 0xbf80;\n\tfma.rn.f32.bf16 %0, l, m, %2;\n\t}"
-        : "=f"(d)
-        : "r"(w), "f"(c));
-    return d;
-}
-__device__ __forceinline__ float sub_bf16hi(float c, uint32_t w) {
-    float d;
-    asm("{\n\t.reg .b16 l, h, m;\n\tmov.b32 {l, h}, %1;\n\tmov.b16 m, 0xbf80;\n\tfma.rn.f32.bf16 %0, h, m, %2;\n\t}"
-        : "=f"(d)
-        : "r"(w), "f"(c));
-    return d;
-}
 // bf16x2 pack with round-to-nearest-even: low half = a, high half = b
 __device__ __forceinline__ uint32_t cvt_bf16x2(float a, float b) {
     uint32_t w;
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(b), "f"(a));
     return w;
 }
+// the fp32 values (low half, high half) a hi/lo pair of bf16x2 words carries: hi + lo, exact widening, one rounding
+__device__ __forceinline__ float2 planes_to_f2(uint32_t h, uint32_t l) {
+    return make_float2(bf16lo_to_f(h) + bf16lo_to_f(l), bf16hi_to_f(h) + bf16hi_to_f(l));
+}
 
-// ---- 2-CTA (cta_group::2) helpers -----------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
+// wgmma shared-memory operand descriptor: K-major, SWIZZLE_128B, rows of 128 B, 8-row groups 1024 B apart (SBO);
+// LBO is unused for swizzled K-major operands.  A k-step of 16 bf16 (32 B) inside the swizzle atom adds 2 to the address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;  // SWIZZLE_128B
+    return d;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// shared::cluster address of `local_addr` in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads whose completion is signalled on an mbarrier given by shared::cluster address (the pair leader's barrier)
-__device__ __forceinline__ void tma_load_5d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1,
-                                                int c2, int c3, int c4) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]^T, fp32 accumulators in the wgmma fragment layout: thread t of the warpgroup holds
+// rows 16 (t / 32) + (t % 32) / 4 + {0, 8} and columns 8 j + 2 (t % 4) + {0, 1} as d[4 j + 2 {0, 1} + {0, 1}]
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-        "%4, %5, %6, %7}], [%2];" ::"r"(dst),
-        "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
+        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, "
+        "%36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, "
+        "%59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tma_load_4d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1,
-                                                int c2, int c3) {
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-        "%4, %5, %6}], [%2];" ::"r"(dst),
-        "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
+        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, "
+        "1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_commit_cg2(uint64_t* bar) {  // arrive on the same barrier offset in both CTAs
+__device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"((uint16_t)3)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
+        "%13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_mma_bf16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+template <int BLOCK_N>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (BLOCK_N == 128) wgmma_m64n128(d, adesc, bdesc, accumulate);
+    else if constexpr (BLOCK_N == 64) wgmma_m64n64(d, adesc, bdesc, accumulate);
+    else wgmma_m64n32(d, adesc, bdesc, accumulate);
 }
 
 // mbar_wait that also returns the cycles spent waiting (role-level profiling; only used when p.dbg != null)
@@ -275,71 +198,48 @@ __device__ __forceinline__ long long mbar_wait_timed(uint64_t* bar, uint32_t par
 }
 
 // RING: 0 = no epilogue inputs, 1 = residual / skip tensors through the ring, 2 = fused bilinear residual (up_mode)
-// HALO: 3x3 stride-1 layers with 64 input channels.  Instead of nine shifted 128-pixel A tiles per 64-channel block (nine TMA
-// loads of the same pixels: these layers are L2 -> SM bound at a third of the MMA rate), the tile is 8 x 16 pixels and the
-// operand "stages" are three column-shifted HALO strips of 8 x 18 pixels (one per kx): a tile row of 8 pixels is exactly one
-// 1024-byte SWIZZLE_128B atom, so the A operand of tap (ky, kx) is strip kx read from row ky on - a plain K-major descriptor
-// whose start address moves by ky * 1024 bytes.  Three loads of 36 KB replace nine of 32 KB, and the weights of all nine taps
-// (this CTA's rows) stay resident in shared memory for the whole kernel.  Taps are visited kx-major (as in every other
-// variant, so that results do not depend on the variant): strip kx is free for the next tile after its three taps.
-template <int BLOCK_N, int NTERMS, int RING, int CG = 1, bool HALO = false>
+template <int BLOCK_N, int NTERMS, int RING>
 struct ConvCfg {
     static constexpr int TA = (NTERMS == 3) ? 2 : 1;  // operand planes held per stage
-    static constexpr int HALO_ROWS = 18 * 8;           // 8 x 18 pixels per strip
-    static constexpr int A_BYTES = HALO ? HALO_ROWS * 128 : 128 * 128;  // rows x 64 bf16
-    // CG = 2: a pair of CTAs (cta_group::2) computes a 256 x BLOCK_N tile; each CTA stages its own 128 rows of A and
-    // BLOCK_N/2 rows of B, and owns the 128 x BLOCK_N slice of the accumulator in its TMEM
-    static constexpr int B_BYTES = (BLOCK_N / CG) * 128;
-    static constexpr int STAGE_BYTES = HALO ? TA * A_BYTES : TA * (A_BYTES + B_BYTES);
-    static constexpr int B_RES_BYTES = HALO ? 9 * TA * B_BYTES : 0;  // resident weights (HALO)
-    static constexpr int CHUNK_COLS = 32;              // epilogue granularity (one tcgen05.ld x32)
-    static constexpr int CHUNKS = BLOCK_N / CHUNK_COLS;
-    static constexpr int CHUNK_BYTES = 128 * 64;       // one plane of one chunk: 128 rows x 32 bf16
+    static constexpr int A_BYTES = 128 * 128;         // rows x 64 bf16
+    static constexpr int B_BYTES = BLOCK_N * 128;
+    static constexpr int STAGE_BYTES = TA * (A_BYTES + B_BYTES);
+    static constexpr int CHUNKS = BLOCK_N / 32;       // epilogue granularity: 32 columns (one TMA store box)
+    static constexpr int CHUNK_BYTES = 128 * 64;      // one plane of one chunk: 128 rows x 32 bf16
     static constexpr int SLOT_BYTES = TA * CHUNK_BYTES;  // hi (+ lo)
-    static constexpr int OUT_BUFS = 2;  // one staging slot per epilogue group
+    static constexpr int OUT_BUFS = 2;  // store staging, alternate chunks
     // RING: the layer streams epilogue inputs (residual / skip adds); without it the smem goes to operand stages
-    // (CTA pairs with BLOCK_N < 256 trade ring depth for a third operand stage)
-    static constexpr int RES_BUFS = !RING ? 0 : (CG == 2 && BLOCK_N < 256) ? 2 : (BLOCK_N >= 128) ? 4 : 2;
-    static constexpr int SPG = RING ? RES_BUFS / 2 : 1;  // ring slots per epilogue group
+    static constexpr int RES_BUFS = RING ? 2 : 0;
+    static constexpr int RES_DIV = RING ? RES_BUFS : 1;  // RES_BUFS as a divisor (no ring slots are used when RING == 0)
     static constexpr int EPI_BYTES = (OUT_BUFS + RES_BUFS) * SLOT_BYTES;
     static constexpr int SMEM_LIMIT = 227 * 1024;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES - B_RES_BYTES) / STAGE_BYTES;
-    static constexpr int STAGES = HALO ? 3 : STAGES_RAW > 8 ? 8 : STAGES_RAW;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + B_RES_BYTES + EPI_BYTES + 2048;  // 1 KB control + 1 KB alignment slack
-    static constexpr int TMEM_COLS = (2 * BLOCK_N <= 32) ? 32 : (2 * BLOCK_N <= 64) ? 64 : (2 * BLOCK_N <= 128) ? 128
-                                     : (2 * BLOCK_N <= 256) ? 256 : 512;
-    static_assert(STAGES >= 2 && STAGES_RAW >= STAGES, "need at least a double buffer");
-    static_assert(BLOCK_N % 32 == 0 && BLOCK_N >= 32 && BLOCK_N <= 256, "BLOCK_N");
-    static_assert(!HALO || (RING == 0 && NTERMS == 3), "the halo variant has no epilogue inputs");
+    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
+    static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 2048;  // 1 KB control + 1 KB alignment slack
+    static_assert(STAGES >= 2, "need at least a double buffer");
+    static_assert(BLOCK_N == 32 || BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
 };
 
-template <int BLOCK_N, int NTERMS, int RING, int CG = 1, bool HALO = false>
+template <int BLOCK_N, int NTERMS, int RING>
 __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__ ConvParams p) {
-    using Cfg = ConvCfg<BLOCK_N, NTERMS, RING, CG, HALO>;
+    using Cfg = ConvCfg<BLOCK_N, NTERMS, RING>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr bool UP = (RING == 2);  // the ring carries low-resolution patches the epilogue interpolates
     extern __shared__ unsigned char smem_raw[];
     // control block at the front, operand ring + epilogue staging 1024-aligned behind it
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_raw);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tfull_bar = empty_bar + STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint64_t* rfull_bar = tempty_bar + 2;
+    uint64_t* rfull_bar = empty_bar + STAGES;
     uint64_t* rempty_bar = rfull_bar + Cfg::RES_BUFS;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(rempty_bar + Cfg::RES_BUFS);
-    uint64_t* bres_bar = reinterpret_cast<uint64_t*>(smem_raw + 512);  // HALO: the resident weights have landed
     const uint32_t ring = (smem_u32(smem_raw) + 1024u + 1023u) & ~1023u;
-    const uint32_t bres = ring + STAGES * Cfg::STAGE_BYTES;  // HALO: [tap][plane][BLOCK_N / CG rows] weights
-    const uint32_t out_stage = bres + Cfg::B_RES_BYTES;
+    const uint32_t out_stage = ring + STAGES * Cfg::STAGE_BYTES;
     const uint32_t res_stage = out_stage + Cfg::OUT_BUFS * Cfg::SLOT_BYTES;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const bool tl = p.dbg_tl != nullptr && blockIdx.x == 0;  // time line of CTA 0: [0] entry [1] set-up done [2] first operands
-                                                            // [3] main loop end [4] last tile's accumulators [5..12] chunk ends [13] epilogue
-                                                            // done [14] exit
+                                                            // [3] main loop end of the last tile [13] epilogue done [15] exit
     if (tl && threadIdx.x == 0) p.dbg_tl[0] = clock64();
-    const uint32_t cta_rank = (CG == 2) ? cluster_ctarank() : 0u;  // rank 0 = pair leader (issues the MMAs)
     const int n_extra = RING ? p.has_res + p.n_post : 0;  // epilogue input tensors streamed through the ring
     const bool tma_out = p.out != nullptr;
 
@@ -353,37 +253,15 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; s++) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&tfull_bar[a], 1);
-            mbar_init(&tempty_bar[a], 256 * CG);  // the leader's MMA waits for the epilogues of both CTAs
+            mbar_init(&empty_bar[s], 8);  // lane 0 of each consumer warp
         }
         for (int s = 0; s < Cfg::RES_BUFS; s++) {
             mbar_init(&rfull_bar[s], 1);
-            mbar_init(&rempty_bar[s], 128);
+            mbar_init(&rempty_bar[s], 256);
         }
-        if (HALO) mbar_init(bres_bar, 1);
         fence_mbar_init();
     }
-    if (warp == 2) {
-        if (CG == 1) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                         "n"(Cfg::TMEM_COLS)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                         "n"(Cfg::TMEM_COLS)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CG == 2) cluster_sync_all();  // peer barriers are initialised before any remote arrive / TMA signal
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int num_kb1 = p.kh * p.kw * p.kchunks;
     const int num_kb = num_kb1 + p.kchunks2;
@@ -396,49 +274,13 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
 
     if (warp == 0) {
         // ============================ operand TMA producer ====================
-        if (lane == 0 && HALO) {
-            // weights first: all nine taps of this CTA's rows, resident for the whole kernel (n_tiles == 1)
-            const uint32_t bbar = (CG == 2) ? mapa_u32(smem_u32(bres_bar), 0u) : 0u;
-            if (cta_rank == 0) mbar_arrive_expect_tx(bres_bar, Cfg::B_RES_BYTES * CG);
-            const int brow = (int)cta_rank * (BLOCK_N / CG);
-            for (int tap = 0; tap < 9; tap++) {
-#pragma unroll
-                for (int t = 0; t < Cfg::TA; t++) {
-                    const uint32_t db = bres + (uint32_t)((tap * Cfg::TA + t) * Cfg::B_BYTES);
-                    if (CG == 1) tma_load_4d(db, &p.tmB, bres_bar, 0, brow, tap, t);
-                    else tma_load_4d_cg2(db, &p.tmB, bbar, 0, brow, tap, t);
-                }
-            }
-            // then, per tile, the three column-shifted strips of (th + 2) x 8 pixels; strip kx is stage kx
-            uint32_t phase = 0;
-            long long w_empty = 0;
-            for (int tile = blockIdx.x / CG; tile < p.total_tiles; tile += gridDim.x / CG) {
-                const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-                const int mt = te * CG + (int)cta_rank;
-                const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
-                const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-                const int x_in0 = (tx << p.tw_log2) - p.pad_x, y_in0 = ty * p.th - p.pad_y;
-                for (int kx = 0; kx < 3; kx++) {
-                    w_empty += mbar_wait_timed(&empty_bar[kx], phase ^ 1u, p.dbg != nullptr);
-                    if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[kx], Cfg::STAGE_BYTES * CG);
-                    const uint32_t fbar = (CG == 2) ? mapa_u32(smem_u32(&full_bar[kx]), 0u) : 0u;
-#pragma unroll
-                    for (int t = 0; t < Cfg::TA; t++) {
-                        const uint32_t da = ring + (uint32_t)(kx * Cfg::STAGE_BYTES + t * Cfg::A_BYTES);
-                        if (CG == 1) tma_load_5d(da, &p.tmA, &full_bar[kx], 0, x_in0 + kx, y_in0, img, t);
-                        else tma_load_5d_cg2(da, &p.tmA, fbar, 0, x_in0 + kx, y_in0, img, t);
-                    }
-                }
-                phase ^= 1u;
-            }
-            if (p.dbg) atomicAdd((unsigned long long*)&p.dbg[0], (unsigned long long)w_empty);
-        } else if (lane == 0) {
+        if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             long long w_empty = 0;
-            for (int tile = blockIdx.x / CG; tile < p.total_tiles; tile += gridDim.x / CG) {
+            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
                 const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-                const int nt = te % p.n_tiles, mt = (te / p.n_tiles) * CG + (int)cta_rank;
+                const int nt = te % p.n_tiles, mt = te / p.n_tiles;
                 const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
                 const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
                 const int x_in0 = (tx << p.tw_log2) * p.stride - p.pad_x;
@@ -446,21 +288,15 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                 for (int kb = 0; kb < num_kb; kb++) {
                     w_empty += mbar_wait_timed(&empty_bar[stage], phase ^ 1u, p.dbg != nullptr);
                     const uint32_t sbase = ring + stage * Cfg::STAGE_BYTES;
-                    // CG = 2: both CTAs' loads complete on the LEADER's full barrier, which the leader arms for both
-                    if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES * CG);
-                    const uint32_t fbar = (CG == 2) ? mapa_u32(smem_u32(&full_bar[stage]), 0u) : 0u;
-                    const int brow = nt * BLOCK_N + (int)cta_rank * (BLOCK_N / CG);  // this CTA's rows of the weight tile
+                    mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+                    const int brow = nt * BLOCK_N;  // rows of the weight tile
                     int kcol, tapc, ax, ay;
                     const CUtensorMap* amap;
                     if (kb < num_kb1) {
-                        // taps are visited kx-major (kx outer, ky inner) in EVERY variant: the accumulation order - hence
-                        // every result bit - is the same whichever variant computes a layer (see HALO above)
+                        // taps are visited kx-major (kx outer, ky inner): the accumulation order - hence every result
+                        // bit - is the same whichever tile shape computes a layer
                         const int ts = kb / p.kchunks, kc = kb - ts * p.kchunks;
-#ifdef SMAPB_TAP_KY_MAJOR  // the order of the builds before the halo variant existed: only for A/B digests (tools/ab_hash.py)
-                        const int ky = ts / p.kw, kx = ts - ky * p.kw;
-#else
                         const int kx = ts / p.kh, ky = ts - kx * p.kh;
-#endif
                         amap = &p.tmA, kcol = kc * 64, tapc = ky * p.kw + kx, ax = x_in0 + kx, ay = y_in0 + ky;
                     } else {  // K-concatenated second input (1x1, own stride): weight columns continue after Cin
                         const int kc2 = kb - num_kb1;
@@ -471,13 +307,8 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
 #pragma unroll
                     for (int t = 0; t < Cfg::TA; t++) {
                         const uint32_t da = sbase + t * Cfg::A_BYTES, db = sbase + Cfg::TA * Cfg::A_BYTES + t * Cfg::B_BYTES;
-                        if (CG == 1) {
-                            tma_load_5d(da, amap, &full_bar[stage], kcol, ax, ay, img, t);
-                            tma_load_4d(db, &p.tmB, &full_bar[stage], wcol, brow, tapc, t);
-                        } else {
-                            tma_load_5d_cg2(da, amap, fbar, kcol, ax, ay, img, t);
-                            tma_load_4d_cg2(db, &p.tmB, fbar, wcol, brow, tapc, t);
-                        }
+                        tma_load_5d(da, amap, &full_bar[stage], kcol, ax, ay, img, t);
+                        tma_load_4d(db, &p.tmB, &full_bar[stage], wcol, brow, tapc, t);
                     }
                     if (++stage == STAGES) {
                         stage = 0;
@@ -488,118 +319,20 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
             if (p.dbg) atomicAdd((unsigned long long*)&p.dbg[0], (unsigned long long)w_empty);
         }
     } else if (warp == 1) {
-        // ============================ MMA issuer ==============================
-        if (lane == 0 && cta_rank == 0) {
-            // instruction descriptor: D=f32, A=B=bf16, both K-major, N, M = 128 (one CTA) or 256 (CTA pair)
-            constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BLOCK_N >> 3) << 17) |
-                                       ((uint32_t)((128 * CG) >> 4) << 24);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            long long w_full = 0, w_tempty = 0;
-            const long long t_begin = p.dbg ? clock64() : 0;
-            if (HALO) {
-                mbar_wait(bres_bar, 0);
-                tc_fence_after();
-            }
-            for (int tile = blockIdx.x / CG; tile < p.total_tiles; tile += gridDim.x / CG) {
-                w_tempty += mbar_wait_timed(&tempty_bar[acc], acc_phase ^ 1u, p.dbg != nullptr);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BLOCK_N);
-                if (HALO) {
-                    constexpr uint64_t A_STEP = (uint64_t)(Cfg::A_BYTES >> 4), B_STEP = (uint64_t)(Cfg::B_BYTES >> 4);
-                    for (int kx = 0; kx < 3; kx++) {
-                        w_full += mbar_wait_timed(&full_bar[kx], phase, p.dbg != nullptr);
-                        if (tl && tile == 0 && kx == 0) p.dbg_tl[2] = clock64();
-                        tc_fence_after();
-                        for (int ky = 0; ky < 3; ky++) {
-                            // strip kx from tile row ky on: 128 consecutive 128-byte rows, 1024-aligned
-                            const uint64_t a0 = umma_desc_sw128(ring + (uint32_t)(kx * Cfg::STAGE_BYTES + ky * 1024));
-                            const uint64_t b0 = umma_desc_sw128(bres + (uint32_t)((ky * 3 + kx) * Cfg::TA * Cfg::B_BYTES));
-#pragma unroll
-                            for (int k = 0; k < 4; k++) {
-                                const uint64_t ka = a0 + (uint64_t)(k * 2), kbd = b0 + (uint64_t)(k * 2);
-                                if (CG == 1) {
-                                    tc_mma_bf16(tmem_d, ka, kbd, idesc, (kx | ky | k) != 0);
-                                    tc_mma_bf16(tmem_d, ka + A_STEP, kbd, idesc, 1u);
-                                    tc_mma_bf16(tmem_d, ka, kbd + B_STEP, idesc, 1u);
-                                } else {
-                                    tc_mma_bf16_cg2(tmem_d, ka, kbd, idesc, (kx | ky | k) != 0);
-                                    tc_mma_bf16_cg2(tmem_d, ka + A_STEP, kbd, idesc, 1u);
-                                    tc_mma_bf16_cg2(tmem_d, ka, kbd + B_STEP, idesc, 1u);
-                                }
-                            }
-                        }
-                        if (CG == 1) tc_commit(&empty_bar[kx]); else tc_commit_cg2(&empty_bar[kx]);  // strip kx is free
-                    }
-                    phase ^= 1u;
-                }
-                for (int kb = 0; !HALO && kb < num_kb; kb++) {
-                    w_full += mbar_wait_timed(&full_bar[stage], phase, p.dbg != nullptr);
-                    if (tl && tile == 0 && kb == 0) p.dbg_tl[2] = clock64();
-                    tc_fence_after();
-                    const uint32_t sbase = ring + stage * Cfg::STAGE_BYTES;
-                    const uint64_t a0 = umma_desc_sw128(sbase);
-                    const uint64_t b0 = umma_desc_sw128(sbase + Cfg::TA * Cfg::A_BYTES);
-                    constexpr uint64_t A_STEP = (uint64_t)(Cfg::A_BYTES >> 4), B_STEP = (uint64_t)(Cfg::B_BYTES >> 4);
-#pragma unroll
-                    for (int k = 0; k < 4; k++) {  // 4 x UMMA_K(16) per 64-channel k-block; +32 B per step
-                        const uint64_t ka = a0 + (uint64_t)(k * 2), kbd = b0 + (uint64_t)(k * 2);
-                        if (CG == 1) {
-                            tc_mma_bf16(tmem_d, ka, kbd, idesc, (kb | k) != 0);  // a_hi * b_hi
-                            if (NTERMS == 3) {
-                                tc_mma_bf16(tmem_d, ka + A_STEP, kbd, idesc, 1u);  // a_lo * b_hi
-                                tc_mma_bf16(tmem_d, ka, kbd + B_STEP, idesc, 1u);  // a_hi * b_lo
-                            }
-                        } else {
-                            tc_mma_bf16_cg2(tmem_d, ka, kbd, idesc, (kb | k) != 0);
-                            if (NTERMS == 3) {
-                                tc_mma_bf16_cg2(tmem_d, ka + A_STEP, kbd, idesc, 1u);
-                                tc_mma_bf16_cg2(tmem_d, ka, kbd + B_STEP, idesc, 1u);
-                            }
-                        }
-                    }
-                    // frees the smem slot (in both CTAs of a pair) once these MMAs have read it
-                    if (CG == 1) tc_commit(&empty_bar[stage]); else tc_commit_cg2(&empty_bar[stage]);
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                if (CG == 1) tc_commit(&tfull_bar[acc]); else tc_commit_cg2(&tfull_bar[acc]);  // accumulator complete
-                if (++acc == 2) {
-                    acc = 0;
-                    acc_phase ^= 1u;
-                }
-            }
-            if (tl) p.dbg_tl[3] = clock64();
-            if (p.dbg) {
-                atomicAdd((unsigned long long*)&p.dbg[1], (unsigned long long)w_full);
-                atomicAdd((unsigned long long*)&p.dbg[2], (unsigned long long)w_tempty);
-                atomicAdd((unsigned long long*)&p.dbg[7], (unsigned long long)(clock64() - t_begin));
-                atomicAdd((unsigned long long*)&p.dbg[8], 1ull);
-            }
-        }
-    } else if (warp == 3) {
-        // ============================ residual TMA producer ===================
+        // ============================ epilogue-input TMA producer =============
+        // One FIFO of RES_BUFS slots, consumed by both consumer warpgroups in the same order
         if (lane == 0 && n_extra > 0) {
-            // Each epilogue group owns its own slice of the ring (slots [g*SPG, (g+1)*SPG)), so every slot is
-            // always consumed by the same 128 threads in FIFO order - a waiter can never be more than one
-            // mbarrier phase ahead of the fill it is waiting for.
-            int cnt[2] = {0, 0};  // fills issued so far per group
-            const int one = p.one_group;
-            for (int tile = blockIdx.x / CG; tile < p.total_tiles; tile += gridDim.x / CG) {
+            int cnt = 0;  // fills issued so far
+            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
                 const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-                const int nt = te % p.n_tiles, mt = (te / p.n_tiles) * CG + (int)cta_rank;
+                const int nt = te % p.n_tiles, mt = te / p.n_tiles;
                 const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
                 const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
                 for (int c = 0; c < Cfg::CHUNKS; c++) {
-                    const int g = one ? 0 : (c & 1);
                     for (int e = 0; e < n_extra; e++) {
-                        const int m = cnt[g]++;
-                        const int slot = g * Cfg::SPG + (m % Cfg::SPG);
-                        mbar_wait(&rempty_bar[slot], ((uint32_t)(m / Cfg::SPG) & 1u) ^ 1u);
+                        const int m = cnt++;
+                        const int slot = m % Cfg::RES_DIV;
+                        mbar_wait(&rempty_bar[slot], ((uint32_t)(m / Cfg::RES_DIV) & 1u) ^ 1u);
                         int cx = tx << p.tw_log2, cy = ty * p.th;
                         uint32_t bytes = Cfg::SLOT_BYTES;
                         if (UP && e == 0) {  // low-resolution patch under this tile
@@ -617,228 +350,211 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
             }
         }
     } else if (warp >= 4) {
-        // ============================ epilogue ================================
-        const int q = warp & 3;          // TMEM lane quarter this warp may access
-        const int g = (warp - 4) >> 2;   // epilogue group: chunks c = g, g+2, ...
-        const int row = q * 32 + lane;
-        const bool leader = (threadIdx.x == 128 + g * 128);
-        const uint32_t ob = out_stage + g * Cfg::SLOT_BYTES;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int rcnt = 0;
-        long long w_tfull = 0, w_stage = 0, w_ring = 0;
-        for (int tile = blockIdx.x / CG; tile < p.total_tiles; tile += gridDim.x / CG) {
+        // ============================ consumers: wgmma + epilogue =============
+        const int ct = threadIdx.x - 128;
+        const int wg = ct >> 7;                   // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+        const int q4 = lane & 3;                  // column pair 2 q4 of every 8-column group
+        const int row0 = wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);  // rows row0 and row0 + 8
+        const bool leader = (ct == 0);
+        int stage = 0;
+        uint32_t phase = 0;
+        int rcnt = 0, ocnt = 0;
+        long long w_full = 0, w_stage = 0, w_ring = 0;
+        const long long t_begin = (p.dbg && leader) ? clock64() : 0;
+        float acc[BLOCK_N / 2];
+        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
             const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-            const int nt = te % p.n_tiles, mt = (te / p.n_tiles) * CG + (int)cta_rank;
+            const int nt = te % p.n_tiles, mt = te / p.n_tiles;
             const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-            const int py = ty * p.th + (row >> p.tw_log2);
-            const int px = (tx << p.tw_log2) + (row & (tw - 1));
-            const bool valid = (py < p.Hout) && (px < p.Wout) && (img < p.Nimg);
-            const long long pix = ((long long)img * p.Hout + py) * p.Wout + px;
             const int n0 = nt * BLOCK_N;
 
-            w_tfull += mbar_wait_timed(&tfull_bar[acc], acc_phase, p.dbg != nullptr && leader);
-            const bool tl_last = tl && leader && g == 0 && tile + (int)gridDim.x / CG >= p.total_tiles;
-            if (tl_last) p.dbg_tl[4] = clock64();
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + (uint32_t)(acc * BLOCK_N) + ((uint32_t)(q * 32) << 16);
-            // this group's chunks of the tile: c_first, c_first + c_step, ...
-            const int c_first = p.one_group ? (g == 0 ? 0 : Cfg::CHUNKS) : g;
-            const int c_step = p.one_group ? 1 : 2;
-            // The TMEM buffer goes back to the MMA issuer as soon as this thread holds its last accumulators in registers
-            // (not after the tile's last store): the next-but-one tile's main loop starts up to a chunk time earlier.
-            auto release_acc = [&]() {
-                tc_fence_before();
-                if (CG == 1 || cta_rank == 0) mbar_arrive(&tempty_bar[acc]);
-                else mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[acc]), 0u));  // the pair leader's barrier
-            };
-            uint32_t acc_r[32];
-            if (c_first < Cfg::CHUNKS) tmem_ld32(taddr + (uint32_t)(c_first * 32), acc_r);
-            else release_acc();
-#pragma unroll 1
-            for (int c = c_first; c < Cfg::CHUNKS; c += c_step) {
-                const int c0 = c * 32;
-                // bias of these 32 columns (every lane reads the same address: L1 broadcasts), requested before the waits
-                float4 bia[8];
-                if (!UP) {  // (the interpolating variant has no registers to spare for an early request)
+            // ---- main loop: one commit group per k-block, the previous k-block's stage is freed once it has retired
+            int prev_stage = -1;
+            for (int kb = 0; kb < num_kb; kb++) {
+                w_full += mbar_wait_timed(&full_bar[stage], phase, p.dbg != nullptr && leader);
+                if (tl && leader && tile == (int)blockIdx.x && kb == 0) p.dbg_tl[2] = clock64();
+                const uint32_t sbase = ring + stage * Cfg::STAGE_BYTES;
+                const uint64_t a0 = wgmma_desc_sw128(sbase + (uint32_t)(wg * 64 * 128));
+                const uint64_t b0 = wgmma_desc_sw128(sbase + Cfg::TA * Cfg::A_BYTES);
+                constexpr uint64_t A_STEP = (uint64_t)(Cfg::A_BYTES >> 4), B_STEP = (uint64_t)(Cfg::B_BYTES >> 4);
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 8; j++) bia[j] = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0) + j);
+                for (int k = 0; k < 4; k++) {  // 4 x k16 per 64-channel k-block; +32 B per step
+                    const uint64_t ka = a0 + (uint64_t)(k * 2), kbd = b0 + (uint64_t)(k * 2);
+                    wgmma_tile<BLOCK_N>(acc, ka, kbd, (kb | k) != 0);  // a_hi * b_hi
+                    if (NTERMS == 3) {
+                        wgmma_tile<BLOCK_N>(acc, ka + A_STEP, kbd, 1u);  // a_lo * b_hi
+                        wgmma_tile<BLOCK_N>(acc, ka, kbd + B_STEP, 1u);  // a_hi * b_lo
+                    }
                 }
-                // epilogue inputs arrive through the residual ring in the order [residual][post1][post2]
-                auto ring_release = [&](int rslot) {
-                    // The slot is refilled by TMA (async proxy) while these were generic-proxy reads: without a proxy
-                    // fence the refill is not ordered after loads that are still in flight, and under memory pressure it
-                    // did overtake them (one 16-byte unit of a row came back holding the NEXT chunk's residual).
-                    fence_proxy_async();
-                    mbar_arrive(&rempty_bar[rslot]);
-                };
-                auto ring_fetch = [&](uint4(&hh)[4], uint4(&ll)[4]) {
-                    const int m = rcnt++;  // this group's FIFO position (mirrors the producer's cnt[g])
-                    const int rslot = g * Cfg::SPG + (m % Cfg::SPG);
-                    w_ring += mbar_wait_timed(&rfull_bar[rslot], (uint32_t)(m / Cfg::SPG) & 1u, p.dbg != nullptr && leader);
-                    const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                prev_stage = stage;
+                if (++stage == STAGES) {
+                    stage = 0;
+                    phase ^= 1u;
+                }
+            }
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            if (tl && leader && tile + (int)gridDim.x >= p.total_tiles) p.dbg_tl[3] = clock64();
+
+            // ---- epilogue: this thread's two rows, 32 columns (16 values) per chunk
+            int py[2], px[2];
+            bool valid[2];
+            long long pix[2];
 #pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        hh[j] = lds_v4(rb + sw64_off(row, j));
-                        ll[j] = (NTERMS == 3) ? lds_v4(rb + Cfg::CHUNK_BYTES + sw64_off(row, j)) : make_uint4(0, 0, 0, 0);
+            for (int i = 0; i < 2; i++) {
+                const int row = row0 + 8 * i;
+                py[i] = ty * p.th + (row >> p.tw_log2);
+                px[i] = (tx << p.tw_log2) + (row & (tw - 1));
+                valid[i] = (py[i] < p.Hout) && (px[i] < p.Wout) && (img < p.Nimg);
+                pix[i] = ((long long)img * p.Hout + py[i]) * p.Wout + px[i];
+            }
+            // epilogue inputs arrive through the ring in the order [residual][post1][post2]; the slot is handed back
+            // right after its values are in registers
+            auto ring_wait = [&]() -> uint32_t {
+                const int m = rcnt++;
+                const int rslot = m % Cfg::RES_DIV;
+                w_ring += mbar_wait_timed(&rfull_bar[rslot], (uint32_t)(m / Cfg::RES_DIV) & 1u, p.dbg != nullptr && leader);
+                return (uint32_t)rslot;
+            };
+            auto ring_release = [&](uint32_t rslot) {
+                // The slot is refilled by TMA (async proxy) while these were generic-proxy reads: without a proxy
+                // fence the refill is not ordered after loads that are still in flight.
+                fence_proxy_async();
+                mbar_arrive(&rempty_bar[rslot]);
+            };
+            // vv += hi + lo (the fp32 value the two planes carry) of the next ring slot
+            auto ring_add = [&](float(&vv)[2][8]) {
+                const uint32_t rslot = ring_wait();
+                const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
+                float2 rv[2][4];
+#pragma unroll
+                for (int i = 0; i < 2; i++)
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++) {
+                        const uint32_t o = sw64_off(row0 + 8 * i, jj) + 4 * q4;
+                        rv[i][jj] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
                     }
-                    // released right away: handing the slot back only after the values are consumed (when the fence has
-                    // nothing left to wait for) measured 1.5 % slower - the refill's head start matters more
-                    ring_release(rslot);
-                };
-                // vv += hi + lo (the fp32 value the two planes carry), two elements per packed add
-                auto add_planes = [&](float(&vv)[32], const uint4(&hh)[4], const uint4(&ll)[4]) {
+                ring_release(rslot);
 #pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        const uint32_t h[4] = {hh[j].x, hh[j].y, hh[j].z, hh[j].w};
-                        const uint32_t l[4] = {ll[j].x, ll[j].y, ll[j].z, ll[j].w};
+                for (int i = 0; i < 2; i++)
 #pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            const float r0 = add_bf16lo(l[e], bf16lo_to_f(h[e]));
-                            const float r1 = add_bf16hi(l[e], bf16hi_to_f(h[e]));
-                            fadd2(vv[8 * j + 2 * e], vv[8 * j + 2 * e + 1], r0, r1);
-                        }
+                    for (int jj = 0; jj < 4; jj++) {
+                        vv[i][2 * jj] += rv[i][jj].x;
+                        vv[i][2 * jj + 1] += rv[i][jj].y;
                     }
-                };
-                uint4 rh[4], rl[4];
-                float upv[32];
-                if (RING == 1 && p.has_res) ring_fetch(rh, rl);
+            };
+#pragma unroll
+            for (int c = 0; c < Cfg::CHUNKS; c++) {
+                const int c0 = c * 32;
+                float v[2][8];  // [row][8 jj + 2 q4 + e as 2 jj + e]
+#pragma unroll
+                for (int jj = 0; jj < 4; jj++) {
+                    const float2 bia = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c0 + 8 * jj + 2 * q4));
+                    const int j = 4 * c + jj;  // 8-column group of the accumulator fragment
+                    v[0][2 * jj] = acc[4 * j + 0] + bia.x;
+                    v[0][2 * jj + 1] = acc[4 * j + 1] + bia.y;
+                    v[1][2 * jj] = acc[4 * j + 2] + bia.x;
+                    v[1][2 * jj + 1] = acc[4 * j + 3] + bia.y;
+                }
+                if (RING == 1 && p.has_res) ring_add(v);
                 if (UP) {
                     // bilinear x2 of the low-resolution patch in the ring slot (weights as ATen computes them)
-                    const int m = rcnt++;
-                    const int rslot = g * Cfg::SPG + (m % Cfg::SPG);
-                    mbar_wait(&rfull_bar[rslot], (uint32_t)(m / Cfg::SPG) & 1u);
+                    const uint32_t rslot = ring_wait();
                     const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
-                    const int pyc = min(py, p.Hout - 1), pxc = min(px, p.Wout - 1);  // clipped rows are never stored
-                    const float sy = up_scale(p.up_Hi, p.Hout) * (float)pyc, sx = up_scale(p.up_Wi, p.Wout) * (float)pxc;
-                    const int y0i = (int)sy, x0i = (int)sx;
-                    const int y1i = y0i + (y0i < p.up_Hi - 1 ? 1 : 0), x1i = x0i + (x0i < p.up_Wi - 1 ? 1 : 0);
-                    const float hy1 = sy - (float)y0i, hy0 = 1.f - hy1, wx1 = sx - (float)x0i, wx0 = 1.f - wx1;
                     const int oy0 = up_src_index(ty * p.th, p.up_Hi, p.Hout), ox0 = up_src_index(tx << p.tw_log2, p.up_Wi, p.Wout);
-                    const int r00 = (y0i - oy0) * p.up_pw + (x0i - ox0), r01 = (y0i - oy0) * p.up_pw + (x1i - ox0);
-                    const int r10 = (y1i - oy0) * p.up_pw + (x0i - ox0), r11 = (y1i - oy0) * p.up_pw + (x1i - ox0);
+                    float upv[2][8];
 #pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        float q[4][8];
-                        const int rr[4] = {r00, r01, r10, r11};
+                    for (int i = 0; i < 2; i++) {
+                        const int pyc = min(py[i], p.Hout - 1), pxc = min(px[i], p.Wout - 1);  // clipped rows are never stored
+                        const float sy = up_scale(p.up_Hi, p.Hout) * (float)pyc, sx = up_scale(p.up_Wi, p.Wout) * (float)pxc;
+                        const int y0i = (int)sy, x0i = (int)sx;
+                        const int y1i = y0i + (y0i < p.up_Hi - 1 ? 1 : 0), x1i = x0i + (x0i < p.up_Wi - 1 ? 1 : 0);
+                        const float hy1 = sy - (float)y0i, hy0 = 1.f - hy1, wx1 = sx - (float)x0i, wx0 = 1.f - wx1;
+                        const int rr[4] = {(y0i - oy0) * p.up_pw + (x0i - ox0), (y0i - oy0) * p.up_pw + (x1i - ox0),
+                                           (y1i - oy0) * p.up_pw + (x0i - ox0), (y1i - oy0) * p.up_pw + (x1i - ox0)};
 #pragma unroll
-                        for (int k = 0; k < 4; k++) {
-                            const uint4 hh = lds_v4(rb + sw64_off(rr[k], j));
-                            const uint4 ll = (NTERMS == 3) ? lds_v4(rb + Cfg::CHUNK_BYTES + sw64_off(rr[k], j)) : make_uint4(0, 0, 0, 0);
-                            const uint32_t h[4] = {hh.x, hh.y, hh.z, hh.w}, l[4] = {ll.x, ll.y, ll.z, ll.w};
+                        for (int jj = 0; jj < 4; jj++) {
+                            float2 q[4];
 #pragma unroll
-                            for (int e = 0; e < 4; e++) {
-                                q[k][2 * e] = add_bf16lo(l[e], bf16lo_to_f(h[e]));
-                                q[k][2 * e + 1] = add_bf16hi(l[e], bf16hi_to_f(h[e]));
+                            for (int k = 0; k < 4; k++) {
+                                const uint32_t o = sw64_off(rr[k], jj) + 4 * q4;
+                                q[k] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
                             }
+                            upv[i][2 * jj] = hy0 * (wx0 * q[0].x + wx1 * q[1].x) + hy1 * (wx0 * q[2].x + wx1 * q[3].x);
+                            upv[i][2 * jj + 1] = hy0 * (wx0 * q[0].y + wx1 * q[1].y) + hy1 * (wx0 * q[2].y + wx1 * q[3].y);
                         }
-#pragma unroll
-                        for (int e = 0; e < 8; e++)
-                            upv[8 * j + e] = hy0 * (wx0 * q[0][e] + wx1 * q[1][e]) + hy1 * (wx0 * q[2][e] + wx1 * q[3][e]);
                     }
-                    fence_proxy_async();  // generic reads of the slot before its async-proxy (TMA) refill, as above
-                    mbar_arrive(&rempty_bar[rslot]);
-                }
-                tmem_ld_wait();
-                if (UP) {
+                    ring_release(rslot);
 #pragma unroll
-                    for (int j = 0; j < 8; j++) bia[j] = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0) + j);
-                }
-                float v[32];
+                    for (int i = 0; i < 2; i++)
 #pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    v[4 * j + 0] = __uint_as_float(acc_r[4 * j + 0]);
-                    v[4 * j + 1] = __uint_as_float(acc_r[4 * j + 1]);
-                    v[4 * j + 2] = __uint_as_float(acc_r[4 * j + 2]);
-                    v[4 * j + 3] = __uint_as_float(acc_r[4 * j + 3]);
-                    fadd2(v[4 * j + 0], v[4 * j + 1], bia[j].x, bia[j].y);
-                    fadd2(v[4 * j + 2], v[4 * j + 3], bia[j].z, bia[j].w);
-                }
-                // the accumulators of this chunk are in registers: request the next chunk's (they arrive while this one is
-                // converted and stored), or hand the TMEM buffer back after the tile's last chunk
-                if (c + c_step < Cfg::CHUNKS) tmem_ld32(taddr + (uint32_t)((c + c_step) * 32), acc_r);
-                else release_acc();
-                if (RING == 1 && p.has_res) add_planes(v, rh, rl);
-                if (UP) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) fadd2(v[j], v[j + 1], upv[j], upv[j + 1]);
+                        for (int e = 0; e < 8; e++) v[i][e] += upv[i][e];
                 }
                 if (p.relu) {
 #pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j], 0.f);
+                    for (int i = 0; i < 2; i++)
+#pragma unroll
+                        for (int e = 0; e < 8; e++) v[i][e] = fmaxf(v[i][e], 0.f);
                 }
-                for (int e = 0; RING == 1 && e < p.n_post; e++) {  // (relu(..) + skip1) + skip2, left to right
-                    ring_fetch(rh, rl);
-                    add_planes(v, rh, rl);
-                }
-                const long long off = pix * p.Cout + n0 + c0;
+                for (int e = 0; RING == 1 && e < p.n_post; e++) ring_add(v);  // (relu(..) + skip1) + skip2, left to right
                 if (tma_out) {
-                    // this group's staging slot must have been drained by its previous TMA store
+                    // staging slot ocnt & 1 was last read by the store issued two chunks ago
+                    const uint32_t ob = out_stage + (uint32_t)(ocnt & 1) * Cfg::SLOT_BYTES;
+                    ocnt++;
                     if (leader) {
                         const long long t0 = p.dbg ? clock64() : 0;
-                        bulk_wait_read<0>();
+                        bulk_wait_read<1>();
                         if (p.dbg) w_stage += clock64() - t0;
                     }
-                    epi_bar_sync(1 + g);
+                    epi_bar_sync();
 #pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        uint32_t hw_[4], lw_[4];
+                    for (int i = 0; i < 2; i++)
 #pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            const float a = v[8 * j + 2 * e], b = v[8 * j + 2 * e + 1];
-                            const uint32_t hw = cvt_bf16x2(a, b);  // hi = bf16(v), two per instruction
-                            hw_[e] = hw;
-                            lw_[e] = cvt_bf16x2(sub_bf16lo(a, hw), sub_bf16hi(b, hw));  // lo = bf16(v - hi)
+                        for (int jj = 0; jj < 4; jj++) {
+                            const float a = v[i][2 * jj], b = v[i][2 * jj + 1];
+                            const uint32_t hw = cvt_bf16x2(a, b);  // hi = bf16(v)
+                            const uint32_t o = sw64_off(row0 + 8 * i, jj) + 4 * q4;
+                            sts_u32(ob + o, hw);
+                            if (NTERMS == 3)  // lo = bf16(v - hi)
+                                sts_u32(ob + Cfg::CHUNK_BYTES + o, cvt_bf16x2(a - bf16lo_to_f(hw), b - bf16hi_to_f(hw)));
                         }
-                        sts_v4(ob + sw64_off(row, j), make_uint4(hw_[0], hw_[1], hw_[2], hw_[3]));
-                        if (NTERMS == 3)
-                            sts_v4(ob + Cfg::CHUNK_BYTES + sw64_off(row, j), make_uint4(lw_[0], lw_[1], lw_[2], lw_[3]));
-                    }
                     fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA store
-                    epi_bar_sync(1 + g);
+                    epi_bar_sync();
                     if (leader) {
 #pragma unroll
                         for (int t = 0; t < Cfg::TA; t++)
                             tma_store_5d(&p.tmO, ob + t * Cfg::CHUNK_BYTES, n0 + c0, tx << p.tw_log2, ty * p.th, img, t);
                         bulk_commit();
                     }
-                } else if (valid) {  // fp32 NHWC heads: small tensors, direct stores
+                } else {  // fp32 NHWC heads: small tensors, direct stores
 #pragma unroll
-                    for (int j = 0; j < 8; j++)
-                        *reinterpret_cast<float4*>(p.out_f32 + off + j * 4) =
-                            make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                    for (int i = 0; i < 2; i++) {
+                        if (!valid[i]) continue;
+#pragma unroll
+                        for (int jj = 0; jj < 4; jj++)
+                            *reinterpret_cast<float2*>(p.out_f32 + pix[i] * p.Cout + n0 + c0 + 8 * jj + 2 * q4) =
+                                make_float2(v[i][2 * jj], v[i][2 * jj + 1]);
+                    }
                 }
-                if (tl_last && c / c_step < 8) p.dbg_tl[5 + c / c_step] = clock64();
-            }
-            if (++acc == 2) {
-                acc = 0;
-                acc_phase ^= 1u;
             }
         }
         if (leader && tma_out) bulk_wait_all();  // stores must be complete before the CTA retires
-        if (tl && leader && g == 0) p.dbg_tl[13] = clock64();
+        if (tl && leader) p.dbg_tl[13] = clock64();
         if (p.dbg && leader) {
-            atomicAdd((unsigned long long*)&p.dbg[3 + 2 * g], (unsigned long long)w_tfull);
-            atomicAdd((unsigned long long*)&p.dbg[4 + 2 * g], (unsigned long long)w_stage);
-            atomicAdd((unsigned long long*)&p.dbg[9 + g], (unsigned long long)w_ring);
+            atomicAdd((unsigned long long*)&p.dbg[1], (unsigned long long)w_full);
+            atomicAdd((unsigned long long*)&p.dbg[4], (unsigned long long)w_stage);
+            atomicAdd((unsigned long long*)&p.dbg[9], (unsigned long long)w_ring);
+            atomicAdd((unsigned long long*)&p.dbg[7], (unsigned long long)(clock64() - t_begin));
+            atomicAdd((unsigned long long*)&p.dbg[8], 1ull);
         }
     }
-
-    tc_fence_before();
     __syncthreads();
-    if (CG == 2) cluster_sync_all();  // the leader's MMAs read this CTA's smem: nobody leaves before both are done
-    if (tl && threadIdx.x == 64) p.dbg_tl[15] = clock64();
-    if (warp == 2) {
-        tc_fence_after();
-        if (CG == 1)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS)
-                         : "memory");
-        else
-            asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS)
-                         : "memory");
-        if (tl && lane == 0) p.dbg_tl[14] = clock64();
-    }
+    if (tl && threadIdx.x == 0) p.dbg_tl[15] = clock64();
 }
 
 }  // namespace smapb

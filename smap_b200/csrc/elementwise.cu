@@ -192,7 +192,7 @@ __global__ void s2d_kernel(const float* __restrict__ x, int N, int H, int W, __n
 cudaError_t launch_s2d(const float* x, int N, int H, int W, __nv_bfloat16* out, long long plane_stride, int terms,
                        cudaStream_t st) {
     const long long total = (long long)N * (H / 2) * (W / 2 + 3);
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     s2d_kernel<<<blocks, 256, 0, st>>>(x, N, H, W, out, plane_stride, terms);
     return cudaGetLastError();
 }
@@ -270,7 +270,7 @@ __global__ void maxpool_kernel(const __nv_bfloat16* __restrict__ in, long long i
 cudaError_t launch_maxpool(const __nv_bfloat16* in, long long in_ps, int N, int H, int W, int C, __nv_bfloat16* out,
                            long long out_ps, int terms, cudaStream_t st) {
     const long long total = (long long)N * (H / 2) * (W / 2) * (C / 8);
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     maxpool_kernel<<<blocks, 256, 0, st>>>(in, in_ps, N, H, W, C, out, out_ps, terms);
     return cudaGetLastError();
 }
@@ -327,7 +327,7 @@ cudaError_t launch_upadd_relu(const __nv_bfloat16* a, long long a_ps, const __nv
                               int H, int W, int Hi, int Wi, int C, __nv_bfloat16* out, long long out_ps, int terms,
                               cudaStream_t st) {
     const long long total = (long long)N * H * W * (C / 8);
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     upadd_relu_kernel<<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms);
     return cudaGetLastError();
 }
@@ -508,7 +508,7 @@ __global__ void merge_scale_kernel(float* __restrict__ hm, const float* __restri
 }
 cudaError_t launch_merge_scale(float* hm, const float* hm_flip, int B, int h, int w, int do_scale, cudaStream_t st) {
     const long long total = (long long)B * 43 * h * w;
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     merge_scale_kernel<<<blocks, 256, 0, st>>>(hm, hm_flip, B, h, w, do_scale);
     return cudaGetLastError();
 }

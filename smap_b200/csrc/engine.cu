@@ -95,7 +95,7 @@ struct Op {
     // conv
     ConvParams cp;
     int block_n = 0;
-    int cg = 1;  // 2: CTA-pair (cta_group::2) tiles
+    int cg = 1;  // tile-table variant (1: one CTA per tile, the only one built)
     double flops = 0;
     // generic tensors
     Act a, b, out;
@@ -126,7 +126,7 @@ struct Plan {
 
 struct smapb_handle {
     int device = 0, max_batch = 0, in_h = 0, in_w = 0, h = 0, w = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int sm_reserve = 0;  // SMs the persistent conv grids leave to concurrent kernels
     std::string err;
     int64_t launches = 0;
@@ -376,32 +376,24 @@ int make_w_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, int Ci
 // ------------------------------------------------------------------------------------------------
 // conv launch
 // ------------------------------------------------------------------------------------------------
-template <int BN, int NT, int RING, int CG, bool HALO = false>
+template <int BN, int NT, int RING>
 cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
-    using Cfg = ConvCfg<BN, NT, RING, CG, HALO>;
+    using Cfg = ConvCfg<BN, NT, RING>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, NT, RING, CG, HALO>,
+        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, NT, RING>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         configured = true;
     }
-    const int slots = sm_count / CG;  // persistent CTAs (CG = 1) or CTA pairs (CG = 2)
-    const int units = cp.total_tiles < slots ? cp.total_tiles : slots;
+    const int units = cp.total_tiles < sm_count ? cp.total_tiles : sm_count;  // persistent CTAs
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(units * CG);
+    cfg.gridDim = dim3(units);
     cfg.blockDim = dim3(384);
     cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
     cfg.stream = st;
-    cudaLaunchAttribute attr[2];
+    cudaLaunchAttribute attr[1];
     int na = 0;
-    if (CG == 2) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = 2;
-        attr[na].val.clusterDim.y = 1;
-        attr[na].val.clusterDim.z = 1;
-        na++;
-    }
     if (pdl) {
         attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[na].val.programmaticStreamSerializationAllowed = 1;
@@ -409,37 +401,20 @@ cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t s
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING, CG, HALO>, cp);
+    return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING>, cp);
 }
-template <int BN, int NT, int CG>
+template <int BN, int NT>
 cudaError_t launch_conv_inst(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
-    if (cp.up_mode) return launch_conv_inst2<BN, NT, 2, CG>(cp, sm_count, st, pdl);  // fused bilinear residual
-    return (cp.has_res + cp.n_post) ? launch_conv_inst2<BN, NT, 1, CG>(cp, sm_count, st, pdl)
-                                    : launch_conv_inst2<BN, NT, 0, CG>(cp, sm_count, st, pdl);
+    if (cp.up_mode) return launch_conv_inst2<BN, NT, 2>(cp, sm_count, st, pdl);  // fused bilinear residual
+    return (cp.has_res + cp.n_post) ? launch_conv_inst2<BN, NT, 1>(cp, sm_count, st, pdl)
+                                    : launch_conv_inst2<BN, NT, 0>(cp, sm_count, st, pdl);
 }
-cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, int sm_count, cudaStream_t st, bool pdl,
-                        int cg = 1) {
-    if (cg == 3) {  // CTA pairs over halo strips (3x3 stride 1, 64 -> 64 channels, bf16x3): see ConvCfg
-        if (nterms != 3 || block_n != 64 || cp.has_res + cp.n_post + cp.up_mode) return cudaErrorInvalidValue;
-        return launch_conv_inst2<64, 3, 0, 2, true>(cp, sm_count, st, pdl);
-    }
-    if (cg == 2) {  // CTA pairs (cta_group::2): 256 x {256,128,64} tiles, bf16x3 only
-        if (nterms != 3) return cudaErrorInvalidValue;
-        switch (block_n) {
-            case 256: return launch_conv_inst<256, 3, 2>(cp, sm_count, st, pdl);
-            case 128: return launch_conv_inst<128, 3, 2>(cp, sm_count, st, pdl);
-            case 64: return launch_conv_inst<64, 3, 2>(cp, sm_count, st, pdl);
-        }
-        return cudaErrorInvalidValue;
-    }
+cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, int sm_count, cudaStream_t st, bool pdl) {
 #define SMAPB_CASE(BN)                                                                  \
     case BN:                                                                            \
-        return nterms == 3 ? launch_conv_inst<BN, 3, 1>(cp, sm_count, st, pdl)          \
-                           : launch_conv_inst<BN, 1, 1>(cp, sm_count, st, pdl);
+        return nterms == 3 ? launch_conv_inst<BN, 3>(cp, sm_count, st, pdl)             \
+                           : launch_conv_inst<BN, 1>(cp, sm_count, st, pdl);
     switch (block_n) {
-        case 256:  // bf16x3: 2 x 96 KB operand stages + output staging fill the smem, no room for an epilogue-input ring
-            if (nterms == 1) return launch_conv_inst<256, 1, 1>(cp, sm_count, st, pdl);
-            return (cp.has_res + cp.n_post) ? cudaErrorInvalidValue : launch_conv_inst2<256, 3, 0, 1>(cp, sm_count, st, pdl);
         SMAPB_CASE(128)
         SMAPB_CASE(64)
         SMAPB_CASE(32)
@@ -447,6 +422,9 @@ cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, int sm_co
 #undef SMAPB_CASE
     return cudaErrorInvalidValue;
 }
+
+// The tile shapes the kernel is built for: one CTA per 128-row tile (tile-table variant 1) of 32, 64 or 128 columns
+bool tile_shape_ok(int bn, int cg) { return cg == 1 && (bn == 32 || bn == 64 || bn == 128); }
 
 // Fill a ConvParams for `layer` applied to `in`, producing (out | out_f32).
 int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* res, const Act* post1, const Act* post2,
@@ -462,24 +440,11 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     if (in2 && (in2->C != L.Cin2 || L.k != 1 || L.stride != 1)) return fail(h, -30, "conv " + L.name + ": bad fused pair");
     if (up && (res || post1)) return fail(h, -30, "conv " + L.name + ": up-residual excludes other epilogue inputs");
     const bool flat = (L.k == 1 && L.stride == 1 && (!in2 || L.stride2 == 1) && !up);
-    // cg = 3: the halo-strip variant of the CTA-pair kernel (conv_tc.cuh, ConvCfg): 3x3, stride 1, 64 -> 64 channels, no
-    // epilogue inputs; tiles are 8 x 16 pixels (a tile row = one swizzle atom).  SMAPB_NO_HALO=1 keeps the generic kernel.
-    const bool halo_ok = L.k == 3 && L.stride == 1 && L.pad == 1 && L.Cin == 64 && L.Cout_pad == 64 && !L.stem_s2d && !in2 && !up &&
-                         !res && !post1 && !post2 && out && !outf && h->nterms == 3 && cg_out;
-    if (!force_bn && getenv("SMAPB_FORCE_TILE")) {  // debug: "bn,cg" for every layer where it is valid
+    if (!force_bn && getenv("SMAPB_FORCE_TILE")) {  // debug: "bn[,1]" for every layer where it is valid
         int fb = 0, fc = 1;
-        if (sscanf(getenv("SMAPB_FORCE_TILE"), "%d,%d", &fb, &fc) >= 1 && fb > 0 && L.Cout_pad % fb == 0 &&
-            !(fc == 3 && !(halo_ok && fb == 64)) &&
-            !(fc == 2 && (outf || !cg_out || fb < 64)) && !(fc != 2 && fc != 3 && fb == 256 && (res || post1 || up)))
+        if (sscanf(getenv("SMAPB_FORCE_TILE"), "%d,%d", &fb, &fc) >= 1 && tile_shape_ok(fb, fc) && L.Cout_pad % fb == 0)
             force_bn = fb, force_cg = fc;
     }
-#ifdef SMAPB_TAP_KY_MAJOR  // A/B build with the pre-halo tap order: the halo variant (kx-major by construction) is left out
-    static const bool halo_on = false;
-#else
-    static const bool halo_on = getenv("SMAPB_NO_HALO") == nullptr;
-#endif
-    if (force_cg == 3 && !(halo_ok && force_bn == 64)) return fail(h, -31, "invalid forced tile");
-    const bool halo = halo_ok && (force_bn ? force_cg == 3 : halo_on);
     int tw, th, tiles_x, tiles_y, nimg;
     int rc;
     if (flat) {
@@ -498,7 +463,7 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
         double best = -1;
         tw = 16;
         const int smax = in2 ? (L.stride2 > L.stride ? L.stride2 : L.stride) : L.stride;
-        for (int c = halo ? 8 : 128; c >= (halo ? 8 : 1); c >>= 1) {
+        for (int c = 128; c >= 1; c >>= 1) {
             const int t_h = 128 / c;
             if (c * smax > 256 || t_h * smax > 256) continue;
             if (up && (c / 2 + 2) * (t_h / 2 + 2) > 128) continue;  // the low-resolution patch must fit one ring slot
@@ -514,11 +479,8 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
         nimg = N;
         cp->Hout = Ho;
         cp->Wout = Wo;
-        if (halo)  // one column-shifted strip of (th + 2) x tw pixels per load
-            rc = make_act_map(h, &cp->tmA, in.ptr, in.C, in.W, in.H, N, h->planes, in.plane(), tw, th + 2, 1);
-        else
-            rc = make_act_map(h, &cp->tmA, in.ptr, in.C, in.W, in.H, N, h->planes, in.plane(), tw * L.stride,
-                              th * L.stride, L.stride);
+        rc = make_act_map(h, &cp->tmA, in.ptr, in.C, in.W, in.H, N, h->planes, in.plane(), tw * L.stride,
+                          th * L.stride, L.stride);
         if (!rc && in2)
             rc = make_act_map(h, &cp->tmA2, in2->ptr, in2->C, in2->W, in2->H, N, h->planes, in2->plane(),
                               tw * L.stride2, th * L.stride2, L.stride2);
@@ -532,51 +494,31 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     cp->tiles_x = tiles_x;
     cp->tiles_y = tiles_y;
     const long long m_tiles = (long long)tiles_x * tiles_y * nimg;
-    // Tile shape from a small cost model calibrated with per-role cycle counters on B200 (tools/conv_micro.py,
-    // SMAPB_ROLES=1): a k-block (64 channels, 12 MMAs) costs ~970 cycles at N=128 and ~880 at N=64 - both limited by
-    // the 128 B/clk shared-memory port, every MMA re-reads its A and B tiles - ~800 at N=32, and 1570 for a CTA pair
-    // (cta_group::2, 256 x 256: 4x the FLOPs, at the tensor-pipe rate); an epilogue chunk pair costs ~1750 cycles
-    // and overlaps the next tile's main loop.  time ~ waves x max(main loop, epilogue).
+    // Tile shape from a coarse model, the starting point of the autotuner and the choice when it is off: a tile's main
+    // loop costs about num_kb x (relative wgmma time of a 128 x c tile), every tile also pays an epilogue that does not
+    // overlap its own main loop, and time ~ waves x (main loop + epilogue).  Near-ties go to the wider tile.
     int bn = 0, cg = 1;
     {
         const int num_kb = L.k * L.k * (L.Cin / 64) + L.Cin2 / 64;
-        static const int pair_mode = getenv("SMAPB_PAIR") ? atoi(getenv("SMAPB_PAIR")) : 1;  // 0 never, 2 always
         double best = 1e30;
-        const int cands[4] = {128, 64, 32, 256};
+        const int cands[3] = {128, 64, 32};
         for (int c : cands) {
             if (L.Cout_pad % c) continue;
-            const bool pair = (c == 256);
-            if (pair && !(pair_mode && cg_out && h->nterms == 3 && outf == nullptr)) continue;
-            if (c == 256 && h->nterms == 1) continue;
-            const double kb_cost = pair ? 1570.0 : c == 128 ? 970.0 : c == 64 ? 880.0 : 800.0;
+            const double kb_cost = c == 128 ? 1.0 : c == 64 ? 0.6 : 0.4;
             const int n_extra = (res || up ? 1 : 0) + (post1 ? 1 : 0) + (post2 ? 1 : 0);
-            // epilogue: ~1750 cycles per chunk pair, more when it also consumes ring operands / interpolates
-            const double chunk_cost = 1750.0 + 600.0 * n_extra + (up ? 1500.0 : 0.0);
-            const double epi = (c / 32) / 2.0 * chunk_cost + (c == 32 ? 0.5 * chunk_cost : 0.0);
-            // HBM: this CTA's share is ~23 B/clk; per tile it writes 128 x c outputs, reads the ring operands and
-            // (once per m-tile, the other n-tiles hit L2) the A tile
-            const int n_tiles_c = L.Cout_pad / c;
-            const double mem = (128.0 * c * 4.0 * (1 + n_extra) + 32768.0 * num_kb / n_tiles_c) / 23.0;
-            const long long units = (pair ? (m_tiles + 1) / 2 : m_tiles) * n_tiles_c;
-            const int slots = pair ? h->sm_count / 2 : h->sm_count;
-            const double waves = (double)((units + slots - 1) / slots);
-            double t = waves * std::max(std::max(num_kb * kb_cost, epi), mem) + epi;  // + the last tile's exposed epilogue
-            t *= (c == 64 ? 1.05 : c == 32 ? 1.10 : 1.0);                             // near-ties go to the wider tile
-            if (pair && pair_mode == 2) t = 0;
-            if (t < best - 1e-9) best = t, bn = c, cg = pair ? 2 : 1;
+            const double epi = (c / 32) * (0.5 + 0.2 * n_extra + (up ? 0.5 : 0.0));
+            const long long units = m_tiles * (L.Cout_pad / c);
+            const double waves = (double)((units + h->sm_count - 1) / h->sm_count);
+            double t = waves * (num_kb * kb_cost + epi);
+            t *= (c == 64 ? 1.05 : c == 32 ? 1.10 : 1.0);
+            if (t < best - 1e-9) best = t, bn = c;
         }
         if (!bn) return fail(h, -30, "conv " + L.name + ": no tile shape for Cout_pad " + std::to_string(L.Cout_pad));
-        if (halo) bn = 64, cg = 3;
     }
-    if (force_bn) {  // autotuner override
+    if (force_bn) {  // autotuner / tile table override
         bn = force_bn;
         cg = force_cg ? force_cg : 1;
-        // one-CTA 128 x 256 tiles in bf16x3 have room for two 96 KB operand stages only without an epilogue-input ring
-        const bool needs_ring = res || post1 || up;
-        if (L.Cout_pad % bn || (cg == 3 && !halo) ||
-            (cg == 2 && ((bn != 256 && bn != 128 && bn != 64) || h->nterms != 3 || outf || !cg_out)) ||
-            (cg == 1 && bn == 256 && h->nterms == 3 && needs_ring))
-            return fail(h, -31, "invalid forced tile");
+        if (L.Cout_pad % bn || !tile_shape_ok(bn, cg)) return fail(h, -31, "invalid forced tile");
     }
     if (cg_out) *cg_out = cg;
     cp->Cout = L.Cout_pad;
@@ -589,8 +531,7 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     cp->kchunks2 = L.Cin2 / 64;
     cp->stride2 = L.stride2;
     cp->n_tiles = L.Cout_pad / bn;
-    const int cs = cg >= 2 ? 2 : 1;  // CTAs per work unit (cluster size)
-    cp->total_tiles = (int)((cs == 2 ? (m_tiles + 1) / 2 : m_tiles) * cp->n_tiles);  // work units (tiles or pair tiles)
+    cp->total_tiles = (int)(m_tiles * cp->n_tiles);
     cp->bias = L.bias_dev;
     cp->has_res = (res || up) ? 1 : 0;
     cp->n_post = (post1 ? 1 : 0) + (post2 ? 1 : 0);
@@ -611,17 +552,7 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     cp->out_f32 = outf ? outf->ptr : nullptr;
     cp->plane_stride = (long long)N * Ho * Wo * L.Cout_pad;
     cp->relu = relu;
-    {
-        const char* og = getenv("SMAPB_DEBUG_ONEGROUP");  // debug: any of 'f' (fp32-out), 'p' (post adds), 'r' (residual), 'o' (others)
-        cp->one_group = 0;
-        if (og) {
-            const bool is_f = outf != nullptr, is_p = post1 != nullptr, is_r = res != nullptr && !is_p;
-            if ((is_f && strchr(og, 'f')) || (is_p && strchr(og, 'p')) || (is_r && strchr(og, 'r')) ||
-                (!is_f && !is_p && !is_r && strchr(og, 'o')))
-                cp->one_group = 1;
-        }
-    }
-    rc = make_w_map(h, &cp->tmB, L.w_dev, L.Cin + L.Cin2, L.Cout_pad, L.k * L.k, h->planes, bn / cs);
+    rc = make_w_map(h, &cp->tmB, L.w_dev, L.Cin + L.Cin2, L.Cout_pad, L.k * L.k, h->planes, bn);
     if (rc) return rc;
     // epilogue tiles: 32 channels x (tw x th) pixels of the output / residual planes
     int n_in = up ? 1 : 0;
@@ -844,7 +775,9 @@ struct PlanBuilder {
         {
             std::lock_guard<std::mutex> lk(g_tiles_mu);
             auto it = g_tiles.find(key);
-            if (it != g_tiles.end()) best_bn = it->second.first, best_cg = it->second.second, known = true;
+            // an entry this kernel has no variant for (a table written for another GPU) is measured again
+            if (it != g_tiles.end() && tile_shape_ok(it->second.first, it->second.second))
+                best_bn = it->second.first, best_cg = it->second.second, known = true;
         }
         if (!known && !h->autotune) return 0;  // cost model (deterministic)
         if (!known) {
@@ -852,12 +785,10 @@ struct PlanBuilder {
             cudaEventCreate(&e0);
             cudaEventCreate(&e1);
             float best_ms = 1e30f;
-            const int cand[8][2] = {{128, 1}, {64, 1}, {256, 2}, {128, 2}, {64, 2}, {256, 1}, {32, 1}, {64, 3}};
+            const int cand[3][2] = {{128, 1}, {64, 1}, {32, 1}};
             for (auto& c : cand) {
                 if (L.Cout_pad % c[0]) continue;
-                if (c[1] >= 2 && h->nterms != 3) continue;
                 if (c[0] == 32 && L.Cout_pad > 64) continue;
-                if (c[0] == 256 && c[1] == 1 && getenv("SMAPB_NO_BN256")) continue;  // A/B switch for the 128 x 256 one-CTA tiles
                 Op trial;
                 int rc2 = setup_conv(h, L, in, res, p1, p2, out, nullptr, relu, &trial.cp, &trial.block_n, &trial.flops, in2,
                                      up, &trial.cg, c[0], c[1]);
@@ -865,7 +796,7 @@ struct PlanBuilder {
                 float ms_best_c = 1e30f;
                 for (int rep = 0; rep < 4; rep++) {
                     cudaEventRecord(e0, nullptr);
-                    if (launch_conv(trial.cp, trial.block_n, h->nterms, h->sm_count, nullptr, false, trial.cg) != cudaSuccess) {
+                    if (launch_conv(trial.cp, trial.block_n, h->nterms, h->sm_count, nullptr, false) != cudaSuccess) {
                         ms_best_c = 1e30f;
                         break;
                     }
@@ -882,8 +813,11 @@ struct PlanBuilder {
             h->err.clear();
             if (!best_bn) return 0;  // keep the model's choice
             std::lock_guard<std::mutex> lk(g_tiles_mu);
-            auto ins = g_tiles.emplace(key, std::make_pair(best_bn, best_cg));
-            best_bn = ins.first->second.first, best_cg = ins.first->second.second;  // another handle may have been first
+            auto it = g_tiles.find(key);
+            if (it == g_tiles.end() || !tile_shape_ok(it->second.first, it->second.second))
+                g_tiles[key] = std::make_pair(best_bn, best_cg);  // new, or replaces an entry this kernel cannot run
+            else
+                best_bn = it->second.first, best_cg = it->second.second;  // another handle may have been first
         }
         if (best_bn == op->block_n && best_cg == op->cg) return 0;
         return setup_conv(h, L, in, res, p1, p2, out, nullptr, relu, &op->cp, &op->block_n, &op->flops, in2, up, &op->cg,
@@ -1164,9 +1098,9 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
                 if (h->profiling && h->roles_dev && h->roles_used < ROLES_CAP) {
                     ConvParams cp = op.cp;  // same launch with the wait-cycle counters of every warp role switched on
                     cp.dbg = h->roles_dev + 16 * h->roles_used++;
-                    CK(launch_conv(cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl, op.cg));
+                    CK(launch_conv(cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl));
                 } else {
-                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl, op.cg));
+                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl));
                 }
                 if (h->profiling) {
                     char d[160];
@@ -1232,8 +1166,8 @@ int smapb_create(smapb_handle** out, int device, int max_batch, int in_h, int in
     }
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
-    if (prop.major != 10) {
-        g_create_error = "smapb_create: this library contains sm_100a code only (device is sm_" +
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_error = "smapb_create: this library contains sm_90a code only (device is sm_" +
                          std::to_string(prop.major) + std::to_string(prop.minor) + ")";
         return -3;
     }
@@ -1818,7 +1752,7 @@ static int infer_body(smapb_handle* h, Plan* plan, const float* imgs, const doub
             if (dev_alloc(h, &h->scratch_detd, MB * NL * hw)) return -10;
             if (dev_alloc(h, &h->scratch_rootd, MB * hw)) return -10;
         }
-        flip_w_kernel<<<148 * 8, 256, 0, st>>>(imgs, h->imgs_flip, (long long)B * 3 * h->in_h, h->in_w);
+        flip_w_kernel<<<132 * 8, 256, 0, st>>>(imgs, h->imgs_flip, (long long)B * 3 * h->in_h, h->in_w);
         CK(cudaGetLastError());
         prof_mark(h, PK_ELEM, st, "flip_w");
         h->launches++;
@@ -2196,7 +2130,7 @@ int smapb_set_tile_table(const char* text) {
         if (t1 == std::string::npos) continue;
         int bn = 0, cg = 1;
         if (sscanf(line.c_str() + t1 + 1, "%d\t%d", &bn, &cg) < 1 || bn <= 0) continue;
-        g_tiles[line.substr(0, t1)] = {bn, (cg == 2 || cg == 3) ? cg : 1};
+        g_tiles[line.substr(0, t1)] = {bn, cg};
         n++;
     }
     return n;
@@ -2280,7 +2214,7 @@ int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int 
             continue;
         }
         CK(cudaMemset(d, 0, 8));
-        checksum_kernel<<<148 * 4, 256>>>((const uint32_t*)ptr, words, d);
+        checksum_kernel<<<132 * 4, 256>>>((const uint32_t*)ptr, words, d);
         CK(cudaMemcpy(&sums[n], d, 8, cudaMemcpyDeviceToHost));
         if (desc) snprintf(desc + (size_t)n * desc_stride, desc_stride, "%s", buf);
         n++;
@@ -2443,9 +2377,8 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     }
     ConvParams cp;
     int bn = 0;
-    int cg = 1;
     rc = setup_conv(h, L, in, res ? &r : nullptr, post1 ? &p1 : nullptr, post2 ? &p2 : nullptr, &out, nullptr, relu,
-                    &cp, &bn, nullptr, nullptr, nullptr, &cg);
+                    &cp, &bn, nullptr);
     if (rc) {
         cleanup();
         return rc;
@@ -2465,36 +2398,31 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         CKT(cudaMalloc((void**)&tl_dev, 16 * sizeof(long long)));
         tmp.push_back(tl_dev);
     }
-    CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false, cg));  // warm-up + result
+    CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));  // warm-up + result
     if (dbg_dev) {
         long long d[16];
         CKT(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));
-        const double n = d[8] > 0 ? (double)d[8] : 1.0;  // number of MMA issuers (CTAs or pairs)
-        const double cs = cg >= 2 ? 2.0 : 1.0;
+        const double n = d[8] > 0 ? (double)d[8] : 1.0;  // number of CTAs
         fprintf(stderr,
-                "[roles] bn%d cg%d units%d kb%d | mean cycles per issuer: total %.0f | producer wait-empty %.0f | mma "
-                "wait-full %.0f wait-tempty %.0f | epi g0 wait-tfull %.0f wait-stage %.0f wait-ring %.0f | g1 wait-tfull %.0f wait-stage %.0f wait-ring %.0f\n",
-                bn, cg, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, d[7] / n, d[0] / n / cs, d[1] / n,
-                d[2] / n, d[3] / n / cs, d[4] / n / cs, d[9] / n / cs, d[5] / n / cs, d[6] / n / cs, d[10] / n / cs);
+                "[roles] bn%d units%d kb%d | mean cycles per CTA: total %.0f | producer wait-empty %.0f | consumer wait-full %.0f "
+                "wait-stage %.0f wait-ring %.0f\n",
+                bn, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, d[7] / n, d[0] / n, d[1] / n, d[4] / n, d[9] / n);
         cp.dbg = nullptr;
     }
     if (tl_dev) {  // time line of CTA 0 of one warm launch (cycles since kernel entry)
         CKT(cudaMemset(tl_dev, 0, 16 * sizeof(long long)));
         cp.dbg_tl = tl_dev;
-        CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false, cg));
+        CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));
         cp.dbg_tl = nullptr;
         long long t[16];
         CKT(cudaMemcpy(t, tl_dev, sizeof t, cudaMemcpyDeviceToHost));
-        fprintf(stderr, "[timeline] bn%d cg%d units%d kb%d | set-up %lld | first operands %lld | main loop end %lld | last acc %lld | chunk ends",
-                bn, cg, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, t[1] - t[0], t[2] - t[0], t[3] - t[0], t[4] - t[0]);
-        for (int i = 5; i < 13; i++)
-            if (t[i]) fprintf(stderr, " %lld", t[i] - t[0]);
-        fprintf(stderr, " | epilogue done %lld | all warps + pair sync %lld | TMEM released, exit %lld\n", t[13] - t[0], t[15] - t[0],
-                t[14] - t[0]);
+        fprintf(stderr, "[timeline] bn%d units%d kb%d | set-up %lld | first operands %lld | last main loop end %lld | epilogue done "
+                "%lld | exit %lld\n", bn, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, t[1] - t[0], t[2] - t[0],
+                t[3] - t[0], t[13] - t[0], t[15] - t[0]);
     }
     const int reps = ms_out ? 5 : 0;
     cudaEventRecord(e0, st);
-    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false, cg));
+    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));
     cudaEventRecord(e1, st);
     h->launches += 1 + reps;
     // de-pad + convert

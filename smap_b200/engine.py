@@ -31,13 +31,13 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-TILE_TABLE_PATH = os.environ.get("SMAPB_TILE_TABLE") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "tiles", "b200.tsv")  # SMAPB_TILE_TABLE: another table (A/B of a re-tune)
+TILE_TABLE_PATH = os.environ.get("SMAPB_TILE_TABLE") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "tiles", "h100.tsv")  # SMAPB_TILE_TABLE: another table (A/B of a re-tune)
 _tile_table_loaded = False
 
 
 def load_tile_table(path=TILE_TABLE_PATH):
     """Install the committed tile-shape table (process-wide, once): every process / rank then runs every layer with the
-    same (BLOCK_N, cta_group), which makes results independent of the handle and of the rank.  Geometries the table does
+    same tile shape (BLOCK_N, variant), which makes results independent of the handle and of the rank.  Geometries the table does
     not cover are autotuned by the library (use smap_b200.dist.sync_tile_table to share rank 0's choices)."""
     global _tile_table_loaded
     if _tile_table_loaded or os.environ.get("SMAPB_NO_TILE_TABLE"):
@@ -66,7 +66,7 @@ class Engine:
         it against other streams (pipelined use: several handles in flight, see EnginePool / bench.py)."""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise SmapB200Error("smap_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise SmapB200Error("smap_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         load_tile_table()
         self.device = torch.device("cuda", device)
         self.stream = stream
@@ -374,7 +374,7 @@ def records_to_numpy(rec):
 class EnginePool:
     """N independent handles on one GPU (each with its own workspace, plan and streams), used round-robin so that N
     batches are in flight: the tail of one batch's kernels (partial last waves) overlaps the other batch's kernels and
-    the H2D of the next batch overlaps compute.  Two handles give +6 % throughput on B200 (bench.py --engines)."""
+    the H2D of the next batch overlaps compute.  Two handles keep two batches in flight (bench.py --engines)."""
 
     def __init__(self, n=2, device=0, max_batch=8, in_h=512, in_w=832):
         self.engines = [Engine(device, max_batch, in_h, in_w) for _ in range(n)]

@@ -36,7 +36,7 @@ class RefineNet(nn.Module):
         if self.training:
             raise NotImplementedError("smap_b200.RefineNet is inference only: call .eval()")
         if not input_x.is_cuda:
-            raise RuntimeError("smap_b200.RefineNet runs on a B200 only: move the model and the input to 'cuda'")
+            raise RuntimeError("smap_b200.RefineNet runs on an H100 only: move the model and the input to 'cuda'")
         dev = input_x.device.index
         eng = self._engines.get(dev)
         if eng is None:

@@ -114,7 +114,7 @@ class SMAP(nn.Module):
         if valids is not None or labels is not None or self.training:
             raise NotImplementedError("smap_b200.SMAP implements the inference branch only (call .eval(); no labels)")
         if not imgs.is_cuda:
-            raise RuntimeError("smap_b200.SMAP runs on a B200 only: move the model and the input to 'cuda'")
+            raise RuntimeError("smap_b200.SMAP runs on an H100 only: move the model and the input to 'cuda'")
         B, _, H, W = imgs.shape
         key = (imgs.device.index, H, W)
         eng = self._engines.get(key)

@@ -127,7 +127,7 @@ def main():
         out["value"] = e2e["reference_bench_workload"]["frames_per_s"]
         out["unit"] = "frames/s"
         out["what"] = ("reference single-GPU path on the bench workload: eager PyTorch/cuDNN (TF32) backbone + unmodified dapalib per "
-                       "image + numpy lift; builder-side run of tests/ref_gpu_compare.py on a B200")
+                       "image + numpy lift; tests/ref_gpu_compare.py")
     eng.close()
     txt = json.dumps(out, indent=1)
     print(txt)

@@ -1,10 +1,13 @@
-"""GPU: association kernels (through the C ABI) bit-exact against the CPU oracle and - when
-oracle/_ref/dapalib_ref*.so is present - against the UNMODIFIED reference extension running on this GPU."""
+"""GPU: association kernels (through the C ABI) bit-exact against the CPU oracle and against what the UNMODIFIED
+reference extension returned on the same inputs (tests/golden/assoc_ref.npz, tests/golden/make_golden_assoc_ref.py)."""
+import hashlib
+import os
+
 import numpy as np
 import pytest
 import torch
 
-from oracle import assoc, build_ref
+from oracle import assoc
 from smap_b200.synth import make_scene
 
 pytestmark = pytest.mark.gpu
@@ -18,11 +21,6 @@ def eng():
     e = Engine(0, max_batch=8, in_h=512, in_w=832)
     yield e
     e.close()
-
-
-@pytest.fixture(scope="module")
-def ref_mod():
-    return build_ref.load_ref()
 
 
 def scenes(seeds, persons=15):
@@ -135,47 +133,63 @@ def test_batch_invariance(eng):
         assert torch.equal(b1[0], b8[i]) and c1[0] == c8[i]
 
 
-# ---------------- the real reference on this GPU ----------------
-def test_against_unmodified_reference_extension(eng, ref_mod):
-    if ref_mod is None:
-        pytest.skip("oracle/_ref/dapalib_ref*.so not built (needs /root/reference at build time)")
+# ---------------- the unmodified reference extension (stored results) ----------------
+def reference_sets():
+    """The (hms, root depth) batches the reference extension is compared on (tests/golden/make_golden_assoc_ref.py)."""
     sets = [scenes(range(40, 44))[:2], random_heatmaps(5, B=2)]
     ec = edge_cases()
     for name in ("plateau_border_threshold", "saturated_127_peaks", "coincident_and_near", "empty"):
         sets.append((ec[name][None], np.random.default_rng(3).uniform(0.5, 3, (1, H, W)).astype(np.float32)))
-    for hms, rd in sets:
+    return sets
+
+
+def _digest(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+@pytest.fixture(scope="module")
+def ref_gold():
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "assoc_ref.npz"))
+
+
+def test_against_unmodified_reference_extension(eng, ref_gold):
+    """Peaks, pair scores and bodies bit-identical to what the reference's dapalib.extract / connect(..., 2, True) returned
+    on the same inputs (tests/golden/assoc_ref.npz)."""
+    pairs = [0, 1, 0, 2, 0, 9, 9, 10, 10, 11, 0, 3, 3, 4, 4, 5, 2, 12, 12, 13, 13, 14, 2, 6, 6, 7, 7, 8]
+    for s, (hms, rd) in enumerate(reference_sets()):
         th = torch.from_numpy(hms).cuda()
         bodies, counts = eng.connect(th, torch.from_numpy(rd).cuda())
         peaks, scores = eng.extract(th)
         torch.cuda.synchronize()
         for b in range(hms.shape[0]):
-            pc, sc = ref_mod.extract(th[b].contiguous())
+            g = "s%d_b%d_" % (s, b)
+            shapes = ref_gold[g + "peak_shapes"]
             for j in range(15):
                 n = int(peaks[b, j, 0, 0].item())
-                assert pc[j].shape[0] == n
-                assert torch.equal(pc[j], peaks[b, j, 1:n + 1].cpu())
-            pairs = [0, 1, 0, 2, 0, 9, 9, 10, 10, 11, 0, 3, 3, 4, 4, 5, 2, 12, 12, 13, 13, 14, 2, 6, 6, 7, 7, 8]
+                assert shapes[j][0] == n
+                ours = peaks[b, j, 1:n + 1].cpu().numpy()
+                assert tuple(ours.shape) == tuple(shapes[j]) and str(ours.dtype) == str(ref_gold[g + "peak_dtype"])
+                assert _digest(ours) == ref_gold[g + "peaks"][j], "peaks of joint %d differ from the reference" % j
             for l in range(14):
-                nA, nB = pc[pairs[2 * l]].shape[0], pc[pairs[2 * l + 1]].shape[0]
-                assert torch.equal(sc[l], scores[b, l, :nA, :nB].cpu()), "pair scores differ from the reference"
-            ref_b = ref_mod.connect(th[b].contiguous(), torch.from_numpy(rd[b]), 2, True)
+                nA, nB = int(shapes[pairs[2 * l]][0]), int(shapes[pairs[2 * l + 1]][0])
+                assert tuple(ref_gold[g + "score_shapes"][l]) == (nA, nB)
+                assert _digest(scores[b, l, :nA, :nB].cpu().numpy()) == ref_gold[g + "scores"][l], \
+                    "pair scores differ from the reference"
             n = int(counts[b].item())
-            if n == 0:
-                assert ref_b.numel() == 0
-            else:
-                assert tuple(ref_b.shape) == (n, 15, 4)
-                assert torch.equal(ref_b, bodies[b, :n].cpu()), "bodies differ from the reference"
+            ours = bodies[b, :n].cpu().numpy()
+            assert tuple(ref_gold[g + "body_shape"]) == ((n, 15, 4) if n else (0,)), "person count differs from the reference"
+            if n:
+                assert str(ours.dtype) == str(ref_gold[g + "body_dtype"])
+                assert _digest(ours) == ref_gold[g + "bodies"], "bodies differ from the reference"
 
 
-def test_oracle_matches_unmodified_reference_extension(ref_mod):
+def test_oracle_matches_unmodified_reference_extension(ref_gold):
     """Pins the CPU oracle itself against the reference (SURVEY.md 8(c))."""
-    if ref_mod is None:
-        pytest.skip("oracle/_ref/dapalib_ref*.so not built")
     hms, rd, _ = scenes(range(50, 53))
     for b in range(3):
-        ref_b = ref_mod.connect(torch.from_numpy(hms[b]).cuda(), torch.from_numpy(rd[b]), 2, True)
         ob = assoc.connect(hms[b], rd[b])
-        assert np.array_equal(ref_b.numpy(), ob)
+        assert tuple(ob.shape) == tuple(ref_gold["o%d_body_shape" % b]) and str(ob.dtype) == str(ref_gold["o%d_body_dtype" % b])
+        assert _digest(ob) == ref_gold["o%d_bodies" % b]
 
 
 # ---------------- lift ----------------

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM convolution against a plain PyTorch fp32 reference of the same op
+"""GPU: the wgmma implicit-GEMM convolution against a plain PyTorch fp32 reference of the same op
 (TF32 disabled).  Tolerance for the bf16x3 (split-bf16, fp32-faithful) mode: 2e-5 of the output max."""
 import pytest
 import torch
@@ -91,12 +91,12 @@ def test_conv_residual_and_post_adds_deterministic(eng, B, H, W, Cin, Cout):
 
 _TILE_CASES = [(8, 32, 52, 256, 256, 3, 1, False), (8, 32, 52, 1024, 256, 1, 1, False), (2, 16, 26, 512, 512, 3, 2, False),
                (4, 64, 104, 128, 512, 1, 1, True), (2, 128, 208, 256, 64, 1, 1, False)]
-_TILES = ("128,1", "64,1", "256,1", "256,2", "128,2", "64,2")
+_TILES = ("128,1", "64,1", "32,1")
 
 
 @pytest.mark.parametrize("case", _TILE_CASES)
 def test_every_tile_shape_gives_the_same_bits(eng, monkeypatch, case):
-    """The tile table / autotuner may pick any of these (BLOCK_N, CTA-group) shapes: each must be correct AND all must
+    """The tile table / autotuner may pick any of these BLOCK_N shapes: each must be correct AND all must
     produce the same bits (every output element accumulates its K products in the same order whatever the tile), so that
     results do not depend on which shape a handle, a process or a rank happens to use."""
     B, H, W, Cin, Cout, k, stride, use_res = case
@@ -109,8 +109,8 @@ def test_every_tile_shape_gives_the_same_bits(eng, monkeypatch, case):
     ref = F.relu(ref + res if use_res else ref)
     first, n = None, 0
     for tile in _TILES:
-        bn, cg = (int(v) for v in tile.split(","))
-        if Cout % bn or (bn == 256 and cg == 1 and use_res):  # one-CTA 128x256 tiles have no epilogue-input ring
+        bn = int(tile.split(",")[0])
+        if Cout % bn:
             continue
         monkeypatch.setenv("SMAPB_FORCE_TILE", tile)
         y = eng.conv_test(x, w, b, res=res, stride=stride, relu=True)
@@ -122,28 +122,3 @@ def test_every_tile_shape_gives_the_same_bits(eng, monkeypatch, case):
         assert torch.equal(y, first), "tile %s differs from tile %s in %d elements" % (tile, _TILES[0], (y != first).sum().item())
         n += 1
     assert n >= 2
-
-
-@pytest.mark.parametrize("B,H,W", [(2, 128, 208), (1, 40, 40), (3, 37, 45)])
-def test_halo_strip_variant_matches_generic_tiles(eng, monkeypatch, B, H, W):
-    """3x3 stride-1 64 -> 64 layers run on the halo-strip variant of the pair kernel (tile = 8 x 16 pixels, three
-    column-shifted strips instead of nine shifted tiles, weights resident; conv_tc.cuh ConvCfg): same bits as the generic
-    tiles, also with ragged borders and an odd number of tiles (the second CTA of the last pair has no tile)."""
-    g = torch.Generator(device="cpu").manual_seed(13)
-    x = torch.randn(B, H, W, 64, generator=g).cuda()
-    w = (torch.randn(64, 64, 3, 3, generator=g) / (64 * 9) ** 0.5).cuda()
-    b = torch.randn(64, generator=g).cuda()
-    ref = F.relu(F.conv2d(x.permute(0, 3, 1, 2), w, b, padding=1).permute(0, 2, 3, 1))
-    outs = {}
-    for tile in ("64,3", "64,2", "64,1"):
-        monkeypatch.setenv("SMAPB_FORCE_TILE", tile)
-        y = eng.conv_test(x, w, b, relu=True)
-        torch.cuda.synchronize()
-        err = (y - ref).abs().max().item() / ref.abs().max().item()
-        assert err < 2e-5, "tile %s: relative error %g" % (tile, err)
-        outs[tile] = y
-    monkeypatch.delenv("SMAPB_FORCE_TILE")
-    assert torch.equal(outs["64,3"], outs["64,2"]), "%d elements differ" % (outs["64,3"] != outs["64,2"]).sum().item()
-    assert torch.equal(outs["64,2"], outs["64,1"])
-    y = eng.conv_test(x, w, b, relu=True)  # the default choice for this geometry is the halo variant
-    assert torch.equal(y, outs["64,3"])

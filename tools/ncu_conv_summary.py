@@ -1,6 +1,6 @@
 """Summarise an `ncu --csv --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum,
 sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active` capture of one step into the JSON the bench line quotes
-(profiles/rNN_conv_traffic.json).   python tools/ncu_conv_summary.py capture.csv out.json "source description" """
+(e.g. out/conv_traffic.json).   python tools/ncu_conv_summary.py capture.csv out.json "source description" """
 import csv
 import json
 import sys

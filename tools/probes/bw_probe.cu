@@ -1,7 +1,7 @@
 // Read-bandwidth ceilings on this GPU for the two access paths the association kernels use (tools only):
 //   (1) LDG.128 streaming (grid-stride float4 loads, U loads in flight per thread)
 //   (2) cp.async.bulk (UBLKCP) global -> shared, one persistent CTA per SM, double-buffered, chunk size C
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probes/bw_probe tools/probes/bw_probe.cu && tools/probes/bw_probe
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probes/bw_probe tools/probes/bw_probe.cu && tools/probes/bw_probe
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(128, 1) bulk_stream(const char* __restrict__ s
 }
 
 int main() {
-    const size_t bytes = (size_t)148 * 213 * 1024 * 48;  // ~1.5 GB
+    const size_t bytes = (size_t)132 * 213 * 1024 * 48;  // ~1.5 GB
     char* src;
     float* out;
     cudaMalloc(&src, bytes);
@@ -82,32 +82,32 @@ int main() {
     for (int rep = 0; rep < 2; rep++) {
         float ms;
         cudaEventRecord(e0);
-        ldg_stream<4><<<148 * 8, 256>>>((const float4*)src, bytes / 16, out);
+        ldg_stream<4><<<132 * 8, 256>>>((const float4*)src, bytes / 16, out);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
-        if (rep) report("LDG.128 x4 in flight, 148*8 CTAs x 256", ms, bytes);
+        if (rep) report("LDG.128 x4 in flight, 132*8 CTAs x 256", ms, bytes);
         cudaEventRecord(e0);
-        ldg_stream<8><<<148 * 8, 256>>>((const float4*)src, bytes / 16, out);
+        ldg_stream<8><<<132 * 8, 256>>>((const float4*)src, bytes / 16, out);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
-        if (rep) report("LDG.128 x8 in flight, 148*8 CTAs x 256", ms, bytes);
+        if (rep) report("LDG.128 x8 in flight, 132*8 CTAs x 256", ms, bytes);
         const uint32_t bufs[3] = {106496, 65536, 32768};
         const uint32_t chunks[4] = {2048, 8192, 16384, 32768};
         for (uint32_t bb : bufs)
             for (uint32_t ch : chunks) {
                 if (bb % ch) continue;
-                const size_t per_cta = (bytes / 148) / bb * bb;
+                const size_t per_cta = (bytes / 132) / bb * bb;
                 cudaFuncSetAttribute(bulk_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 + 2 * bb);
                 cudaEventRecord(e0);
-                bulk_stream<<<148, 128, 128 + 2 * bb>>>(src, per_cta, bb, ch, out);
+                bulk_stream<<<132, 128, 128 + 2 * bb>>>(src, per_cta, bb, ch, out);
                 cudaEventRecord(e1);
                 cudaEventSynchronize(e1);
                 cudaEventElapsedTime(&ms, e0, e1);
                 char name[96];
                 snprintf(name, sizeof name, "UBLKCP 1 CTA/SM, 2 x %u KB buffers, %u KB chunks", bb / 1024, ch / 1024);
-                if (rep) report(name, ms, per_cta * 148);
+                if (rep) report(name, ms, per_cta * 132);
             }
     }
     printf("%s\n", cudaGetErrorString(cudaGetLastError()));

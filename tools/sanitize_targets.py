@@ -19,7 +19,7 @@ g = torch.Generator().manual_seed(1)
 if which in ("all", "conv"):
     cases = [(1, 16, 24, 64, 64, 1, 1, False), (1, 16, 24, 64, 256, 1, 1, True), (2, 16, 26, 128, 128, 3, 1, False),
              (1, 16, 26, 128, 128, 3, 2, False), (2, 16, 26, 256, 64, 1, 1, False), (1, 16, 24, 256, 14, 3, 1, False),
-             (3, 20, 26, 64, 64, 3, 1, False)]  # the last one runs on the halo-strip variant when no tile is forced
+             (3, 20, 26, 64, 64, 3, 1, False)]
     for tile in (None, "256,2", "128,2", "64,2", "64,1"):
         if tile:
             os.environ["SMAPB_FORCE_TILE"] = tile

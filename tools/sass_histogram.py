@@ -1,6 +1,6 @@
-"""Opcode histogram of libsmap_b200.so (cuobjdump -sass): the SASS mnemonics that prove tcgen05 / TMEM / TMA / clusters
-(B200_PROFILING.md): UTCHMMA (tcgen05.mma), LDTM (tcgen05.ld), UTMALDG / UTMASTG (TMA tensor loads / stores), UBLKCP (1-D bulk
-copy), UTCBAR (tcgen05.commit), SYNCS (mbarrier), UCGABAR (cluster barrier).   python tools/sass_histogram.py > profiles/rNN_sass_opcodes.txt"""
+"""Opcode histogram of libsmap_b200.so (cuobjdump -sass): the SASS mnemonics that prove wgmma / TMA / mbarrier use:
+HGMMA (wgmma.mma_async), WARPGROUP (wgmma fence / arrive), UTMALDG / UTMASTG (TMA tensor loads / stores), UBLKCP (1-D bulk
+copy), SYNCS (mbarrier).   python tools/sass_histogram.py > out/sass_opcodes.txt"""
 import collections
 import os
 import re
@@ -21,9 +21,8 @@ for line in txt.splitlines():
     if m:
         total[m.group(1)] += 1
         per_kernel[cur][m.group(1).split(".")[0]] += 1
-KEYS = ("UTCHMMA", "LDTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "UTCATOMSWS", "SYNCS", "UCGABAR", "FENCE", "HMMA", "IMMA",
-        "FADD2", "FHADD", "FHFMA")  # the last three: packed fp32 / mixed bf16-fp32 arithmetic of the conv epilogue
-print("opcode histogram of smap_b200/lib/libsmap_b200.so (cuobjdump -sass, sm_100a)")
+KEYS = ("HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "FENCE", "HMMA", "IMMA")
+print("opcode histogram of smap_b200/lib/libsmap_b200.so (cuobjdump -sass, sm_90a)")
 for op, n in sorted(total.items(), key=lambda kv: -kv[1]):
     if op.startswith(KEYS):
         print("%8d  %s" % (n, op))
