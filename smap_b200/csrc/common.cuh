@@ -47,13 +47,16 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
         : "memory");
     return ok;
 }
+// Out of line: a trap inlined after setmaxnreg.inc makes ptxas hold that role to the launch-time register budget
+// (spills in the 232-register consumers of conv_tc_kernel); behind a call it does not.
+static __device__ __noinline__ void mbar_timeout() { __trap(); }
 // Bounded wait: a protocol bug traps (kernel error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
         if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-            __trap();
+            mbar_timeout();
         }
     }
 }

@@ -13,14 +13,17 @@
 // (dropped terms are O(2^-16) relative) - fp32-faithful results at 3x the bf16 MMA count.  NTERMS = 1 is the
 // plain bf16 fast mode.
 //
-// Warp roles (384 threads, persistent CTA, static tile schedule):
-//   warp 0 : operand TMA producer (one lane)        warp 1 : epilogue-input TMA producer (one lane)
-//   warpgroups 1-2 (warps 4-11) : consumers; warpgroup g owns rows [64 g, 64 g + 64) of the 128-row tile and all BLOCK_N
-//                columns: wgmma m64nBLOCK_Nk16 into registers, then the epilogue from those registers in 32-column
-//                chunks: (+bias +residual, ReLU, +skips, hi/lo split) -> swizzled smem -> one TMA store per chunk
-// Pipelines: operand full/empty ring (TMA <-> wgmma), epilogue-input full/empty ring (TMA <-> epilogue), bulk-async store
-// groups (epilogue <-> TMA store).  The producer runs ahead into the next tile's operands while the consumers run the
-// epilogue of the current one.
+// Roles (384 threads, persistent CTA, static tile schedule; every role branch is warpgroup-uniform, registers are
+// rebalanced per role with setmaxnreg):
+//   warpgroup 0 (40 registers) : warp 0 = operand TMA producer (one lane), warp 1 = epilogue-input TMA producer (one lane)
+//   warpgroups 1-2 (232 registers) : ping-pong consumers.  The CTA's tiles alternate between them: warpgroup g runs tiles
+//                g, g + 2, ... of the CTA's list, each a whole 128-row tile issued as two m64nBLOCK_Nk16 row halves into
+//                registers, then the epilogue from those registers in 32-column chunks: (+bias +residual, ReLU, +skips,
+//                hi/lo split) -> the warpgroup's swizzled staging slot -> one TMA store per chunk and plane.
+//                Main loops are handed from one warpgroup to the other in tile order (a named-barrier token), so one
+//                warpgroup's epilogue runs while the other issues the next tile's wgmma.
+// Pipelines: operand full/empty ring (TMA <-> wgmma, consumed tile by tile in the CTA's tile order), epilogue-input
+// full/empty ring (TMA <-> epilogue, one FIFO in the same tile order), bulk-async store groups (per warpgroup leader).
 // Taps of a k x k filter are visited kx-major and every tile width issues the same MMAs per output element in the same
 // order, i.e. all tile shapes produce the same bits.
 #pragma once
@@ -59,7 +62,7 @@ struct alignas(64) ConvParams {
     // the ring carries the (ph x pw)-pixel patch under each output tile and the epilogue interpolates
     // (align_corners=True) before the ReLU.  up_mode = 0: plain residual.
     int up_mode, up_Hi, up_Wi, up_pw, up_ph;
-    long long* dbg;  // optional: per-role wait-cycle counters (tools/conv_micro.py --roles), null in production
+    long long* dbg;  // optional: per-role cycle counters, layout ConvDbg below (tools/roles_plan.py), null in production
     long long* dbg_tl;  // optional: clock64 time line of CTA 0 (SMAPB_TIMELINE, smapb_conv_test only), null in production
 };
 
@@ -95,8 +98,37 @@ __device__ __forceinline__ void bulk_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// named barrier of the two consumer warpgroups
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// Named barriers (0 is __syncthreads): 1 + g = epilogue of consumer warpgroup g (128 threads).  Turns (2 x 128 threads,
+// synced by warpgroup g, arrived at by the other consumer warpgroup when it is done with its previous tile):
+// 3 + g = main-loop turn of g, 5 + g = epilogue-input ring turn of g
+enum { TURN_MAIN = 3, TURN_RING = 5 };
+__device__ __forceinline__ void epi_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+__device__ __forceinline__ void turn_wait(int turn, int wg) { asm volatile("bar.sync %0, 256;" ::"r"(turn + wg) : "memory"); }
+__device__ __forceinline__ void turn_pass(int turn, int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(turn + wg) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+// Per-role cycle counters (p.dbg != null), summed over CTAs.  Consumer warpgroup g uses CONS + CONS_N g + {...}.
+struct ConvDbg {
+    enum {
+        PRODUCER_WAIT_EMPTY = 0,  // operand producer waiting for a free stage
+        TOTAL = 1,                // CTA lifetime from set-up to exit
+        CTAS = 2,                 // number of CTAs that added to the counters
+        CONS = 3,
+        WAIT_FULL = 0,   // operands not yet landed
+        WAIT_ORDER = 1,  // waiting for the main-loop turn (the other warpgroup still issuing its tile)
+        EPILOGUE = 2,    // time in epilogues
+        WAIT_RING = 3,   // epilogue inputs not yet landed
+        WAIT_STAGE = 4,  // own staging slot still being read by the previous TMA store
+        CONS_N = 5,
+        COUNT = CONS + 2 * CONS_N
+    };
+};
 __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
     uint32_t r;
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(addr));
@@ -207,14 +239,21 @@ struct ConvCfg {
     static constexpr int CHUNKS = BLOCK_N / 32;       // epilogue granularity: 32 columns (one TMA store box)
     static constexpr int CHUNK_BYTES = 128 * 64;      // one plane of one chunk: 128 rows x 32 bf16
     static constexpr int SLOT_BYTES = TA * CHUNK_BYTES;  // hi (+ lo)
-    static constexpr int OUT_BUFS = 2;  // store staging, alternate chunks
     // RING: the layer streams epilogue inputs (residual / skip adds); without it the smem goes to operand stages
     static constexpr int RES_BUFS = RING ? 2 : 0;
     static constexpr int RES_DIV = RING ? RES_BUFS : 1;  // RES_BUFS as a divisor (no ring slots are used when RING == 0)
-    static constexpr int EPI_BYTES = (OUT_BUFS + RES_BUFS) * SLOT_BYTES;
     static constexpr int SMEM_LIMIT = 227 * 1024;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
-    static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
+    static constexpr int stages_with(int out_bufs) {
+        return (SMEM_LIMIT - 2048 - (out_bufs + RES_BUFS) * SLOT_BYTES) / STAGE_BYTES > 8
+                   ? 8
+                   : (SMEM_LIMIT - 2048 - (out_bufs + RES_BUFS) * SLOT_BYTES) / STAGE_BYTES;
+    }
+    // store staging per consumer warpgroup: two slots (chunk c + 1 is written while chunk c is stored) where that costs
+    // no operand stage, else one
+    static constexpr int OUT_PER_WG = stages_with(4) == stages_with(2) ? 2 : 1;
+    static constexpr int OUT_BUFS = 2 * OUT_PER_WG;
+    static constexpr int EPI_BYTES = (OUT_BUFS + RES_BUFS) * SLOT_BYTES;
+    static constexpr int STAGES = stages_with(OUT_BUFS);
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 2048;  // 1 KB control + 1 KB alignment slack
     static_assert(STAGES >= 2, "need at least a double buffer");
     static_assert(BLOCK_N == 32 || BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
@@ -253,11 +292,11 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; s++) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 8);  // lane 0 of each consumer warp
+            mbar_init(&empty_bar[s], 4);  // lane 0 of each warp of the consumer warpgroup that used the stage
         }
         for (int s = 0; s < Cfg::RES_BUFS; s++) {
             mbar_init(&rfull_bar[s], 1);
-            mbar_init(&rempty_bar[s], 256);
+            mbar_init(&rempty_bar[s], 128);  // the consumer warpgroup whose epilogue read the slot
         }
         fence_mbar_init();
     }
@@ -271,10 +310,13 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
     if (tl && threadIdx.x == 0) p.dbg_tl[1] = clock64();
     pdl_wait();     // inputs of this layer are produced by the previous kernel in the stream
     pdl_trigger();  // let the next kernel's CTAs be scheduled onto SMs as they drain (they block in their own wait)
+    const long long t_begin = p.dbg ? clock64() : 0;  // CTA lifetime from here: the wait for the previous kernel excluded
 
-    if (warp == 0) {
-        // ============================ operand TMA producer ====================
-        if (lane == 0) {
+    if (warp < 4) {
+        // ============================ producer warpgroup ======================
+        setmaxnreg_dec<40>();  // two single-lane TMA issuers: their registers go to the consumer warpgroups
+        if (warp == 0 && lane == 0) {
+            // ---- operand TMA producer: the CTA's tiles in order, num_kb stages each
             int stage = 0;
             uint32_t phase = 0;
             long long w_empty = 0;
@@ -316,12 +358,10 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                     }
                 }
             }
-            if (p.dbg) atomicAdd((unsigned long long*)&p.dbg[0], (unsigned long long)w_empty);
-        }
-    } else if (warp == 1) {
-        // ============================ epilogue-input TMA producer =============
-        // One FIFO of RES_BUFS slots, consumed by both consumer warpgroups in the same order
-        if (lane == 0 && n_extra > 0) {
+            if (p.dbg) atomicAdd((unsigned long long*)&p.dbg[ConvDbg::PRODUCER_WAIT_EMPTY], (unsigned long long)w_empty);
+        } else if (warp == 1 && lane == 0 && n_extra > 0) {
+            // ---- epilogue-input TMA producer: one FIFO of RES_BUFS slots, filled in the CTA's tile order; the epilogues
+            // of the two consumer warpgroups take their tiles' entries in that same order
             int cnt = 0;  // fills issued so far
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
                 const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
@@ -349,43 +389,62 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                 }
             }
         }
-    } else if (warp >= 4) {
-        // ============================ consumers: wgmma + epilogue =============
-        const int ct = threadIdx.x - 128;
-        const int wg = ct >> 7;                   // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+    } else {
+        // ============================ consumer warpgroups: wgmma + epilogue ===
+        setmaxnreg_inc<232>();  // 128 fp32 accumulators per thread at BLOCK_N = 128
+        const int wg = (warp >> 2) - 1;           // consumer warpgroup 0 / 1: tiles wg, wg + 2, ... of the CTA's list
         const int q4 = lane & 3;                  // column pair 2 q4 of every 8-column group
-        const int row0 = wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);  // rows row0 and row0 + 8
-        const bool leader = (ct == 0);
-        int stage = 0;
-        uint32_t phase = 0;
-        int rcnt = 0, ocnt = 0;
-        long long w_full = 0, w_stage = 0, w_ring = 0;
-        const long long t_begin = (p.dbg && leader) ? clock64() : 0;
-        float acc[BLOCK_N / 2];
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int rw = (warp & 3) * 16 + (lane >> 2);  // this thread's rows: 64 h + rw + 8 i (row half h, i = 0, 1)
+        const bool leader = (threadIdx.x & 127) == 0;
+        const bool timed = p.dbg != nullptr && leader;
+        const uint32_t ob0 = out_stage + (uint32_t)(wg * Cfg::OUT_PER_WG) * Cfg::SLOT_BYTES;  // this warpgroup's staging
+        const int n_cta = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles of this CTA
+        // role counters: operand waits are summed in a register over a tile's main loop (no atomics between its wgmma);
+        // epilogue waits go to global memory as they happen (registers are short there in the fused bilinear variants)
+        long long* const dc = p.dbg ? p.dbg + ConvDbg::CONS + ConvDbg::CONS_N * wg : nullptr;
+        auto tally = [&](int k, long long cycles) {
+            if (timed) atomicAdd((unsigned long long*)&dc[k], (unsigned long long)cycles);
+        };
+        float acc[2][BLOCK_N / 2];  // [row half][wgmma fragment]
+        for (int j = wg; j < n_cta; j += 2) {
+            const int tile = blockIdx.x + j * gridDim.x;
             const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
             const int nt = te % p.n_tiles, mt = te / p.n_tiles;
             const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
             const int n0 = nt * BLOCK_N;
 
-            // ---- main loop: one commit group per k-block, the previous k-block's stage is freed once it has retired
+            // ---- main loop, in turn: the operand ring holds the CTA's tiles in order, j * num_kb stages precede this one
+            const uint32_t it0 = (uint32_t)j * (uint32_t)num_kb;
+            int stage = (int)(it0 % STAGES);
+            uint32_t phase = (it0 / STAGES) & 1u;
+            if (j > 0) {
+                const long long t0 = timed ? clock64() : 0;
+                turn_wait(TURN_MAIN, wg);
+                tally(ConvDbg::WAIT_ORDER, timed ? clock64() - t0 : 0);
+            }
+            // one commit group per k-block, the previous k-block's stage is freed once it has retired
             int prev_stage = -1;
+            uint32_t w_full = 0;  // per-tile sums fit in 32 bits
             for (int kb = 0; kb < num_kb; kb++) {
-                w_full += mbar_wait_timed(&full_bar[stage], phase, p.dbg != nullptr && leader);
-                if (tl && leader && tile == (int)blockIdx.x && kb == 0) p.dbg_tl[2] = clock64();
+                w_full += (uint32_t)mbar_wait_timed(&full_bar[stage], phase, timed);
+                if (tl && leader && j == 0 && kb == 0) p.dbg_tl[2] = clock64();
                 const uint32_t sbase = ring + stage * Cfg::STAGE_BYTES;
-                const uint64_t a0 = wgmma_desc_sw128(sbase + (uint32_t)(wg * 64 * 128));
+                const uint64_t a0 = wgmma_desc_sw128(sbase);
                 const uint64_t b0 = wgmma_desc_sw128(sbase + Cfg::TA * Cfg::A_BYTES);
                 constexpr uint64_t A_STEP = (uint64_t)(Cfg::A_BYTES >> 4), B_STEP = (uint64_t)(Cfg::B_BYTES >> 4);
+                constexpr uint64_t A_HALF = (uint64_t)((64 * 128) >> 4);  // rows 64..127 of the A tile
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; k++) {  // 4 x k16 per 64-channel k-block; +32 B per step
-                    const uint64_t ka = a0 + (uint64_t)(k * 2), kbd = b0 + (uint64_t)(k * 2);
-                    wgmma_tile<BLOCK_N>(acc, ka, kbd, (kb | k) != 0);  // a_hi * b_hi
-                    if (NTERMS == 3) {
-                        wgmma_tile<BLOCK_N>(acc, ka + A_STEP, kbd, 1u);  // a_lo * b_hi
-                        wgmma_tile<BLOCK_N>(acc, ka, kbd + B_STEP, 1u);  // a_hi * b_lo
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const uint64_t ka = a0 + (uint64_t)(k * 2) + h * A_HALF, kbd = b0 + (uint64_t)(k * 2);
+                        wgmma_tile<BLOCK_N>(acc[h], ka, kbd, (kb | k) != 0);  // a_hi * b_hi
+                        if (NTERMS == 3) {
+                            wgmma_tile<BLOCK_N>(acc[h], ka + A_STEP, kbd, 1u);  // a_lo * b_hi
+                            wgmma_tile<BLOCK_N>(acc[h], ka, kbd + B_STEP, 1u);  // a_hi * b_lo
+                        }
                     }
                 }
                 wgmma_commit();
@@ -397,28 +456,37 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                     phase ^= 1u;
                 }
             }
+            if (j + 1 < n_cta) turn_pass(TURN_MAIN, wg ^ 1);  // every wgmma of this tile is issued: the other warpgroup's turn
+            tally(ConvDbg::WAIT_FULL, w_full);
             wgmma_wait<0>();
             if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-            if (tl && leader && tile + (int)gridDim.x >= p.total_tiles) p.dbg_tl[3] = clock64();
+            if (tl && leader && j == n_cta - 1) p.dbg_tl[3] = clock64();
 
-            // ---- epilogue: this thread's two rows, 32 columns (16 values) per chunk
-            int py[2], px[2];
-            bool valid[2];
-            long long pix[2];
+            // ---- epilogue: this thread's four rows (index 2 h + i), 32 columns (8 values per row) per chunk
+            const long long t_epi0 = timed ? clock64() : 0;
+            int py[4], px[4];
+            bool valid[4];
+            long long pix[4];
 #pragma unroll
-            for (int i = 0; i < 2; i++) {
-                const int row = row0 + 8 * i;
-                py[i] = ty * p.th + (row >> p.tw_log2);
-                px[i] = (tx << p.tw_log2) + (row & (tw - 1));
-                valid[i] = (py[i] < p.Hout) && (px[i] < p.Wout) && (img < p.Nimg);
-                pix[i] = ((long long)img * p.Hout + py[i]) * p.Wout + px[i];
+            for (int q = 0; q < 4; q++) {
+                const int row = 64 * (q >> 1) + rw + 8 * (q & 1);
+                py[q] = ty * p.th + (row >> p.tw_log2);
+                px[q] = (tx << p.tw_log2) + (row & (tw - 1));
+                valid[q] = (py[q] < p.Hout) && (px[q] < p.Wout) && (img < p.Nimg);
+                pix[q] = ((long long)img * p.Hout + py[q]) * p.Wout + px[q];
             }
-            // epilogue inputs arrive through the ring in the order [residual][post1][post2]; the slot is handed back
-            // right after its values are in registers
+            auto row_of = [&](int q) { return 64 * (q >> 1) + rw + 8 * (q & 1); };
+            // epilogue inputs arrive through the ring in the order [residual][post1][post2]; this tile's entries follow
+            // those of the CTA's j earlier tiles.  The warpgroups take the ring in turns, tile by tile: a parity wait is
+            // only sound while the slot's barrier is at most one phase behind, and the other warpgroup may still be reading
+            // the previous tile's entries when this one's main loop ends.
+            const bool ring_turns = RING != 0 && n_extra > 0;
+            if (ring_turns && j > 0) turn_wait(TURN_RING, wg);
+            int rcnt = j * Cfg::CHUNKS * n_extra;
             auto ring_wait = [&]() -> uint32_t {
                 const int m = rcnt++;
                 const int rslot = m % Cfg::RES_DIV;
-                w_ring += mbar_wait_timed(&rfull_bar[rslot], (uint32_t)(m / Cfg::RES_DIV) & 1u, p.dbg != nullptr && leader);
+                tally(ConvDbg::WAIT_RING, mbar_wait_timed(&rfull_bar[rslot], (uint32_t)(m / Cfg::RES_DIV) & 1u, timed));
                 return (uint32_t)rslot;
             };
             auto ring_release = [&](uint32_t rslot) {
@@ -428,38 +496,35 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                 mbar_arrive(&rempty_bar[rslot]);
             };
             // vv += hi + lo (the fp32 value the two planes carry) of the next ring slot
-            auto ring_add = [&](float(&vv)[2][8]) {
+            auto ring_add = [&](float(&vv)[4][8]) {
                 const uint32_t rslot = ring_wait();
                 const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
-                float2 rv[2][4];
 #pragma unroll
-                for (int i = 0; i < 2; i++)
+                for (int q = 0; q < 4; q++)
 #pragma unroll
                     for (int jj = 0; jj < 4; jj++) {
-                        const uint32_t o = sw64_off(row0 + 8 * i, jj) + 4 * q4;
-                        rv[i][jj] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                        const uint32_t o = sw64_off(row_of(q), jj) + 4 * q4;
+                        const float2 rv = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                        vv[q][2 * jj] += rv.x;
+                        vv[q][2 * jj + 1] += rv.y;
                     }
                 ring_release(rslot);
-#pragma unroll
-                for (int i = 0; i < 2; i++)
-#pragma unroll
-                    for (int jj = 0; jj < 4; jj++) {
-                        vv[i][2 * jj] += rv[i][jj].x;
-                        vv[i][2 * jj + 1] += rv[i][jj].y;
-                    }
             };
 #pragma unroll
             for (int c = 0; c < Cfg::CHUNKS; c++) {
                 const int c0 = c * 32;
-                float v[2][8];  // [row][8 jj + 2 q4 + e as 2 jj + e]
+                float v[4][8];  // [row 2 h + i][8 jj + 2 q4 + e as 2 jj + e]
 #pragma unroll
                 for (int jj = 0; jj < 4; jj++) {
                     const float2 bia = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c0 + 8 * jj + 2 * q4));
-                    const int j = 4 * c + jj;  // 8-column group of the accumulator fragment
-                    v[0][2 * jj] = acc[4 * j + 0] + bia.x;
-                    v[0][2 * jj + 1] = acc[4 * j + 1] + bia.y;
-                    v[1][2 * jj] = acc[4 * j + 2] + bia.x;
-                    v[1][2 * jj + 1] = acc[4 * j + 3] + bia.y;
+                    const int f = 4 * (4 * c + jj);  // 8-column group 4 c + jj of the accumulator fragment
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        v[2 * h][2 * jj] = acc[h][f + 0] + bia.x;
+                        v[2 * h][2 * jj + 1] = acc[h][f + 1] + bia.y;
+                        v[2 * h + 1][2 * jj] = acc[h][f + 2] + bia.x;
+                        v[2 * h + 1][2 * jj + 1] = acc[h][f + 3] + bia.y;
+                    }
                 }
                 if (RING == 1 && p.has_res) ring_add(v);
                 if (UP) {
@@ -467,10 +532,9 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                     const uint32_t rslot = ring_wait();
                     const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
                     const int oy0 = up_src_index(ty * p.th, p.up_Hi, p.Hout), ox0 = up_src_index(tx << p.tw_log2, p.up_Wi, p.Wout);
-                    float upv[2][8];
 #pragma unroll
-                    for (int i = 0; i < 2; i++) {
-                        const int pyc = min(py[i], p.Hout - 1), pxc = min(px[i], p.Wout - 1);  // clipped rows are never stored
+                    for (int q = 0; q < 4; q++) {
+                        const int pyc = min(py[q], p.Hout - 1), pxc = min(px[q], p.Wout - 1);  // clipped rows are never stored
                         const float sy = up_scale(p.up_Hi, p.Hout) * (float)pyc, sx = up_scale(p.up_Wi, p.Wout) * (float)pxc;
                         const int y0i = (int)sy, x0i = (int)sx;
                         const int y1i = y0i + (y0i < p.up_Hi - 1 ? 1 : 0), x1i = x0i + (x0i < p.up_Wi - 1 ? 1 : 0);
@@ -479,52 +543,47 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                                            (y1i - oy0) * p.up_pw + (x0i - ox0), (y1i - oy0) * p.up_pw + (x1i - ox0)};
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++) {
-                            float2 q[4];
+                            float2 s[4];
 #pragma unroll
                             for (int k = 0; k < 4; k++) {
                                 const uint32_t o = sw64_off(rr[k], jj) + 4 * q4;
-                                q[k] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                                s[k] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
                             }
-                            upv[i][2 * jj] = hy0 * (wx0 * q[0].x + wx1 * q[1].x) + hy1 * (wx0 * q[2].x + wx1 * q[3].x);
-                            upv[i][2 * jj + 1] = hy0 * (wx0 * q[0].y + wx1 * q[1].y) + hy1 * (wx0 * q[2].y + wx1 * q[3].y);
+                            v[q][2 * jj] += hy0 * (wx0 * s[0].x + wx1 * s[1].x) + hy1 * (wx0 * s[2].x + wx1 * s[3].x);
+                            v[q][2 * jj + 1] += hy0 * (wx0 * s[0].y + wx1 * s[1].y) + hy1 * (wx0 * s[2].y + wx1 * s[3].y);
                         }
                     }
                     ring_release(rslot);
-#pragma unroll
-                    for (int i = 0; i < 2; i++)
-#pragma unroll
-                        for (int e = 0; e < 8; e++) v[i][e] += upv[i][e];
                 }
                 if (p.relu) {
 #pragma unroll
-                    for (int i = 0; i < 2; i++)
+                    for (int q = 0; q < 4; q++)
 #pragma unroll
-                        for (int e = 0; e < 8; e++) v[i][e] = fmaxf(v[i][e], 0.f);
+                        for (int e = 0; e < 8; e++) v[q][e] = fmaxf(v[q][e], 0.f);
                 }
                 for (int e = 0; RING == 1 && e < p.n_post; e++) ring_add(v);  // (relu(..) + skip1) + skip2, left to right
                 if (tma_out) {
-                    // staging slot ocnt & 1 was last read by the store issued two chunks ago
-                    const uint32_t ob = out_stage + (uint32_t)(ocnt & 1) * Cfg::SLOT_BYTES;
-                    ocnt++;
+                    // the staging slot was last read by the store this warpgroup issued OUT_PER_WG chunks ago
+                    const uint32_t ob = ob0 + (uint32_t)((((j >> 1) * Cfg::CHUNKS + c) % Cfg::OUT_PER_WG) * Cfg::SLOT_BYTES);
                     if (leader) {
-                        const long long t0 = p.dbg ? clock64() : 0;
-                        bulk_wait_read<1>();
-                        if (p.dbg) w_stage += clock64() - t0;
+                        const long long t0 = timed ? clock64() : 0;
+                        bulk_wait_read<Cfg::OUT_PER_WG - 1>();
+                        tally(ConvDbg::WAIT_STAGE, timed ? clock64() - t0 : 0);
                     }
-                    epi_bar_sync();
+                    epi_bar_sync(wg);
 #pragma unroll
-                    for (int i = 0; i < 2; i++)
+                    for (int q = 0; q < 4; q++)
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++) {
-                            const float a = v[i][2 * jj], b = v[i][2 * jj + 1];
+                            const float a = v[q][2 * jj], b = v[q][2 * jj + 1];
                             const uint32_t hw = cvt_bf16x2(a, b);  // hi = bf16(v)
-                            const uint32_t o = sw64_off(row0 + 8 * i, jj) + 4 * q4;
+                            const uint32_t o = sw64_off(row_of(q), jj) + 4 * q4;
                             sts_u32(ob + o, hw);
                             if (NTERMS == 3)  // lo = bf16(v - hi)
                                 sts_u32(ob + Cfg::CHUNK_BYTES + o, cvt_bf16x2(a - bf16lo_to_f(hw), b - bf16hi_to_f(hw)));
                         }
                     fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA store
-                    epi_bar_sync();
+                    epi_bar_sync(wg);
                     if (leader) {
 #pragma unroll
                         for (int t = 0; t < Cfg::TA; t++)
@@ -533,28 +592,30 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                     }
                 } else {  // fp32 NHWC heads: small tensors, direct stores
 #pragma unroll
-                    for (int i = 0; i < 2; i++) {
-                        if (!valid[i]) continue;
+                    for (int q = 0; q < 4; q++) {
+                        if (!valid[q]) continue;
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++)
-                            *reinterpret_cast<float2*>(p.out_f32 + pix[i] * p.Cout + n0 + c0 + 8 * jj + 2 * q4) =
-                                make_float2(v[i][2 * jj], v[i][2 * jj + 1]);
+                            *reinterpret_cast<float2*>(p.out_f32 + pix[q] * p.Cout + n0 + c0 + 8 * jj + 2 * q4) =
+                                make_float2(v[q][2 * jj], v[q][2 * jj + 1]);
                     }
                 }
             }
+            if (ring_turns && j + 1 < n_cta) turn_pass(TURN_RING, wg ^ 1);  // this tile's ring entries are all released
+            tally(ConvDbg::EPILOGUE, timed ? clock64() - t_epi0 : 0);
         }
         if (leader && tma_out) bulk_wait_all();  // stores must be complete before the CTA retires
-        if (tl && leader) p.dbg_tl[13] = clock64();
-        if (p.dbg && leader) {
-            atomicAdd((unsigned long long*)&p.dbg[1], (unsigned long long)w_full);
-            atomicAdd((unsigned long long*)&p.dbg[4], (unsigned long long)w_stage);
-            atomicAdd((unsigned long long*)&p.dbg[9], (unsigned long long)w_ring);
-            atomicAdd((unsigned long long*)&p.dbg[7], (unsigned long long)(clock64() - t_begin));
-            atomicAdd((unsigned long long*)&p.dbg[8], 1ull);
+        // the warpgroup that runs the CTA's last tile finishes last: it closes the CTA's lifetime
+        if (leader && wg == ((n_cta - 1) & 1)) {
+            if (p.dbg) {
+                atomicAdd((unsigned long long*)&p.dbg[ConvDbg::TOTAL], (unsigned long long)(clock64() - t_begin));
+                atomicAdd((unsigned long long*)&p.dbg[ConvDbg::CTAS], 1ull);
+            }
+            if (tl) p.dbg_tl[13] = p.dbg_tl[15] = clock64();
         }
     }
-    __syncthreads();
-    if (tl && threadIdx.x == 0) p.dbg_tl[15] = clock64();
+    // no CTA-wide barrier at exit: every TMA load is waited for by a consumer, and each warpgroup leader waits for its
+    // own stores, so the roles end independently (the two register budgets never meet again)
 }
 
 }  // namespace smapb

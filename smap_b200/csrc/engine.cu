@@ -495,8 +495,11 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     cp->tiles_y = tiles_y;
     const long long m_tiles = (long long)tiles_x * tiles_y * nimg;
     // Tile shape from a coarse model, the starting point of the autotuner and the choice when it is off: a tile's main
-    // loop costs about num_kb x (relative wgmma time of a 128 x c tile), every tile also pays an epilogue that does not
-    // overlap its own main loop, and time ~ waves x (main loop + epilogue).  Near-ties go to the wider tile.
+    // loop costs about num_kb x (relative wgmma time of a 128 x c tile) and every tile pays an epilogue.  The two consumer
+    // warpgroups overlap one tile's epilogue with the next tile's main loop, but a CTA's last epilogue and the epilogues
+    // of short-K tiles (epilogue longer than a main loop) stay exposed, so the model keeps time ~ waves x (main loop +
+    // epilogue).  Near-ties go to the wider tile.  The model only decides geometries that neither the committed tile table
+    // (smap_b200/tiles/h100.tsv, measured with this kernel by tools/make_tile_table.py) nor the autotuner covers.
     int bn = 0, cg = 1;
     {
         const int num_kb = L.k * L.k * (L.Cin / 64) + L.Cin2 / 64;
@@ -2264,20 +2267,20 @@ int smapb_profile_end(smapb_handle* h, double* ms_by_kind, int* launches_by_kind
     if (f) fclose(f);
     h->prof_used = 0;
     if (h->roles_dev && h->roles_used && getenv("SMAPB_ROLES_PLAN")) {
-        // mean wait cycles per role and CTA (or CTA pair) of every conv launch of the profiled window
+        // mean cycles per role and CTA of every conv launch of the profiled window (counter layout: ConvDbg)
         std::vector<long long> d(h->roles_used * 16);
         CK(cudaMemcpy(d.data(), h->roles_dev, d.size() * sizeof(long long), cudaMemcpyDeviceToHost));
         FILE* g = fopen(getenv("SMAPB_ROLES_PLAN"), "w");
         if (g) {
-            fprintf(g, "idx,name,desc,issuers,total,producer_wait_empty,mma_wait_full,mma_wait_tempty,g0_wait_tfull,g0_wait_stage,"
-                       "g0_wait_ring,g1_wait_tfull,g1_wait_stage,g1_wait_ring\n");
+            fprintf(g, "idx,name,desc,ctas,total,producer_wait_empty,g0_wait_full,g0_wait_order,g0_epilogue,g0_wait_ring,"
+                       "g0_wait_stage,g1_wait_full,g1_wait_order,g1_epilogue,g1_wait_ring,g1_wait_stage\n");
             for (size_t i = 0; i < h->roles_used && i < h->roles_desc.size(); i++) {
                 const long long* r = &d[i * 16];
-                const double n = r[8] > 0 ? (double)r[8] : 1.0;
-                const double cg = (strstr(h->roles_desc[i].c_str(), " cg2 ") || strstr(h->roles_desc[i].c_str(), " cg3 ")) ? 2.0 : 1.0;
-                fprintf(g, "%zu,%s,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f,%.0f\n", i, h->roles_desc[i].c_str(), n,
-                        r[7] / n, r[0] / n / cg, r[1] / n, r[2] / n, r[3] / n / cg, r[4] / n / cg, r[9] / n / cg, r[5] / n / cg,
-                        r[6] / n / cg, r[10] / n / cg);
+                const double n = r[ConvDbg::CTAS] > 0 ? (double)r[ConvDbg::CTAS] : 1.0;
+                fprintf(g, "%zu,%s,%.0f,%.0f,%.0f", i, h->roles_desc[i].c_str(), n, r[ConvDbg::TOTAL] / n,
+                        r[ConvDbg::PRODUCER_WAIT_EMPTY] / n);
+                for (int c = ConvDbg::CONS; c < ConvDbg::COUNT; c++) fprintf(g, ",%.0f", r[c] / n);
+                fprintf(g, "\n");
             }
             fclose(g);
         }
@@ -2402,11 +2405,17 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     if (dbg_dev) {
         long long d[16];
         CKT(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));
-        const double n = d[8] > 0 ? (double)d[8] : 1.0;  // number of CTAs
-        fprintf(stderr,
-                "[roles] bn%d units%d kb%d | mean cycles per CTA: total %.0f | producer wait-empty %.0f | consumer wait-full %.0f "
-                "wait-stage %.0f wait-ring %.0f\n",
-                bn, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, d[7] / n, d[0] / n, d[1] / n, d[4] / n, d[9] / n);
+        const double n = d[ConvDbg::CTAS] > 0 ? (double)d[ConvDbg::CTAS] : 1.0;
+        fprintf(stderr, "[roles] bn%d units%d kb%d | mean cycles per CTA: total %.0f | producer wait-empty %.0f", bn,
+                cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, d[ConvDbg::TOTAL] / n,
+                d[ConvDbg::PRODUCER_WAIT_EMPTY] / n);
+        for (int g = 0; g < 2; g++) {
+            const long long* c = d + ConvDbg::CONS + ConvDbg::CONS_N * g;
+            fprintf(stderr, " | g%d wait-full %.0f wait-order %.0f epilogue %.0f wait-ring %.0f wait-stage %.0f", g,
+                    c[ConvDbg::WAIT_FULL] / n, c[ConvDbg::WAIT_ORDER] / n, c[ConvDbg::EPILOGUE] / n, c[ConvDbg::WAIT_RING] / n,
+                    c[ConvDbg::WAIT_STAGE] / n);
+        }
+        fprintf(stderr, "\n");
         cp.dbg = nullptr;
     }
     if (tl_dev) {  // time line of CTA 0 of one warm launch (cycles since kernel entry)

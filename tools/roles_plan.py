@@ -1,8 +1,9 @@
 """Where every conv launch of one whole-path step waits (tools only): per-role wait cycles of the warp-specialised conv kernel
 collected INSIDE the plan (cache state and clocks of the real step, one handle, eager), grouped by layer geometry.
   SMAPB_ROLES_PLAN=out/roles_plan.csv python tools/roles_plan.py
-Columns (fractions of the MMA role's lifetime): mma waiting for operands (load bound) / for a free accumulator (epilogue
-bound); epilogue groups waiting for accumulators (main-loop bound) / epilogue inputs (ring) / output staging (store bound)."""
+Columns (fractions of the CTA's lifetime, both consumer warpgroups together): operands not landed (load bound), waiting
+for the main-loop turn (the other warpgroup's main loop: tensor bound), time in epilogues, and within it epilogue inputs not
+landed (ring) and the staging slot still being stored (store bound)."""
 import collections
 import csv
 import os
@@ -15,6 +16,7 @@ import torch
 from smap_b200 import schema
 from smap_b200.engine import RECORD_BYTES, Engine, scale_row
 
+COLS = ("wait_full", "wait_order", "epilogue", "wait_ring", "wait_stage")  # per consumer warpgroup (smapb_profile_end)
 path = os.environ.setdefault("SMAPB_ROLES_PLAN", "out/roles_plan.csv")
 B, H, W = 8, 512, 832
 eng = Engine(0, max_batch=B, in_h=H, in_w=W)
@@ -42,12 +44,11 @@ for r in rows:
     desc = r["desc"]
     a = agg.setdefault(desc, collections.defaultdict(float))
     a["n"] += 1
-    for k in ("total", "producer_wait_empty", "mma_wait_full", "mma_wait_tempty", "g0_wait_tfull", "g0_wait_stage", "g0_wait_ring",
-              "g1_wait_tfull", "g1_wait_stage", "g1_wait_ring"):
+    for k in ("total", "producer_wait_empty") + tuple("g%d_%s" % (g, c) for g in (0, 1) for c in COLS):
         a[k] += float(r[k])
-print("%-62s %7s %6s | mma: %5s %6s | epi: %5s %5s %5s" % ("layer", "ms/step", "n", "full", "tempty", "tfull", "ring", "stage"))
+print("%-62s %7s %6s | %5s %5s %5s | %5s %5s" % ("layer", "ms/step", "n", "full", "order", "epi", "ring", "stage"))
 for desc, a in sorted(agg.items(), key=lambda kv: -ms_by_desc.get(kv[0], 0)):
     t = a["total"] or 1.0
-    e = lambda k: 50.0 * (a["g0_" + k] + a["g1_" + k]) / t
-    print("%-62s %7.3f %6d | %5.0f%% %5.0f%% | %5.0f%% %4.0f%% %4.0f%%" % (desc[:62], ms_by_desc.get(desc, 0), a["n"] / 3,
-          100 * a["mma_wait_full"] / t, 100 * a["mma_wait_tempty"] / t, e("wait_tfull"), e("wait_ring"), e("wait_stage")))
+    e = lambda c: 50.0 * (a["g0_" + c] + a["g1_" + c]) / t
+    print("%-62s %7.3f %6d | %4.0f%% %4.0f%% %4.0f%% | %4.0f%% %4.0f%%" % (desc[:62], ms_by_desc.get(desc, 0), a["n"] / 3,
+          e("wait_full"), e("wait_order"), e("epilogue"), e("wait_ring"), e("wait_stage")))
