@@ -12,9 +12,19 @@ extern "C" {
 #endif
 
 /* 64-bit position-weighted checksums of the output tensor of every op of the batch-B plan, as left by the last forward.
- * sums[max_ops]; desc (optional): max_ops strings of desc_stride bytes describing each op.  Returns the number of ops. */
+ * sums[max_ops]; desc (optional): max_ops strings of desc_stride bytes (512 is enough) describing each op.  Returns the number
+ * of ops.  Op i here is dump index i of smapb_debug_dump.  A description is space-separated key=value fields:
+ *   name=<unit name>  kind=conv | conv_f32 | stem_tc | stem | s2d | maxpool | upadd
+ *     conv: tensor-core conv with split-bf16 output; conv_f32: fp32 NHWC output (heads, *.tapexp); stem_tc: the 7x7/s2
+ *     stem as a 4x1-tap conv over the s2d view; stem: the CUDA-core stem; s2d: space-to-depth of the image
+ *   inputs by role, as dump indices, absent roles left out: in= in2= res= p1= p2= up= (convs), a= b= (maxpool, upadd);
+ *     in=x is the network input image
+ *   convs:  tw= (patch width; 128 on the flat path) rev= (reverse tile order) k=<kh>x<kw> s= pad=<y>x<x> cin= cin2= s2=
+ *           cout= (padded) out=NxHxWxC bn= cg= relu= hasres= post= upmode= tiles= nterms=
+ *   others: out=NxHxWxC nterms= */
 int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int max_ops, char* desc, int desc_stride);
-/* Raw copy (both bf16 planes, or fp32 for head outputs) of op `idx`'s output into host memory; returns the bytes copied. */
+/* Raw copy (both bf16 planes, or fp32 for head outputs) of op `idx`'s output into host or device memory (the copy direction
+ * is inferred from the pointer); returns the bytes copied. */
 long long smapb_debug_dump(smapb_handle* h, int B, int idx, void* host, long long max_bytes, int which);
 
 /* Host-only: the resampling plan smapb_preprocess uses for a src_w x src_h image (no GPU work).  dims6 = {dst_w, dst_h,

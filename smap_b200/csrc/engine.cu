@@ -109,6 +109,10 @@ struct Op {
     bool record = false;     // some op on the other stream consumes this op's output
     cudaEvent_t ev = nullptr;
     std::string name;  // reference unit name (NVTX range, profiles)
+    // debug descriptions (smapb_debug_checksums): the tensors the op reads, in the order PlanBuilder::wire received them
+    // (conv: in, res, p1, p2, in2, up; null = role absent), and the output shape N, H, W, C of a conv
+    std::vector<const void*> inputs;
+    int dims[4] = {0, 0, 0, 0};
 };
 
 struct Plan {
@@ -707,6 +711,7 @@ struct PlanBuilder {
         const int idx = (int)plan->ops.size() - 1;
         Op& op = plan->ops[idx];
         op.stream = cur_stream;
+        op.inputs.assign(inputs.begin(), inputs.end());
         for (const void* in : inputs) {
             if (!in) continue;
             auto it = plan->producer.find(in);
@@ -841,6 +846,7 @@ struct PlanBuilder {
         if (!rc) rc = tune(*L, in, res, p1, p2, &out, relu, in2, up, &op);
         op.name = name;
         op.cp.reverse = reverse_for(in.ptr);
+        op.dims[0] = out.N, op.dims[1] = out.H, op.dims[2] = out.W, op.dims[3] = out.C;
         plan->ops.push_back(op);
         wire(out.ptr, {in.ptr, res ? res->ptr : nullptr, p1 ? p1->ptr : nullptr, p2 ? p2->ptr : nullptr,
                        in2 ? in2->ptr : nullptr, up ? up->ptr : nullptr});
@@ -860,6 +866,7 @@ struct PlanBuilder {
         rc = setup_conv(h, *L, in, nullptr, nullptr, nullptr, nullptr, &out, 0, &op.cp, &op.block_n, &op.flops);
         op.name = name;
         op.cp.reverse = reverse_for(in.ptr);
+        op.dims[0] = out.N, op.dims[1] = out.H, op.dims[2] = out.W, op.dims[3] = out.C;
         plan->ops.push_back(op);
         wire(out.ptr, {in.ptr});
         plan->n_conv++;
@@ -910,6 +917,7 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan, int instance = 0) {
                 os.name = "top.s2d";
                 oc.name = "top.conv";
                 os.out = s2d;
+                oc.dims[0] = stem.N, oc.dims[1] = stem.H, oc.dims[2] = stem.W, oc.dims[3] = stem.C;
                 plan->ops.push_back(os);
                 pb.wire(s2d.ptr, {});
                 plan->ops.push_back(oc);
@@ -921,6 +929,7 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan, int instance = 0) {
         if (!tc) {
             Op op;
             op.kind = OP_STEM;
+            op.name = "top.conv";
             op.out = stem;
             plan->ops.push_back(op);
             pb.wire(stem.ptr, {});
@@ -1140,6 +1149,48 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
         if (debug_sync) CK(cudaStreamSynchronize(st));
     }
     return 0;
+}
+
+// debug: the output tensor of an op that smapb_debug_dump / smapb_debug_checksums report (null: the op has no dumped
+// output) and its size in bytes (both bf16 planes, or fp32).  Both entry points number the dumped ops with this predicate.
+const void* dumped_output(const smapb_handle* h, const Op& op, long long* bytes) {
+    if (op.kind == OP_CONV && op.cp.out) return *bytes = op.cp.plane_stride * h->planes * 2, op.cp.out;
+    if (op.kind == OP_CONV && op.cp.out_f32) return *bytes = op.cp.plane_stride * 4, op.cp.out_f32;
+    if (op.out.ptr) return *bytes = op.out.plane() * h->planes * 2, op.out.ptr;
+    *bytes = 0;
+    return nullptr;
+}
+
+// debug: one self-describing line per dumped op (format: include/smap_b200_debug.h).  `dump_idx` maps every dumped
+// output tensor to its dump index, so that the op's inputs can be named by index.
+std::string debug_op_desc(const smapb_handle* h, const Op& op, const std::map<const void*, int>& dump_idx) {
+    static const char* const CONV_ROLES[6] = {"in", "res", "p1", "p2", "in2", "up"};
+    const bool is_conv = op.kind == OP_CONV;
+    const bool stem_tc = is_conv && op.cp.kh == 4 && op.cp.kw == 1;
+    const char* kind = is_conv ? (stem_tc ? "stem_tc" : op.cp.out ? "conv" : "conv_f32")
+                       : op.kind == OP_STEM ? "stem" : op.kind == OP_S2D ? "s2d" : op.kind == OP_MAXPOOL ? "maxpool"
+                       : op.kind == OP_UPADD ? "upadd" : "other";
+    std::string s = "name=" + (op.name.empty() ? std::string("?") : op.name) + " kind=" + kind;
+    if (op.kind == OP_STEM || op.kind == OP_S2D) s += " in=x";  // the network input image
+    for (size_t r = 0; r < op.inputs.size(); r++) {
+        if (!op.inputs[r]) continue;
+        const char* role = is_conv ? (r < 6 ? CONV_ROLES[r] : "?") : (r == 0 ? "a" : "b");
+        auto it = dump_idx.find(op.inputs[r]);
+        s += std::string(" ") + role + "=" + (it == dump_idx.end() ? std::string("?") : std::to_string(it->second));
+    }
+    char buf[320];
+    if (is_conv) {
+        snprintf(buf, sizeof buf,
+                 " tw=%d rev=%d k=%dx%d s=%d pad=%dx%d cin=%d cin2=%d s2=%d cout=%d out=%dx%dx%dx%d bn=%d cg=%d relu=%d "
+                 "hasres=%d post=%d upmode=%d tiles=%d nterms=%d",
+                 1 << op.cp.tw_log2, op.cp.reverse, op.cp.kh, op.cp.kw, op.cp.stride, op.cp.pad_y, op.cp.pad_x,
+                 op.cp.kchunks * 64, op.cp.kchunks2 * 64, op.cp.stride2, op.cp.Cout, op.dims[0], op.dims[1], op.dims[2],
+                 op.dims[3], op.block_n, op.cg, op.cp.relu, op.cp.has_res, op.cp.n_post, op.cp.up_mode,
+                 op.cp.total_tiles, h->nterms);
+    } else {
+        snprintf(buf, sizeof buf, " out=%dx%dx%dx%d nterms=%d", op.out.N, op.out.H, op.out.W, op.out.C, h->nterms);
+    }
+    return s + buf;
 }
 
 }  // namespace
@@ -2168,16 +2219,14 @@ long long smapb_debug_dump(smapb_handle* h, int B, int idx, void* host, long lon
     cudaDeviceSynchronize();
     int n = 0;
     for (const Op& op : plan->ops) {
-        const void* ptr = nullptr;
         long long bytes = 0;
-        if (op.kind == OP_CONV && op.cp.out) ptr = op.cp.out, bytes = op.cp.plane_stride * h->planes * 2;
-        else if (op.kind == OP_CONV && op.cp.out_f32) ptr = op.cp.out_f32, bytes = op.cp.plane_stride * 4;
-        else if (op.out.ptr) ptr = op.out.ptr, bytes = op.out.plane() * h->planes * 2;
-        else continue;
+        const void* ptr = dumped_output(h, op, &bytes);
+        if (!ptr) continue;
         if (n++ != idx) continue;
         (void)which;
         if (bytes > max_bytes) bytes = max_bytes;
-        if (bytes > 0) cudaMemcpy(host, ptr, (size_t)bytes, cudaMemcpyDeviceToHost);
+        // cudaMemcpyDefault: `host` may also be device memory (a test keeps large dumps on the GPU)
+        if (bytes > 0) CK(cudaMemcpy(host, ptr, (size_t)bytes, cudaMemcpyDefault));
         return bytes;
     }
     return -2;
@@ -2192,34 +2241,28 @@ int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int 
     CK(cudaDeviceSynchronize());
     unsigned long long* d = nullptr;
     CK(cudaMalloc((void**)&d, 8));
+    std::map<const void*, int> dump_idx;  // output tensor -> dump index (the numbering of smapb_debug_dump)
+    int n_dumped = 0;
+    for (const Op& op : plan->ops) {
+        long long bytes = 0;
+        const void* out = dumped_output(h, op, &bytes);
+        if (!out) continue;
+        if (!dump_idx.emplace(out, n_dumped++).second) {
+            cudaFree(d);
+            return fail(h, -2, "smapb_debug_checksums: two ops share an output tensor (" + op.name + ")");
+        }
+    }
     int n = 0;
     for (const Op& op : plan->ops) {
         if (n >= max_ops) break;
-        const void* ptr = nullptr;
-        long long words = 0;
-        char buf[160];
-        if (op.kind == OP_CONV && op.cp.out) {
-            ptr = op.cp.out;
-            words = op.cp.plane_stride * h->planes / 2;
-            snprintf(buf, sizeof buf, "conv k%dx%d s%d cin%d(+%d) cout%d out%dx%d bn%d cg%d res%d post%d up%d", op.cp.kh, op.cp.kw,
-                     op.cp.stride, op.cp.kchunks * 64, op.cp.kchunks2 * 64, op.cp.Cout, op.cp.Hout, op.cp.Wout, op.block_n,
-                     op.cg, op.cp.has_res, op.cp.n_post, op.cp.up_mode);
-        } else if (op.kind == OP_CONV && op.cp.out_f32) {
-            ptr = op.cp.out_f32;
-            words = op.cp.plane_stride;
-            snprintf(buf, sizeof buf, "conv_f32 k%dx%d cin%d cout%d out%dx%d bn%d", op.cp.kh, op.cp.kw, op.cp.kchunks * 64,
-                     op.cp.Cout, op.cp.Hout, op.cp.Wout, op.block_n);
-        } else if (op.out.ptr) {
-            ptr = op.out.ptr;
-            words = op.out.plane() * h->planes / 2;
-            snprintf(buf, sizeof buf, "op kind %d out %dx%dx%d", (int)op.kind, op.out.H, op.out.W, op.out.C);
-        } else {
-            continue;
-        }
+        long long bytes = 0;
+        const void* ptr = dumped_output(h, op, &bytes);
+        if (!ptr) continue;
+        const long long words = bytes / 4;
         CK(cudaMemset(d, 0, 8));
         checksum_kernel<<<132 * 4, 256>>>((const uint32_t*)ptr, words, d);
         CK(cudaMemcpy(&sums[n], d, 8, cudaMemcpyDeviceToHost));
-        if (desc) snprintf(desc + (size_t)n * desc_stride, desc_stride, "%s", buf);
+        if (desc) snprintf(desc + (size_t)n * desc_stride, desc_stride, "%s", debug_op_desc(h, op, dump_idx).c_str());
         n++;
     }
     cudaFree(d);
