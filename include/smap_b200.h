@@ -29,6 +29,11 @@ typedef struct smapb_handle smapb_handle;
 /* precision of the tensor-core convolutions */
 #define SMAPB_PREC_BF16X3 3 /* split-bf16 (hi+lo) operands, 3 MMAs per product, fp32 accumulate: fp32-faithful */
 #define SMAPB_PREC_BF16 1   /* single bf16 operands (fast, ~1e-2 relative; NOT parity grade) */
+/* single fp16 operands and activations: the cost of SMAPB_PREC_BF16 (same bytes, same MMA rate) with a 10-bit mantissa
+ * (4x finer rounding; the operand precision of cuDNN's TF32 convolutions).  fp16 is finite only up to 65504: folded weights
+ * beyond it make smapb_finalize_weights fail, and activations beyond it are clamped to +-65504 and counted
+ * (smapb_saturation_count). */
+#define SMAPB_PREC_FP16 16
 
 /* ---- lifetime -------------------------------------------------------------------------------- */
 /* Replaces: per-call ArrayGpu<T> scratch (extensions/arraygpu.hpp:62-77, re-created on every
@@ -209,6 +214,11 @@ int smapb_json_close(smapb_json_writer* w);
 /* ---- introspection ----------------------------------------------------------------------------- */
 /* number of kernels launched by this handle since creation */
 int64_t smapb_launch_count(const smapb_handle* h);
+/* SMAPB_PREC_FP16: number of activation elements this handle's kernels clamped to +-65504 since creation (or the last
+ * reset != 0, which zeroes the counter after reading it); 0 in the bf16 precisions.  Synchronises the device.  Any nonzero
+ * count means some layer produced values fp16 cannot hold and those outputs are not the model's: run such inputs (or
+ * weights) with SMAPB_PREC_BF16X3, or SMAPB_PREC_BF16 when speed matters more than the last digits.  < 0: error. */
+int64_t smapb_saturation_count(smapb_handle* h, int reset);
 /* Per-op device timing with CUDA events on the launching stream (bench.py roofline leg).  After
  * smapb_profile_begin every kernel launched through this handle is bracketed by events; smapb_profile_end
  * synchronises the device, sums milliseconds and launch counts per kind

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SMAPB_LIB") or os.path.join(HERE, "lib", "libsmap_b200.so")
 
 NJ, NL, MAXP, NC2D, SCALE_LEN = 15, 14, 127, 43, 9
-PREC_BF16X3, PREC_BF16 = 3, 1
+PREC_BF16X3, PREC_BF16, PREC_FP16 = 3, 1, 16
 RECORD_BYTES = MAXP * NJ * 4 * 8 + MAXP * 8 + MAXP * NJ * 4 * 4 + 8
 
 EXPORTS = [
@@ -20,7 +20,7 @@ EXPORTS = [
     "smapb_json_open", "smapb_json_append", "smapb_json_close", "smapb_preprocess", "smapb_preprocess_host",
     "smapb_comm_unique_id", "smapb_comm_create", "smapb_comm_attach", "smapb_allgather_records",
     "smapb_infer_device_gather", "smapb_submit_host_gather", "smapb_set_tile_table", "smapb_get_tile_table",
-    "smapb_lift3d_gt", "smapb_infer_device_gather_async", "smapb_gather_sync",
+    "smapb_lift3d_gt", "smapb_infer_device_gather_async", "smapb_gather_sync", "smapb_saturation_count",
 ]
 
 _lib = None
@@ -63,6 +63,8 @@ def load():
     lib.smapb_wait.argtypes = [vp, i32]
     lib.smapb_launch_count.argtypes = [vp]
     lib.smapb_launch_count.restype = i64
+    lib.smapb_saturation_count.argtypes = [vp, i32]
+    lib.smapb_saturation_count.restype = i64
     lib.smapb_profile_begin.argtypes = [vp]
     lib.smapb_profile_end.argtypes = [vp, c.POINTER(c.c_double), c.POINTER(i32), c.c_char_p]
     lib.smapb_plan_info.argtypes = [vp, i32, c.POINTER(i32), c.POINTER(c.c_double)]

@@ -1,7 +1,9 @@
 // Shared device helpers for the smap_b200 kernels (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 
 #ifndef __CUDA_ARCH_FEAT_SM90_ALL
@@ -86,5 +88,53 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
 }
 __device__ __forceinline__ float bf16lo_to_f(uint32_t packed) { return __uint_as_float(packed << 16); }
 __device__ __forceinline__ float bf16hi_to_f(uint32_t packed) { return __uint_as_float(packed & 0xffff0000u); }
+
+// ---------------------------------------------------------------------------------------------
+// Activation / weight element format.  Every 2-byte format the kernels store is described here: the wgmma operand type,
+// the TMA data type, pack (fp32 -> 2 elements, round to nearest even) and unpack (exact widening).
+//   ElemBF16 : bf16, fp32's exponent range (the bf16x3 and bf16 precisions)
+//   ElemF16  : fp16, 10-bit mantissa, finite range +-65504: stores clamp to it and count the clamped elements
+// ---------------------------------------------------------------------------------------------
+struct ElemBF16 {
+    static constexpr bool F16 = false;
+    static constexpr CUtensorMapDataType TMA_DTYPE = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    // low half = a, high half = b
+    static __device__ __forceinline__ uint32_t pack2(float a, float b) {
+        uint32_t w;
+        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(b), "f"(a));
+        return w;
+    }
+    static __device__ __forceinline__ float lo(uint32_t w) { return bf16lo_to_f(w); }
+    static __device__ __forceinline__ float hi(uint32_t w) { return bf16hi_to_f(w); }
+};
+struct ElemF16 {
+    static constexpr bool F16 = true;
+    static constexpr CUtensorMapDataType TMA_DTYPE = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    static constexpr float MAX = 65504.f;
+    static __device__ __forceinline__ uint32_t pack2(float a, float b) {
+        uint32_t w;
+        asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(b), "f"(a));
+        return w;
+    }
+    static __device__ __forceinline__ float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xffffu))); }
+    static __device__ __forceinline__ float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
+    // max(m, |v|), NaN if either is NaN
+    static __device__ __forceinline__ float absmax(float m, float v) {
+        float r;
+        asm("{\n\t.reg .f32 t;\n\tabs.f32 t, %2;\n\tmax.NaN.f32 %0, %1, t;\n\t}" : "=f"(r) : "f"(m), "f"(v));
+        return r;
+    }
+    // v limited to the finite fp16 range (NaN -> -MAX); n counts the values that were outside it
+    static __device__ __forceinline__ float clamp(float v, int& n) {
+        n += !(fabsf(v) <= MAX);
+        return fminf(fmaxf(v, -MAX), MAX);
+    }
+};
+// Adds a warp's clamp count to the saturation counter: one atomic per warp, and none when nothing was clamped.  Every lane
+// of the warp must call it.
+__device__ __forceinline__ void saturation_add(unsigned long long* counter, int n) {
+    const unsigned total = __reduce_add_sync(0xffffffffu, (unsigned)n);
+    if (total != 0 && (threadIdx.x & 31) == 0 && counter) atomicAdd(counter, (unsigned long long)total);
+}
 
 }  // namespace smapb

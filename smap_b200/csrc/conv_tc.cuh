@@ -3,7 +3,7 @@
 //   y[n, oy, ox, co] = epilogue( sum_{ky,kx,ci} x[n, oy*s+ky-p, ox*s+kx-p, ci] * w[co, ci, ky, kx] )
 //
 // GEMM view: M = output pixels (a th x tw spatial patch = 128 rows per tile), N = Cout, K = taps * Cin.
-// One k-block = one filter tap x 64 input channels.  Operands are K-major bf16 tiles of 128-byte rows in
+// One k-block = one filter tap x 64 input channels.  Operands are K-major 2-byte (bf16 or fp16) tiles of 128-byte rows in
 // SWIZZLE_128B shared-memory layout, written by TMA:
 //   A: 5-D tensor map (C, W, H, N, term) over the NHWC activation planes; the tap shift is a coordinate
 //      offset, zero padding is TMA out-of-bounds fill, conv stride is the map's elementStrides.
@@ -11,7 +11,8 @@
 // Precision: "bf16x3" - every fp32 value v is carried as two bf16 planes (hi = bf16(v), lo = bf16(v - hi));
 // a product a*b is issued as 3 MMAs  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  into the same fp32 accumulator
 // (dropped terms are O(2^-16) relative) - fp32-faithful results at 3x the bf16 MMA count.  NTERMS = 1 is the
-// plain bf16 fast mode.
+// plain bf16 fast mode.  With E = ElemF16 (NTERMS = 1) operands and stored activations are fp16 (same bytes, same MMA rate,
+// 4x finer rounding than bf16); the epilogue clamps every stored value to +-65504 and counts the clamped elements in p.sat.
 //
 // Roles (384 threads, persistent CTA, static tile schedule; every role branch is warpgroup-uniform, registers are
 // rebalanced per role with setmaxnreg):
@@ -64,6 +65,7 @@ struct alignas(64) ConvParams {
     int up_mode, up_Hi, up_Wi, up_pw, up_ph;
     long long* dbg;  // optional: per-role cycle counters, layout ConvDbg below (tools/roles_plan.py), null in production
     long long* dbg_tl;  // optional: clock64 time line of CTA 0 (SMAPB_TIMELINE, smapb_conv_test only), null in production
+    unsigned long long* sat;  // fp16 kernels: count of stored elements clamped to +-65504 (the handle's saturation counter)
 };
 
 // ---- TMA / wgmma PTX wrappers -------------------------------------------------------------------
@@ -144,12 +146,6 @@ __device__ __forceinline__ uint32_t sw64_off(int r, int j) { return (uint32_t)(r
 __device__ __forceinline__ float up_scale(int in, int out) { return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f; }
 __device__ __forceinline__ int up_src_index(int dst, int in, int out) { return (int)(up_scale(in, out) * (float)dst); }
 
-// bf16x2 pack with round-to-nearest-even: low half = a, high half = b
-__device__ __forceinline__ uint32_t cvt_bf16x2(float a, float b) {
-    uint32_t w;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(b), "f"(a));
-    return w;
-}
 // the fp32 values (low half, high half) a hi/lo pair of bf16x2 words carries: hi + lo, exact widening, one rounding
 __device__ __forceinline__ float2 planes_to_f2(uint32_t h, uint32_t l) {
     return make_float2(bf16lo_to_f(h) + bf16lo_to_f(l), bf16hi_to_f(h) + bf16hi_to_f(l));
@@ -173,49 +169,64 @@ __device__ __forceinline__ void wgmma_wait() {
 }
 // D[64 x N] (+)= A[64 x 16] * B[16 x N]^T, fp32 accumulators in the wgmma fragment layout: thread t of the warpgroup holds
 // rows 16 (t / 32) + (t % 32) / 4 + {0, 8} and columns 8 j + 2 (t % 4) + {0, 1} as d[4 j + 2 {0, 1} + {0, 1}]
+template <class E>
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, "
-        "%36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, "
-        "%59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
-          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
-          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
-          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
-          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+#define SMAPB_WGMMA(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, " \
+        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, " \
+        "%36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, " \
+        "%59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), \
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), \
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), \
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), \
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), \
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), \
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+    if constexpr (E::F16) SMAPB_WGMMA("f16");
+    else SMAPB_WGMMA("bf16");
+#undef SMAPB_WGMMA
 }
+template <class E>
 __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, "
-        "1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+#define SMAPB_WGMMA(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, " \
+        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, " \
+        "1, 0, 0;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), \
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), \
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+    if constexpr (E::F16) SMAPB_WGMMA("f16");
+    else SMAPB_WGMMA("bf16");
+#undef SMAPB_WGMMA
 }
+template <class E>
 __device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+#define SMAPB_WGMMA(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, " \
+        "%13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+    if constexpr (E::F16) SMAPB_WGMMA("f16");
+    else SMAPB_WGMMA("bf16");
+#undef SMAPB_WGMMA
 }
-template <int BLOCK_N>
+template <int BLOCK_N, class E>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    if constexpr (BLOCK_N == 128) wgmma_m64n128(d, adesc, bdesc, accumulate);
-    else if constexpr (BLOCK_N == 64) wgmma_m64n64(d, adesc, bdesc, accumulate);
-    else wgmma_m64n32(d, adesc, bdesc, accumulate);
+    if constexpr (BLOCK_N == 128) wgmma_m64n128<E>(d, adesc, bdesc, accumulate);
+    else if constexpr (BLOCK_N == 64) wgmma_m64n64<E>(d, adesc, bdesc, accumulate);
+    else wgmma_m64n32<E>(d, adesc, bdesc, accumulate);
 }
 
 // mbar_wait that also returns the cycles spent waiting (role-level profiling; only used when p.dbg != null)
@@ -259,8 +270,10 @@ struct ConvCfg {
     static_assert(BLOCK_N == 32 || BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
 };
 
-template <int BLOCK_N, int NTERMS, int RING>
+// E: element format of activations and weights (common.cuh); ElemF16 requires NTERMS == 1
+template <int BLOCK_N, int NTERMS, int RING, class E>
 __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__ ConvParams p) {
+    static_assert(!E::F16 || NTERMS == 1, "fp16 operands are single-term");
     using Cfg = ConvCfg<BLOCK_N, NTERMS, RING>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr bool UP = (RING == 2);  // the ring carries low-resolution patches the epilogue interpolates
@@ -440,10 +453,10 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         const uint64_t ka = a0 + (uint64_t)(k * 2) + h * A_HALF, kbd = b0 + (uint64_t)(k * 2);
-                        wgmma_tile<BLOCK_N>(acc[h], ka, kbd, (kb | k) != 0);  // a_hi * b_hi
+                        wgmma_tile<BLOCK_N, E>(acc[h], ka, kbd, (kb | k) != 0);  // a_hi * b_hi
                         if (NTERMS == 3) {
-                            wgmma_tile<BLOCK_N>(acc[h], ka + A_STEP, kbd, 1u);  // a_lo * b_hi
-                            wgmma_tile<BLOCK_N>(acc[h], ka, kbd + B_STEP, 1u);  // a_hi * b_lo
+                            wgmma_tile<BLOCK_N, E>(acc[h], ka + A_STEP, kbd, 1u);  // a_lo * b_hi
+                            wgmma_tile<BLOCK_N, E>(acc[h], ka, kbd + B_STEP, 1u);  // a_hi * b_lo
                         }
                     }
                 }
@@ -495,7 +508,17 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                 fence_proxy_async();
                 mbar_arrive(&rempty_bar[rslot]);
             };
-            // vv += hi + lo (the fp32 value the two planes carry) of the next ring slot
+            // the fp32 values (low half, high half) of the two channels at byte offset o of a ring slot: hi + lo of the planes,
+            // or the widened fp16 pair
+            auto ring_f2 = [&](uint32_t rb, uint32_t o) -> float2 {
+                if constexpr (E::F16) {
+                    const uint32_t w = lds_u32(rb + o);
+                    return make_float2(E::lo(w), E::hi(w));
+                } else {
+                    return planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                }
+            };
+            // vv += the fp32 value the next ring slot carries
             auto ring_add = [&](float(&vv)[4][8]) {
                 const uint32_t rslot = ring_wait();
                 const uint32_t rb = res_stage + rslot * Cfg::SLOT_BYTES;
@@ -504,7 +527,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
 #pragma unroll
                     for (int jj = 0; jj < 4; jj++) {
                         const uint32_t o = sw64_off(row_of(q), jj) + 4 * q4;
-                        const float2 rv = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                        const float2 rv = ring_f2(rb, o);
                         vv[q][2 * jj] += rv.x;
                         vv[q][2 * jj + 1] += rv.y;
                     }
@@ -547,7 +570,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
 #pragma unroll
                             for (int k = 0; k < 4; k++) {
                                 const uint32_t o = sw64_off(rr[k], jj) + 4 * q4;
-                                s[k] = planes_to_f2(lds_u32(rb + o), NTERMS == 3 ? lds_u32(rb + Cfg::CHUNK_BYTES + o) : 0u);
+                                s[k] = ring_f2(rb, o);
                             }
                             v[q][2 * jj] += hy0 * (wx0 * s[0].x + wx1 * s[1].x) + hy1 * (wx0 * s[2].x + wx1 * s[3].x);
                             v[q][2 * jj + 1] += hy0 * (wx0 * s[0].y + wx1 * s[1].y) + hy1 * (wx0 * s[2].y + wx1 * s[3].y);
@@ -570,18 +593,41 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
                         bulk_wait_read<Cfg::OUT_PER_WG - 1>();
                         tally(ConvDbg::WAIT_STAGE, timed ? clock64() - t0 : 0);
                     }
+                    // fp16: the clamp-and-count path only runs for a warp that holds a value outside +-65504 (or a NaN)
+                    bool sat_warp = false;
+                    if constexpr (E::F16) {
+                        float m = 0.f;
+#pragma unroll
+                        for (int q = 0; q < 4; q++)
+#pragma unroll
+                            for (int e = 0; e < 8; e++) m = E::absmax(m, v[q][e]);
+                        sat_warp = __any_sync(0xffffffffu, !(m <= E::MAX));
+                    }
                     epi_bar_sync(wg);
+                    int n_sat = 0;  // fp16: stored elements of this thread outside +-65504 (clamped)
 #pragma unroll
                     for (int q = 0; q < 4; q++)
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++) {
                             const float a = v[q][2 * jj], b = v[q][2 * jj + 1];
-                            const uint32_t hw = cvt_bf16x2(a, b);  // hi = bf16(v)
                             const uint32_t o = sw64_off(row_of(q), jj) + 4 * q4;
-                            sts_u32(ob + o, hw);
-                            if (NTERMS == 3)  // lo = bf16(v - hi)
-                                sts_u32(ob + Cfg::CHUNK_BYTES + o, cvt_bf16x2(a - bf16lo_to_f(hw), b - bf16hi_to_f(hw)));
+                            if constexpr (E::F16) {
+                                if (sat_warp) {
+                                    int n = 0;
+                                    sts_u32(ob + o, E::pack2(E::clamp(a, n), E::clamp(b, n)));
+                                    n_sat += valid[q] ? n : 0;  // rows outside the output are never stored
+                                } else {
+                                    sts_u32(ob + o, E::pack2(a, b));
+                                }
+                            } else {
+                                const uint32_t hw = E::pack2(a, b);  // hi = bf16(v)
+                                sts_u32(ob + o, hw);
+                                if (NTERMS == 3)  // lo = bf16(v - hi)
+                                    sts_u32(ob + Cfg::CHUNK_BYTES + o, E::pack2(a - E::lo(hw), b - E::hi(hw)));
+                            }
                         }
+                    if constexpr (E::F16)
+                        if (sat_warp) saturation_add(p.sat, n_sat);
                     fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA store
                     epi_bar_sync(wg);
                     if (leader) {

@@ -1,5 +1,7 @@
-// Non-GEMM kernels of the backbone (HBM-bound, NHWC split-bf16 activations): stem 7x7 conv, max-pool,
+// Non-GEMM kernels of the backbone (HBM-bound, NHWC split-bf16 or fp16 activations): stem 7x7 conv, max-pool,
 // bilinear(align_corners) up-sample + add + ReLU, head merge + NHWC->NCHW, flip-TTA merge / rescale.
+// Kernels that write activations are templated on the element format E (common.cuh).  The fp16 variants clamp every value
+// they compute to +-65504 and add the number of clamped elements to the handle's saturation counter.
 #include "elementwise.h"
 #include "common.cuh"
 
@@ -8,18 +10,26 @@ namespace smapb {
 // ---------------------------------------------------------------------------------------------
 // fp32 NHWC -> split-bf16 planes (test hook + generic converter)
 // ---------------------------------------------------------------------------------------------
+template <class E>
 __global__ void f32_to_split_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, long long n,
                                     long long plane_stride, int terms) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    __nv_bfloat16 h, l;
-    split_bf16(x[i], h, l);
-    out[i] = h;
-    if (terms == 2) out[plane_stride + i] = l;
+    if constexpr (E::F16) {
+        reinterpret_cast<__half*>(out)[i] = __float2half_rn(x[i]);
+    } else {
+        __nv_bfloat16 h, l;
+        split_bf16(x[i], h, l);
+        out[i] = h;
+        if (terms == 2) out[plane_stride + i] = l;
+    }
 }
 cudaError_t launch_f32_to_split(const float* x, __nv_bfloat16* out, long long n, long long plane_stride, int terms,
-                                cudaStream_t st) {
-    f32_to_split_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, out, n, plane_stride, terms);
+                                cudaStream_t st, bool f16) {
+    if (f16)
+        f32_to_split_kernel<ElemF16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, out, n, plane_stride, terms);
+    else
+        f32_to_split_kernel<ElemBF16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, out, n, plane_stride, terms);
     return cudaGetLastError();
 }
 
@@ -35,10 +45,11 @@ constexpr int ST_PWP = ST_PW + 3;                               // padded row pi
 
 // thread = 4 adjacent output pixels x 16 channels (4 passes over the channel groups): per (ky, ci) row the 13 input
 // values and the 7x16 weights are loaded once and feed 448 FFMAs (11 FFMA per shared-memory load).
+template <class E>
 __global__ void __launch_bounds__(256, 2)
 stem_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[147][64] (ky,kx,ci) x co*/,
             const float* __restrict__ bias, int H, int W, __nv_bfloat16* __restrict__ out, long long plane_stride,
-            int terms) {
+            int terms, unsigned long long* sat) {
     extern __shared__ __align__(16) float stem_smem[];
     float* s_w = stem_smem;                   // [147*64]
     float* s_in = stem_smem + 147 * 64;       // [3][ST_PH][ST_PWP]
@@ -59,6 +70,7 @@ stem_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[147][6
     __syncthreads();
     const int ty = threadIdx.x / (ST_TW / ST_PX), tx = (threadIdx.x % (ST_TW / ST_PX)) * ST_PX;
     const int oy = oy0 + ty;
+    int n_sat = 0;
 #pragma unroll 1
     for (int cg = 0; cg < 4; cg++) {
         float acc[ST_PX][16];
@@ -105,38 +117,51 @@ stem_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[147][6
                 for (int j = 0; j < 8; j++) {
                     const float a = fmaxf(acc[p][2 * j] + bias[cg * 16 + 2 * j], 0.f);
                     const float b = fmaxf(acc[p][2 * j + 1] + bias[cg * 16 + 2 * j + 1], 0.f);
-                    __nv_bfloat16 ah, al, bh, bl;
-                    split_bf16(a, ah, al);
-                    split_bf16(b, bh, bl);
-                    hw_[j] = pack_bf16x2(ah, bh);
-                    lw_[j] = pack_bf16x2(al, bl);
+                    if constexpr (E::F16) {
+                        hw_[j] = E::pack2(E::clamp(a, n_sat), E::clamp(b, n_sat));
+                    } else {
+                        __nv_bfloat16 ah, al, bh, bl;
+                        split_bf16(a, ah, al);
+                        split_bf16(b, bh, bl);
+                        hw_[j] = pack_bf16x2(ah, bh);
+                        lw_[j] = pack_bf16x2(al, bl);
+                    }
                 }
                 uint4* oh = reinterpret_cast<uint4*>(out + obase + cg * 16);
                 oh[0] = make_uint4(hw_[0], hw_[1], hw_[2], hw_[3]);
                 oh[1] = make_uint4(hw_[4], hw_[5], hw_[6], hw_[7]);
-                if (terms == 2) {
-                    uint4* ol = reinterpret_cast<uint4*>(out + plane_stride + obase + cg * 16);
-                    ol[0] = make_uint4(lw_[0], lw_[1], lw_[2], lw_[3]);
-                    ol[1] = make_uint4(lw_[4], lw_[5], lw_[6], lw_[7]);
+                if constexpr (!E::F16) {
+                    if (terms == 2) {
+                        uint4* ol = reinterpret_cast<uint4*>(out + plane_stride + obase + cg * 16);
+                        ol[0] = make_uint4(lw_[0], lw_[1], lw_[2], lw_[3]);
+                        ol[1] = make_uint4(lw_[4], lw_[5], lw_[6], lw_[7]);
+                    }
                 }
             }
         }
     }
+    if constexpr (E::F16) saturation_add(sat, n_sat);
     pdl_trigger();
 }
-cudaError_t launch_stem(const float* x, const float* wgt, const float* bias, int N, int H, int W, __nv_bfloat16* out,
-                        long long plane_stride, int terms, cudaStream_t st) {
+template <class E>
+cudaError_t launch_stem_e(const float* x, const float* wgt, const float* bias, int N, int H, int W, __nv_bfloat16* out,
+                          long long plane_stride, int terms, cudaStream_t st, unsigned long long* sat) {
     const int Ho = H / 2, Wo = W / 2;
     dim3 grid((Wo + ST_TW - 1) / ST_TW, (Ho + ST_TH - 1) / ST_TH, N);
     constexpr int smem = (147 * 64 + 3 * ST_PH * ST_PWP) * 4;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(stem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(stem_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
         configured = true;
     }
-    stem_kernel<<<grid, 256, smem, st>>>(x, wgt, bias, H, W, out, plane_stride, terms);
+    stem_kernel<E><<<grid, 256, smem, st>>>(x, wgt, bias, H, W, out, plane_stride, terms, sat);
     return cudaGetLastError();
+}
+cudaError_t launch_stem(const float* x, const float* wgt, const float* bias, int N, int H, int W, __nv_bfloat16* out,
+                        long long plane_stride, int terms, cudaStream_t st, bool f16, unsigned long long* sat) {
+    return f16 ? launch_stem_e<ElemF16>(x, wgt, bias, N, H, W, out, plane_stride, terms, st, sat)
+               : launch_stem_e<ElemBF16>(x, wgt, bias, N, H, W, out, plane_stride, terms, st, sat);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -145,10 +170,12 @@ cudaError_t launch_stem(const float* x, const float* wgt, const float* bias, int
 // zero pixel columns 0,1 (left) and W/2+2 (right), so that every 4-pixel sliding window [x-2, x+1] of the 7x7/s2
 // receptive field is a contiguous, in-bounds 128-byte row for TMA.
 // ---------------------------------------------------------------------------------------------
+template <class E>
 __global__ void s2d_kernel(const float* __restrict__ x, int N, int H, int W, __nv_bfloat16* __restrict__ out,
-                           long long plane_stride, int terms) {
+                           long long plane_stride, int terms, unsigned long long* sat) {
     const int H2 = H / 2, W2 = W / 2, WP = W2 + 3;
     const long long total = (long long)N * H2 * WP;
+    int n_sat = 0;
     pdl_wait();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int xp = (int)(i % WP);
@@ -172,28 +199,38 @@ __global__ void s2d_kernel(const float* __restrict__ x, int N, int H, int W, __n
         uint32_t hw_[8], lw_[8];
 #pragma unroll
         for (int j = 0; j < 8; j++) {
-            __nv_bfloat16 ah, al, bh, bl;
-            split_bf16(v[2 * j], ah, al);
-            split_bf16(v[2 * j + 1], bh, bl);
-            hw_[j] = pack_bf16x2(ah, bh);
-            lw_[j] = pack_bf16x2(al, bl);
+            if constexpr (E::F16) {
+                hw_[j] = E::pack2(E::clamp(v[2 * j], n_sat), E::clamp(v[2 * j + 1], n_sat));
+            } else {
+                __nv_bfloat16 ah, al, bh, bl;
+                split_bf16(v[2 * j], ah, al);
+                split_bf16(v[2 * j + 1], bh, bl);
+                hw_[j] = pack_bf16x2(ah, bh);
+                lw_[j] = pack_bf16x2(al, bl);
+            }
         }
         uint4* oh = reinterpret_cast<uint4*>(out + i * 16);
         oh[0] = make_uint4(hw_[0], hw_[1], hw_[2], hw_[3]);
         oh[1] = make_uint4(hw_[4], hw_[5], hw_[6], hw_[7]);
-        if (terms == 2) {
-            uint4* ol = reinterpret_cast<uint4*>(out + plane_stride + i * 16);
-            ol[0] = make_uint4(lw_[0], lw_[1], lw_[2], lw_[3]);
-            ol[1] = make_uint4(lw_[4], lw_[5], lw_[6], lw_[7]);
+        if constexpr (!E::F16) {
+            if (terms == 2) {
+                uint4* ol = reinterpret_cast<uint4*>(out + plane_stride + i * 16);
+                ol[0] = make_uint4(lw_[0], lw_[1], lw_[2], lw_[3]);
+                ol[1] = make_uint4(lw_[4], lw_[5], lw_[6], lw_[7]);
+            }
         }
     }
+    if constexpr (E::F16) saturation_add(sat, n_sat);
     pdl_trigger();
 }
 cudaError_t launch_s2d(const float* x, int N, int H, int W, __nv_bfloat16* out, long long plane_stride, int terms,
-                       cudaStream_t st) {
+                       cudaStream_t st, bool f16, unsigned long long* sat) {
     const long long total = (long long)N * (H / 2) * (W / 2 + 3);
     const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
-    s2d_kernel<<<blocks, 256, 0, st>>>(x, N, H, W, out, plane_stride, terms);
+    if (f16)
+        s2d_kernel<ElemF16><<<blocks, 256, 0, st>>>(x, N, H, W, out, plane_stride, terms, sat);
+    else
+        s2d_kernel<ElemBF16><<<blocks, 256, 0, st>>>(x, N, H, W, out, plane_stride, terms, sat);
     return cudaGetLastError();
 }
 
@@ -221,23 +258,41 @@ __device__ __forceinline__ void pack8(const float (&v)[8], uint4& h, uint4& l) {
     h = make_uint4(hh[0], hh[1], hh[2], hh[3]);
     l = make_uint4(ll[0], ll[1], ll[2], ll[3]);
 }
+template <class E>
 __device__ __forceinline__ void load8(const __nv_bfloat16* p, long long plane_stride, int terms, float (&v)[8]) {
     const uint4 h = *reinterpret_cast<const uint4*>(p);
-    const uint4 l = (terms == 2) ? *reinterpret_cast<const uint4*>(p + plane_stride) : make_uint4(0, 0, 0, 0);
-    unpack8(h, l, v);
+    if constexpr (E::F16) {
+        const uint32_t hh[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+        for (int e = 0; e < 4; e++) v[2 * e] = E::lo(hh[e]), v[2 * e + 1] = E::hi(hh[e]);
+    } else {
+        const uint4 l = (terms == 2) ? *reinterpret_cast<const uint4*>(p + plane_stride) : make_uint4(0, 0, 0, 0);
+        unpack8(h, l, v);
+    }
 }
-__device__ __forceinline__ void store8(__nv_bfloat16* p, long long plane_stride, int terms, const float (&v)[8]) {
-    uint4 h, l;
-    pack8(v, h, l);
-    *reinterpret_cast<uint4*>(p) = h;
-    if (terms == 2) *reinterpret_cast<uint4*>(p + plane_stride) = l;
+// fp16: values outside +-65504 are clamped and counted in n_sat
+template <class E>
+__device__ __forceinline__ void store8(__nv_bfloat16* p, long long plane_stride, int terms, const float (&v)[8], int& n_sat) {
+    if constexpr (E::F16) {
+        *reinterpret_cast<uint4*>(p) = make_uint4(E::pack2(E::clamp(v[0], n_sat), E::clamp(v[1], n_sat)),
+                                                  E::pack2(E::clamp(v[2], n_sat), E::clamp(v[3], n_sat)),
+                                                  E::pack2(E::clamp(v[4], n_sat), E::clamp(v[5], n_sat)),
+                                                  E::pack2(E::clamp(v[6], n_sat), E::clamp(v[7], n_sat)));
+    } else {
+        uint4 h, l;
+        pack8(v, h, l);
+        *reinterpret_cast<uint4*>(p) = h;
+        if (terms == 2) *reinterpret_cast<uint4*>(p + plane_stride) = l;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
 // MaxPool 3x3 stride 2 pad 1 (model/smap.py:86).  Input is post-ReLU (>= 0) so zero padding == -inf padding.
 // ---------------------------------------------------------------------------------------------
+template <class E>
 __global__ void maxpool_kernel(const __nv_bfloat16* __restrict__ in, long long in_ps, int N, int H, int W, int C,
                                __nv_bfloat16* __restrict__ out, long long out_ps, int terms) {
+    int n_sat = 0;  // the maximum of stored values is a stored value: nothing to clamp
     const int Ho = H / 2, Wo = W / 2, CG = C / 8;
     const long long total = (long long)N * Ho * Wo * CG;
     pdl_wait();
@@ -258,20 +313,23 @@ __global__ void maxpool_kernel(const __nv_bfloat16* __restrict__ in, long long i
                 const int ix = ox * 2 + dx;
                 if (ix < 0 || ix >= W) continue;
                 float v[8];
-                load8(in + (((long long)n * H + iy) * W + ix) * C + cg * 8, in_ps, terms, v);
+                load8<E>(in + (((long long)n * H + iy) * W + ix) * C + cg * 8, in_ps, terms, v);
 #pragma unroll
                 for (int j = 0; j < 8; j++) m[j] = fmaxf(m[j], v[j]);
             }
         }
-        store8(out + (((long long)n * Ho + oy) * Wo + ox) * C + cg * 8, out_ps, terms, m);
+        store8<E>(out + (((long long)n * Ho + oy) * Wo + ox) * C + cg * 8, out_ps, terms, m, n_sat);
     }
     pdl_trigger();
 }
 cudaError_t launch_maxpool(const __nv_bfloat16* in, long long in_ps, int N, int H, int W, int C, __nv_bfloat16* out,
-                           long long out_ps, int terms, cudaStream_t st) {
+                           long long out_ps, int terms, cudaStream_t st, bool f16) {
     const long long total = (long long)N * (H / 2) * (W / 2) * (C / 8);
     const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
-    maxpool_kernel<<<blocks, 256, 0, st>>>(in, in_ps, N, H, W, C, out, out_ps, terms);
+    if (f16)
+        maxpool_kernel<ElemF16><<<blocks, 256, 0, st>>>(in, in_ps, N, H, W, C, out, out_ps, terms);
+    else
+        maxpool_kernel<ElemBF16><<<blocks, 256, 0, st>>>(in, in_ps, N, H, W, C, out, out_ps, terms);
     return cudaGetLastError();
 }
 
@@ -290,11 +348,13 @@ __device__ __forceinline__ void bilin_coeff(int o, int in, int out, int& i0, int
     l0 = 1.f - l1;
 }
 
+template <class E>
 __global__ void upadd_relu_kernel(const __nv_bfloat16* __restrict__ a, long long a_ps, const __nv_bfloat16* __restrict__ t,
                                   long long t_ps, int N, int H, int W, int Hi, int Wi, int C,
-                                  __nv_bfloat16* __restrict__ out, long long out_ps, int terms) {
+                                  __nv_bfloat16* __restrict__ out, long long out_ps, int terms, unsigned long long* sat) {
     const int CG = C / 8;
     const long long total = (long long)N * H * W * CG;
+    int n_sat = 0;
     pdl_wait();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int cg = (int)(i % CG);
@@ -309,26 +369,30 @@ __global__ void upadd_relu_kernel(const __nv_bfloat16* __restrict__ a, long long
         bilin_coeff(x, Wi, W, x0, x1, wx0, wx1);
         float v00[8], v01[8], v10[8], v11[8], va[8], o[8];
         const long long tb = (long long)n * Hi * Wi;
-        load8(t + ((tb + (long long)y0 * Wi + x0) * C) + cg * 8, t_ps, terms, v00);
-        load8(t + ((tb + (long long)y0 * Wi + x1) * C) + cg * 8, t_ps, terms, v01);
-        load8(t + ((tb + (long long)y1 * Wi + x0) * C) + cg * 8, t_ps, terms, v10);
-        load8(t + ((tb + (long long)y1 * Wi + x1) * C) + cg * 8, t_ps, terms, v11);
-        load8(a + i * 8, a_ps, terms, va);
+        load8<E>(t + ((tb + (long long)y0 * Wi + x0) * C) + cg * 8, t_ps, terms, v00);
+        load8<E>(t + ((tb + (long long)y0 * Wi + x1) * C) + cg * 8, t_ps, terms, v01);
+        load8<E>(t + ((tb + (long long)y1 * Wi + x0) * C) + cg * 8, t_ps, terms, v10);
+        load8<E>(t + ((tb + (long long)y1 * Wi + x1) * C) + cg * 8, t_ps, terms, v11);
+        load8<E>(a + i * 8, a_ps, terms, va);
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const float up = hy0 * (wx0 * v00[j] + wx1 * v01[j]) + hy1 * (wx0 * v10[j] + wx1 * v11[j]);
             o[j] = fmaxf(va[j] + up, 0.f);
         }
-        store8(out + i * 8, out_ps, terms, o);
+        store8<E>(out + i * 8, out_ps, terms, o, n_sat);
     }
+    if constexpr (E::F16) saturation_add(sat, n_sat);
     pdl_trigger();
 }
 cudaError_t launch_upadd_relu(const __nv_bfloat16* a, long long a_ps, const __nv_bfloat16* t, long long t_ps, int N,
                               int H, int W, int Hi, int Wi, int C, __nv_bfloat16* out, long long out_ps, int terms,
-                              cudaStream_t st) {
+                              cudaStream_t st, bool f16, unsigned long long* sat) {
     const long long total = (long long)N * H * W * (C / 8);
     const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
-    upadd_relu_kernel<<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms);
+    if (f16)
+        upadd_relu_kernel<ElemF16><<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms, sat);
+    else
+        upadd_relu_kernel<ElemBF16><<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms, sat);
     return cudaGetLastError();
 }
 

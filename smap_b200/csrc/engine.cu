@@ -53,6 +53,7 @@ inline float bf16_to_f32(uint16_t b) {
     memcpy(&f, &u, 4);
     return f;
 }
+inline uint16_t f32_to_f16_rn(float f) { return __half_as_ushort(__float2half_rn(f)); }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -142,8 +143,10 @@ struct smapb_handle {
     ConvLayer stem_tc;        // space-to-depth tensor-core stem (4 ky-blocks x 64 k)
     int stem_tc_ok = -1;      // -1 untested, 0 overlapped TMA view rejected (CUDA-core stem), 1 in use
     float* stem_b = nullptr;
-    int nterms = 3;  // MMA terms (3 = bf16x3, 1 = bf16)
+    int nterms = 3;  // MMA terms (3 = bf16x3, 1 = bf16 or fp16)
     int planes = 2;  // activation planes (2 or 1)
+    bool f16 = false;  // element format of weights and activations: fp16 (SMAPB_PREC_FP16) instead of bf16
+    unsigned long long* sat_dev = nullptr;  // fp16: activation elements clamped to +-65504 (smapb_saturation_count)
     bool finalized = false;
     std::map<int, std::unique_ptr<Plan>> plans;
     // association workspace (sized for max_batch)
@@ -341,6 +344,7 @@ int dev_alloc(smapb_handle* h, T** p, size_t count) {
 // ------------------------------------------------------------------------------------------------
 // tensor maps
 // ------------------------------------------------------------------------------------------------
+CUtensorMapDataType elem_dtype(const smapb_handle* h) { return h->f16 ? ElemF16::TMA_DTYPE : ElemBF16::TMA_DTYPE; }
 int make_act_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, long long C, long long W, long long H,
                  long long N, int T, long long plane_elems, int box_w, int box_h, int stride, int box_c = 64) {
     EncodeTiledFn fn = get_encode_fn();
@@ -351,7 +355,7 @@ int make_act_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, long
     cuuint32_t box[5] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1};
     cuuint32_t es[5] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1, 1};
     // 64-channel boxes (operands) use 128-byte rows, 32-channel boxes (epilogue tiles) 64-byte rows
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)ptr, dims, strides, box, es,
+    CUresult r = fn(m, elem_dtype(h), 5, (void*)ptr, dims, strides, box, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, box_c == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -370,7 +374,7 @@ int make_w_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, int Ci
     cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cout_pad * Cin * 2, (cuuint64_t)taps * Cout_pad * Cin * 2};
     cuuint32_t box[4] = {64, (cuuint32_t)block_n, 1, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)ptr, dims, strides, box, es,
+    CUresult r = fn(m, elem_dtype(h), 4, (void*)ptr, dims, strides, box, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(h, -21, "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r));
@@ -380,12 +384,12 @@ int make_w_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, int Ci
 // ------------------------------------------------------------------------------------------------
 // conv launch
 // ------------------------------------------------------------------------------------------------
-template <int BN, int NT, int RING>
+template <int BN, int NT, int RING, class E>
 cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
     using Cfg = ConvCfg<BN, NT, RING>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, NT, RING>,
+        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, NT, RING, E>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) return e;
         configured = true;
@@ -405,17 +409,18 @@ cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t s
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING>, cp);
+    return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING, E>, cp);
 }
-template <int BN, int NT>
+template <int BN, int NT, class E = ElemBF16>
 cudaError_t launch_conv_inst(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
-    if (cp.up_mode) return launch_conv_inst2<BN, NT, 2>(cp, sm_count, st, pdl);  // fused bilinear residual
-    return (cp.has_res + cp.n_post) ? launch_conv_inst2<BN, NT, 1>(cp, sm_count, st, pdl)
-                                    : launch_conv_inst2<BN, NT, 0>(cp, sm_count, st, pdl);
+    if (cp.up_mode) return launch_conv_inst2<BN, NT, 2, E>(cp, sm_count, st, pdl);  // fused bilinear residual
+    return (cp.has_res + cp.n_post) ? launch_conv_inst2<BN, NT, 1, E>(cp, sm_count, st, pdl)
+                                    : launch_conv_inst2<BN, NT, 0, E>(cp, sm_count, st, pdl);
 }
-cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, int sm_count, cudaStream_t st, bool pdl) {
+cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, bool f16, int sm_count, cudaStream_t st, bool pdl) {
 #define SMAPB_CASE(BN)                                                                  \
     case BN:                                                                            \
+        if (f16) return launch_conv_inst<BN, 1, ElemF16>(cp, sm_count, st, pdl);        \
         return nterms == 3 ? launch_conv_inst<BN, 3>(cp, sm_count, st, pdl)             \
                            : launch_conv_inst<BN, 1>(cp, sm_count, st, pdl);
     switch (block_n) {
@@ -559,6 +564,7 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const Act& in, const Act* re
     cp->out_f32 = outf ? outf->ptr : nullptr;
     cp->plane_stride = (long long)N * Ho * Wo * L.Cout_pad;
     cp->relu = relu;
+    cp->sat = h->sat_dev;
     rc = make_w_map(h, &cp->tmB, L.w_dev, L.Cin + L.Cin2, L.Cout_pad, L.k * L.k, h->planes, bn);
     if (rc) return rc;
     // epilogue tiles: 32 channels x (tw x th) pixels of the output / residual planes
@@ -600,7 +606,7 @@ int setup_stem_conv(smapb_handle* h, const __nv_bfloat16* s2d, long long s2d_pla
     cuuint64_t strides[4] = {32, (cuuint64_t)WP * 32, (cuuint64_t)H2 * WP * 32, (cuuint64_t)s2d_plane * 2};
     cuuint32_t box[5] = {64, (cuuint32_t)tw, (cuuint32_t)th, 1, 1};
     cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = fn(&cp->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)s2d, dims, strides, box, es,
+    CUresult r = fn(&cp->tmA, elem_dtype(h), 5, (void*)s2d, dims, strides, box, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(h, -22, "sliding-window tensor map rejected: " + std::to_string((int)r));
@@ -618,6 +624,7 @@ int setup_stem_conv(smapb_handle* h, const __nv_bfloat16* s2d, long long s2d_pla
     cp->out = out.ptr;
     cp->plane_stride = out.plane();
     cp->relu = 1;
+    cp->sat = h->sat_dev;
     int rc = make_w_map(h, &cp->tmB, L.w_dev, 64, 64, 4, h->planes, 64);
     if (rc) return rc;
     rc = make_act_map(h, &cp->tmO, out.ptr, 64, W2, H2, N, h->planes, out.plane(), tw, th, 1, 32);
@@ -660,16 +667,29 @@ int fold_unit(smapb_handle* h, const std::string& name, std::vector<float>* wf, 
     return 0;
 }
 
+// fp16 weights: a folded weight beyond the fp16 range cannot be represented (the unit needs bf16x3 or bf16)
+int check_f16_range(smapb_handle* h, const std::string& unit, const float* w, size_t n) {
+    for (size_t i = 0; i < n; i++)
+        if (!(fabsf(w[i]) <= 65504.f)) {
+            char buf[96];
+            snprintf(buf, sizeof buf, "%g", (double)w[i]);
+            return fail(h, -42, "fp16 precision: folded weight " + std::string(buf) + " of unit " + unit +
+                                    " exceeds the fp16 range (65504); use bf16x3 or bf16");
+        }
+    return 0;
+}
+
 int upload_conv_layer(smapb_handle* h, ConvLayer& L, const std::vector<float>& wf, const std::vector<float>& bf) {
     const int taps = L.k * L.k;
     const int cin = L.Cin + L.Cin2;  // wf holds [Cout][Cin + Cin2][taps] (taps == 1 for fused pairs)
     const size_t plane = (size_t)taps * L.Cout_pad * cin;
+    if (h->f16 && check_f16_range(h, L.name, wf.data(), wf.size())) return -42;
     std::vector<uint16_t> host(plane * h->planes, 0);
     for (int co = 0; co < L.Cout; co++)
         for (int ci = 0; ci < cin; ci++)
             for (int t = 0; t < taps; t++) {
                 const float v = wf[((size_t)co * cin + ci) * taps + t];
-                const uint16_t hi = f32_to_bf16_rn(v);
+                const uint16_t hi = h->f16 ? f32_to_f16_rn(v) : f32_to_bf16_rn(v);
                 const size_t o = ((size_t)t * L.Cout_pad + co) * cin + ci;
                 host[o] = hi;
                 if (h->planes == 2) host[plane + o] = f32_to_bf16_rn(v - bf16_to_f32(hi));
@@ -775,9 +795,10 @@ struct PlanBuilder {
     int tune(const ConvLayer& L, const Act& in, const Act* res, const Act* p1, const Act* p2, const Act* out, int relu,
              const Act* in2, const Act* up, Op* op) {
         char key[256];
-        snprintf(key, sizeof key, "%d/%d/%d k%d s%d %dx%dx%d r%d p%d u%d c2_%d s2_%d t%d", L.Cin, L.Cout_pad, L.Cin2, L.k,
+        // fp16 rows carry the element type: they never match (or overwrite) a bf16 row of the same geometry
+        snprintf(key, sizeof key, "%d/%d/%d k%d s%d %dx%dx%d r%d p%d u%d c2_%d s2_%d t%d%s", L.Cin, L.Cout_pad, L.Cin2, L.k,
                  L.stride, in.N, in.H, in.W, res ? 1 : 0, (p1 ? 1 : 0) + (p2 ? 1 : 0), up ? 1 : 0, L.Cin2, L.stride2,
-                 h->nterms);
+                 h->nterms, h->f16 ? " f16" : "");
         int best_bn = 0, best_cg = 1;
         bool known = false;
         {
@@ -804,7 +825,7 @@ struct PlanBuilder {
                 float ms_best_c = 1e30f;
                 for (int rep = 0; rep < 4; rep++) {
                     cudaEventRecord(e0, nullptr);
-                    if (launch_conv(trial.cp, trial.block_n, h->nterms, h->sm_count, nullptr, false) != cudaSuccess) {
+                    if (launch_conv(trial.cp, trial.block_n, h->nterms, h->f16, h->sm_count, nullptr, false) != cudaSuccess) {
                         ms_best_c = 1e30f;
                         break;
                     }
@@ -1095,24 +1116,26 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
         if (h->nvtx_ops) nvtxRangePushA(op.name.empty() ? "smapb.op" : op.name.c_str());
         switch (op.kind) {
             case OP_STEM:
-                CK(launch_stem(imgs, h->stem_w, h->stem_b, B, h->in_h, h->in_w, op.out.ptr, op.out.plane(), T, st));
+                CK(launch_stem(imgs, h->stem_w, h->stem_b, B, h->in_h, h->in_w, op.out.ptr, op.out.plane(), T, st, h->f16,
+                               h->sat_dev));
                 prof_mark(h, PK_STEM, st, "stem7x7");
                 break;
             case OP_S2D:
-                CK(launch_s2d(imgs, B, h->in_h, h->in_w, op.out.ptr, op.out.plane(), T, st));
+                CK(launch_s2d(imgs, B, h->in_h, h->in_w, op.out.ptr, op.out.plane(), T, st, h->f16, h->sat_dev));
                 prof_mark(h, PK_STEM, st, "s2d");
                 break;
             case OP_MAXPOOL:
-                CK(launch_maxpool(op.a.ptr, op.a.plane(), B, op.a.H, op.a.W, op.a.C, op.out.ptr, op.out.plane(), T, st));
+                CK(launch_maxpool(op.a.ptr, op.a.plane(), B, op.a.H, op.a.W, op.a.C, op.out.ptr, op.out.plane(), T, st,
+                                  h->f16));
                 prof_mark(h, PK_STEM, st, "maxpool");
                 break;
             case OP_CONV:
                 if (h->profiling && h->roles_dev && h->roles_used < ROLES_CAP) {
                     ConvParams cp = op.cp;  // same launch with the wait-cycle counters of every warp role switched on
                     cp.dbg = h->roles_dev + 16 * h->roles_used++;
-                    CK(launch_conv(cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl));
+                    CK(launch_conv(cp, op.block_n, h->nterms, h->f16, h->sm_count - h->sm_reserve, st, h->use_pdl));
                 } else {
-                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->sm_count - h->sm_reserve, st, h->use_pdl));
+                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->f16, h->sm_count - h->sm_reserve, st, h->use_pdl));
                 }
                 if (h->profiling) {
                     char d[160];
@@ -1125,7 +1148,7 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
                 break;
             case OP_UPADD:
                 CK(launch_upadd_relu(op.a.ptr, op.a.plane(), op.b.ptr, op.b.plane(), B, op.a.H, op.a.W, op.b.H, op.b.W,
-                                     op.a.C, op.out.ptr, op.out.plane(), T, st));
+                                     op.a.C, op.out.ptr, op.out.plane(), T, st, h->f16, h->sat_dev));
                 prof_mark(h, PK_ELEM, st, "upadd_relu");
                 break;
             case OP_TAPSUM: {
@@ -1190,7 +1213,7 @@ std::string debug_op_desc(const smapb_handle* h, const Op& op, const std::map<co
     } else {
         snprintf(buf, sizeof buf, " out=%dx%dx%dx%d nterms=%d", op.out.N, op.out.H, op.out.W, op.out.C, h->nterms);
     }
-    return s + buf;
+    return s + buf + (h->f16 ? " dtype=f16" : "");
 }
 
 }  // namespace
@@ -1250,6 +1273,8 @@ int smapb_create(smapb_handle** out, int device, int max_batch, int in_h, int in
     rc |= dev_alloc(h, &h->rootd, MB * hw);
     rc |= dev_alloc(h, &h->scales_dev, MB * SMAPB_SCALE_LEN);
     rc |= dev_alloc(h, &h->records_dev, MB);
+    rc |= dev_alloc(h, &h->sat_dev, 1);
+    if (!rc && cudaMemset(h->sat_dev, 0, sizeof(unsigned long long)) != cudaSuccess) rc = -10;
     if (rc) {
         g_create_error = h->err;
         delete h;
@@ -1306,7 +1331,7 @@ void smapb_destroy(smapb_handle* h) {
     cudaFree(h->stem_tc.bias_dev);
     void* ptrs[] = {h->peaks, h->scores, h->bodies, h->counts, h->imgs_dev, h->imgs_flip, h->hm, h->hm_flip, h->detd,
                     h->rootd, h->scratch_detd, h->scratch_rootd, h->scales_dev, h->records_dev, h->stem_w, h->stem_b,
-                    h->gather_dev, h->gt_dist, h->nms_masks};
+                    h->gather_dev, h->gt_dist, h->nms_masks, h->sat_dev};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (h->refine_buf) cudaFree(h->refine_buf);
@@ -1334,11 +1359,13 @@ int smapb_load_weight(smapb_handle* h, const char* key, const float* host, const
 
 int smapb_finalize_weights(smapb_handle* h, int precision) {
     if (!h) return -1;
-    if (precision != SMAPB_PREC_BF16X3 && precision != SMAPB_PREC_BF16) return fail(h, -1, "unknown precision");
+    if (precision != SMAPB_PREC_BF16X3 && precision != SMAPB_PREC_BF16 && precision != SMAPB_PREC_FP16)
+        return fail(h, -1, "unknown precision");
     cudaSetDevice(h->device);
     // a new weight set invalidates cached plans (they hold tensor maps over the old weight buffers only if
     // buffers are re-allocated; buffers are reused in place, but the plane count may change)
     const int new_planes = precision == SMAPB_PREC_BF16X3 ? 2 : 1;
+    h->finalized = false;
     for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
     h->graphs.clear();
     h->eager_runs.clear();
@@ -1356,8 +1383,9 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
         h->stem_tc.w_dev = nullptr;
         h->stem_tc.bias_dev = nullptr;
     }
-    h->nterms = precision;
+    h->nterms = precision == SMAPB_PREC_BF16X3 ? 3 : 1;
     h->planes = new_planes;
+    h->f16 = precision == SMAPB_PREC_FP16;
     // unit names: every "<name>.conv.weight" key
     std::vector<std::string> units;
     for (auto& kv : h->raw) {
@@ -1398,6 +1426,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
                 S.name = "top.conv(s2d)";
                 S.Cin = 64, S.Cout = 64, S.Cout_pad = 64, S.k = 1, S.stride = 1, S.pad = 0, S.stem_s2d = true;
                 const size_t plane = (size_t)4 * 64 * 64;
+                if (h->f16 && check_f16_range(h, name, wf.data(), wf.size())) return -42;
                 std::vector<uint16_t> host(plane * h->planes, 0);
                 for (int co = 0; co < 64; co++)
                     for (int ay = 0; ay < 4; ay++)
@@ -1408,7 +1437,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
                                         const int ky = 2 * ay + by - 1, kx = 2 * ax + bx - 1;
                                         if (ky < 0 || ky > 6 || kx < 0 || kx > 6) continue;
                                         const float v = wf[((co * 3 + c) * 7 + ky) * 7 + kx];
-                                        const uint16_t hi = f32_to_bf16_rn(v);
+                                        const uint16_t hi = h->f16 ? f32_to_f16_rn(v) : f32_to_bf16_rn(v);
                                         const size_t o = ((size_t)ay * 64 + co) * 64 + ax * 16 + (by * 2 + bx) * 3 + c;
                                         host[o] = hi;
                                         if (h->planes == 2) host[plane + o] = f32_to_bf16_rn(v - bf16_to_f32(hi));
@@ -2271,6 +2300,16 @@ int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int 
 
 int64_t smapb_launch_count(const smapb_handle* h) { return h ? h->launches : 0; }
 
+int64_t smapb_saturation_count(smapb_handle* h, int reset) {
+    if (!h) return -1;
+    cudaSetDevice(h->device);
+    CK(cudaDeviceSynchronize());  // the handle's work runs on non-blocking streams
+    unsigned long long n = 0;
+    CK(cudaMemcpy(&n, h->sat_dev, sizeof n, cudaMemcpyDeviceToHost));
+    if (reset) CK(cudaMemset(h->sat_dev, 0, sizeof n));
+    return (int64_t)n;
+}
+
 int smapb_profile_begin(smapb_handle* h) {
     if (!h) return -1;
     h->profiling = true;
@@ -2345,11 +2384,15 @@ int smapb_plan_info(const smapb_handle* hc, int B, int* n_conv, double* conv_flo
     return 0;
 }
 
-// split-bf16 planes -> fp32 (test hook)
+// split-bf16 planes (or the fp16 plane, f16 != 0) -> fp32 (test hook)
 __global__ void split_to_f32_kernel(const __nv_bfloat16* __restrict__ in, long long plane, int terms, float* __restrict__ out,
-                                    long long n) {
+                                    long long n, int f16) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (f16) {
+        out[i] = __half2float(reinterpret_cast<const __half*>(in)[i]);
+        return;
+    }
     float v = __bfloat162float(in[i]);
     if (terms == 2) v += __bfloat162float(in[plane + i]);
     out[i] = v;
@@ -2361,9 +2404,13 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     if (!h) return -1;
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
+    if (precision != SMAPB_PREC_BF16X3 && precision != SMAPB_PREC_BF16 && precision != SMAPB_PREC_FP16)
+        return fail(h, -1, "smapb_conv_test: unknown precision");
     const int save_terms = h->nterms, save_planes = h->planes;
-    h->nterms = precision == SMAPB_PREC_BF16 ? 1 : 3;
-    h->planes = precision == SMAPB_PREC_BF16 ? 1 : 2;
+    const bool save_f16 = h->f16;
+    h->nterms = precision == SMAPB_PREC_BF16X3 ? 3 : 1;
+    h->planes = precision == SMAPB_PREC_BF16X3 ? 2 : 1;
+    h->f16 = precision == SMAPB_PREC_FP16;
     int rc = 0;
     ConvLayer L;
     L.name = "conv_test";
@@ -2376,6 +2423,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         cudaFree(L.bias_dev);
         h->nterms = save_terms;
         h->planes = save_planes;
+        h->f16 = save_f16;
     };
 #define CKT(call)                                                                         \
     do {                                                                                  \
@@ -2407,7 +2455,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     tmp.push_back(p);
     out.ptr = (__nv_bfloat16*)p;
     CKT(cudaMemset(p, 0, (size_t)out.plane() * 2 * h->planes));  // TMA stores are invisible to initcheck
-    CKT(launch_f32_to_split(x, in.ptr, in.plane(), in.plane(), h->planes, st));
+    CKT(launch_f32_to_split(x, in.ptr, in.plane(), in.plane(), h->planes, st, h->f16));
     const float* extra_src[3] = {res, post1, post2};
     Act* extra_act[3] = {&r, &p1, &p2};
     for (int e = 0; e < 3; e++) {
@@ -2419,7 +2467,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         CKT(cudaMalloc(&p, (size_t)out.plane() * 2 * h->planes));
         tmp.push_back(p);
         extra_act[e]->ptr = (__nv_bfloat16*)p;
-        CKT(launch_f32_to_split(extra_src[e], extra_act[e]->ptr, out.plane(), out.plane(), h->planes, st));
+        CKT(launch_f32_to_split(extra_src[e], extra_act[e]->ptr, out.plane(), out.plane(), h->planes, st, h->f16));
     }
     ConvParams cp;
     int bn = 0;
@@ -2444,7 +2492,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         CKT(cudaMalloc((void**)&tl_dev, 16 * sizeof(long long)));
         tmp.push_back(tl_dev);
     }
-    CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));  // warm-up + result
+    CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));  // warm-up + result
     if (dbg_dev) {
         long long d[16];
         CKT(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));
@@ -2464,7 +2512,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     if (tl_dev) {  // time line of CTA 0 of one warm launch (cycles since kernel entry)
         CKT(cudaMemset(tl_dev, 0, 16 * sizeof(long long)));
         cp.dbg_tl = tl_dev;
-        CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));
+        CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));
         cp.dbg_tl = nullptr;
         long long t[16];
         CKT(cudaMemcpy(t, tl_dev, sizeof t, cudaMemcpyDeviceToHost));
@@ -2474,7 +2522,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     }
     const int reps = ms_out ? 5 : 0;
     cudaEventRecord(e0, st);
-    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->sm_count, st, false));
+    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));
     cudaEventRecord(e1, st);
     h->launches += 1 + reps;
     // de-pad + convert
@@ -2482,7 +2530,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     CKT(cudaMalloc((void**)&ytmp, (size_t)out.plane() * 4));
     tmp.push_back(ytmp);
     split_to_f32_kernel<<<(unsigned)((out.plane() + 255) / 256), 256, 0, st>>>(out.ptr, out.plane(), h->planes, ytmp,
-                                                                               out.plane());
+                                                                               out.plane(), h->f16);
     CKT(cudaGetLastError());
     CKT(cudaMemcpy2DAsync(y, (size_t)Cout * 4, ytmp, (size_t)L.Cout_pad * 4, (size_t)Cout * 4, (size_t)B * Ho * Wo,
                           cudaMemcpyDeviceToDevice, st));

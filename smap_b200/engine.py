@@ -8,13 +8,15 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import MAXP, NC2D, NJ, NL, PREC_BF16, PREC_BF16X3, RECORD_BYTES, SCALE_LEN, SmapB200Error
+from ._lib import MAXP, NC2D, NJ, NL, PREC_BF16, PREC_BF16X3, PREC_FP16, RECORD_BYTES, SCALE_LEN, SmapB200Error
 
 RECORD_DTYPE = np.dtype([("pred3d", "<f8", (MAXP, NJ, 4)), ("root_depth", "<f8", (MAXP,)),
                          ("pred2d", "<f4", (MAXP, NJ, 4)), ("count", "<i4"), ("pad_", "<i4")])
 assert RECORD_DTYPE.itemsize == RECORD_BYTES
 
-PRECISIONS = {"bf16x3": PREC_BF16X3, "bf16": PREC_BF16}
+# bf16x3: fp32-faithful (split-bf16 operands, 3 MMAs); fp16: the cost of bf16 with 4x finer rounding, range +-65504
+# (Engine.saturation_count); bf16: the cost of fp16 with fp32's range and 8-bit mantissa
+PRECISIONS = {"bf16x3": PREC_BF16X3, "fp16": PREC_FP16, "bf16": PREC_BF16}
 
 
 def scale_row(scale):
@@ -330,6 +332,14 @@ class Engine:
     # ---- introspection ------------------------------------------------------------------------
     def launch_count(self):
         return int(self.lib.smapb_launch_count(self._h))
+
+    def saturation_count(self, reset=False):
+        """fp16 precision: activation elements clamped to +-65504 since creation (or the last reset=True); synchronises the
+        device.  Nonzero means some outputs are not the model's: use precision "bf16x3" (or "bf16") for such inputs."""
+        n = self.lib.smapb_saturation_count(self._h, int(bool(reset)))
+        if n < 0:
+            raise SmapB200Error("smapb_saturation_count failed (%d): %s" % (n, self.lib.smapb_last_error(self._h).decode()))
+        return int(n)
 
     def profile_begin(self):
         self._check(self.lib.smapb_profile_begin(self._h), "smapb_profile_begin")

@@ -2,7 +2,7 @@
 path: images on disk -> result JSON.
 
     python -m smap_b200.run_inference -p SMAP.pth [-rp RefineNet.pth] --dataset_path DIR --batch_size 8 --do_flip 1 \
-        [--json_name SUFFIX] [--output_dir OUT] [--dataset_name CMU]
+        [--json_name SUFFIX] [--output_dir OUT] [--dataset_name CMU] [--precision {bf16x3,fp16,bf16}]
 
 Same flags and the same output file name / schema as the reference ('{OUT}/stage3_root2_run_inference_{data_mode}_{suffix}.json',
 test.py:147-152).  Differences, both deliberate: images are visited in sorted path order unless --glob_order 1 (the
@@ -17,7 +17,7 @@ import os.path as osp
 import numpy as np
 import torch
 
-from .engine import RECORD_BYTES, Engine
+from .engine import PRECISIONS, RECORD_BYTES, Engine
 from .results import ResultWriter, result_file_name
 
 
@@ -37,8 +37,11 @@ def image_name(path, dataset_path):
 
 
 def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False, dataset_name="CMU",
-        device=0, in_h=512, in_w=832, imread=None, glob_order=False):
-    """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3]; defaults to cv2.imread(path, IMREAD_COLOR)."""
+        device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None):
+    """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3]; defaults to cv2.imread(path, IMREAD_COLOR).
+    precision: one of engine.PRECISIONS.  stats (a dict, optional) receives "saturation": the fp16 clamp count."""
+    if precision not in PRECISIONS:
+        raise ValueError("unknown precision %r (choose from %s)" % (precision, ", ".join(PRECISIONS)))
     if imread is None:
         import cv2
 
@@ -50,7 +53,7 @@ def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batc
 
     eng = Engine(device, max_batch=batch_size, in_h=in_h, in_w=in_w)
     try:
-        eng.load_state_dict(smap_state_dict)
+        eng.load_state_dict(smap_state_dict, precision)
         if refine_state_dict is not None:
             eng.load_refine_state_dict(refine_state_dict)
             eng.set_refine(True)
@@ -65,6 +68,8 @@ def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batc
                 host[:len(chunk)].copy_(rec)
                 torch.cuda.current_stream().synchronize()
                 w.append(host[:len(chunk)], [image_name(p, dataset_path) for p in chunk])
+        if stats is not None:
+            stats["saturation"] = eng.saturation_count()
         return len(paths)
     finally:
         eng.close()
@@ -85,6 +90,9 @@ def main(argv=None):
     ap.add_argument("--output_dir", default="model_logs/stage3_root2/result")
     ap.add_argument("--dataset_name", default="CMU", help="cfg.DATASET.NAME written as 'model_pattern'")
     ap.add_argument("--glob_order", type=int, default=0, help="1: visit images in the reference's glob order instead of sorted")
+    ap.add_argument("--precision", default="bf16x3", choices=list(PRECISIONS),
+                    help="convolution precision: bf16x3 (fp32-faithful), fp16 (cost of bf16, 4x finer rounding, range "
+                         "+-65504) or bf16 (8-bit mantissa, fp32 range)")
     a = ap.parse_args(argv)
     if not os.path.exists(a.SMAP_path):
         print("No such checkpoint of SMAP {}".format(a.SMAP_path))  # test.py:222
@@ -98,8 +106,13 @@ def main(argv=None):
         rsd = torch.load(a.RefineNet_path, map_location="cpu")         # test.py:214
     os.makedirs(a.output_dir, exist_ok=True)
     out = result_file_name(a.output_dir, a.test_mode, a.data_mode, a.json_name)
-    n = run(sd, a.dataset_path, out, rsd, a.batch_size, a.do_flip, a.dataset_name, glob_order=bool(a.glob_order))
+    stats = {}
+    n = run(sd, a.dataset_path, out, rsd, a.batch_size, a.do_flip, a.dataset_name, glob_order=bool(a.glob_order),
+            precision=a.precision, stats=stats)
     print("Pairs writed to {} ({} images)".format(out, n))             # test.py:152
+    if stats.get("saturation"):
+        print("fp16: {} activation values exceeded +-65504 and were clamped; rerun with --precision bf16x3 (or bf16) "
+              "for exact results".format(stats["saturation"]))
     return 0
 
 
