@@ -215,7 +215,9 @@ int smapb_json_close(smapb_json_writer* w);
 /* number of kernels launched by this handle since creation */
 int64_t smapb_launch_count(const smapb_handle* h);
 /* SMAPB_PREC_FP16: number of activation elements this handle's kernels clamped to +-65504 since creation (or the last
- * reset != 0, which zeroes the counter after reading it); 0 in the bf16 precisions.  Synchronises the device.  Any nonzero
+ * reset != 0, which zeroes the counter after reading it); 0 in the bf16 precisions.  Every forward (eager, graph replay,
+ * each half of a flip pass, a profiled run) and each smapb_conv_test call adds its clamps once; the autotuner's trial
+ * launches at plan build and smapb_conv_test's timed re-runs add nothing.  Synchronises the device.  Any nonzero
  * count means some layer produced values fp16 cannot hold and those outputs are not the model's: run such inputs (or
  * weights) with SMAPB_PREC_BF16X3, or SMAPB_PREC_BF16 when speed matters more than the last digits.  < 0: error. */
 int64_t smapb_saturation_count(smapb_handle* h, int reset);

@@ -822,6 +822,9 @@ struct PlanBuilder {
                 int rc2 = setup_conv(h, L, in, res, p1, p2, out, nullptr, relu, &trial.cp, &trial.block_n, &trial.flops, in2,
                                      up, &trial.cg, c[0], c[1]);
                 if (rc2) continue;
+                // trial launches run on the plan's zero-filled activations (output = bias): their clamps are not the
+                // user's, so they stay out of the saturation counter (the kernel still clamps)
+                trial.cp.sat = nullptr;
                 float ms_best_c = 1e30f;
                 for (int rep = 0; rep < 4; rep++) {
                     cudaEventRecord(e0, nullptr);
@@ -2493,6 +2496,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         tmp.push_back(tl_dev);
     }
     CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));  // warm-up + result
+    cp.sat = nullptr;  // the saturation counter counts the result launch; the time-line and timed re-runs leave it alone
     if (dbg_dev) {
         long long d[16];
         CKT(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));

@@ -359,19 +359,20 @@ def _consumers(ops):
     return uses
 
 
-def check_plan(precision, H, W, B, eng=None):
+def check_plan(precision, H, W, B, eng=None, sd=None):
     """Run the plan twice (different images), then check every dumped op of the second run against its reference.
     Returns a summary: worst error per op class, the op descriptions, and which wrong references were flagged.  Each
     wrong reference is tried on the first op of its class where it differs from the right one.
-    eng: an existing handle (max_batch >= B, make_state_dict(SEED, "random") loaded in `precision`), left open; by
-    default a handle with max_batch == B is created and closed."""
+    eng: an existing handle (max_batch >= B, the state dict loaded in `precision`), left open; by default a handle with
+    max_batch == B is created and closed.  sd: the state dict (default make_state_dict(SEED, "random"))."""
     from smap_b200.engine import Engine
 
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     t0 = time.time()
     print("\n[plan ops %s %dx%d B=%d%s]" % (precision, H, W, B, "" if eng is None else " max_batch=%d" % eng.max_batch))
-    sd = smap_torch.make_state_dict(SEED, "random")
+    if sd is None:
+        sd = smap_torch.make_state_dict(SEED, "random")
     own = eng is None
     if own:
         eng = Engine(0, max_batch=B, in_h=H, in_w=W)
