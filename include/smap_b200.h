@@ -67,6 +67,33 @@ int smapb_preprocess(smapb_handle* h, const uint8_t* bgr_dev, int img_h, int img
 int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, int img_w, float* out_nchw_dev,
                           double* scale_row_host, void* stream);
 
+/* ---- JPEG decoding (the step in front of pre-processing) ------------------------------------------------------------- */
+/* Replaces: cv2.imread(path, IMREAD_COLOR) (dataset/custom_dataset.py:27) for the JPEGs it can decode, byte for byte:
+ * baseline / extended-sequential Huffman (SOF0/SOF1), 8-bit samples, 8- or 16-bit DQT, any DHT (optimised tables too),
+ * DRI restart intervals, one interleaved scan of every component, grayscale (replicated to BGR) or 3 components libjpeg
+ * treats as YCbCr, luma sampling H, V in {1, 2} with chroma 1x1 (4:4:4, 4:2:2, 4:4:0, 4:2:0), EXIF orientation 1..8 applied
+ * as cv2 applies it, up to SMAPB_JPEG_MAX_PIXELS.  Everything else (progressive, arithmetic, 12-bit, lossless, CMYK, RGB,
+ * other sampling, several scans, non-JPEG data, truncated or corrupt data) gets a status != SMAPB_JPEG_OK and is meant for
+ * cv2.imread. */
+#define SMAPB_JPEG_OK 0
+#define SMAPB_JPEG_UNSUPPORTED 1 /* a JPEG (or a block of one) this decoder does not handle */
+#define SMAPB_JPEG_MALFORMED 2   /* not a JPEG, or a header that does not parse */
+#define SMAPB_JPEG_CORRUPT 3     /* entropy-coded data that does not decode to the frame's blocks */
+#define SMAPB_JPEG_TOO_LARGE 4   /* over SMAPB_JPEG_MAX_PIXELS */
+#define SMAPB_JPEG_MAX_PIXELS (1 << 26)
+/* Host only (no GPU work): header walk of one file.  *status = SMAPB_JPEG_*; when it is SMAPB_JPEG_OK, *h x *w is the shape
+ * cv2.imread returns (after the EXIF orientation) and *orientation the EXIF value (1 without one); zeros otherwise.
+ * Returns 0, or -1 for a NULL status. */
+int smapb_jpeg_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* orientation, int* status);
+/* Decodes n files (host memory) into bgr_dev[i]: uint8 [h, w, 3] BGR as smapb_jpeg_info reports the shape, which
+ * smapb_preprocess consumes.  bgr_dev[i] may be NULL only for files smapb_jpeg_info does not accept.  status_host[i]
+ * (SMAPB_JPEG_*) says whether bgr_dev[i] holds the image; the header status can turn into SMAPB_JPEG_CORRUPT or
+ * SMAPB_JPEG_UNSUPPORTED once the data is decoded.  Each phase is one launch for the whole batch.  The workspace is owned
+ * by the handle and grows on demand; the call synchronises `stream` and returns once status_host is known, so it cannot be
+ * captured into a CUDA graph. */
+int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                      int* status_host, void* stream);
+
 /* ---- backbone -------------------------------------------------------------------------------- */
 /* Replaces: SMAP.forward inference branch (model/smap.py:403-419).
  * imgs_nchw_dev: fp32 [B,3,in_h,in_w] (normalised BGR).  Outputs fp32 NCHW:

@@ -20,6 +20,7 @@
 #include "assoc.h"
 #include "conv_tc.cuh"
 #include "elementwise.h"
+#include "jpeg.h"
 #include "preprocess.h"
 #include "refine.h"
 
@@ -219,6 +220,7 @@ struct smapb_handle {
     std::map<std::pair<int, int>, PreEntry> pre_cache;
     uint8_t* pre_stage = nullptr;
     size_t pre_stage_bytes = 0;
+    smapb::JpegWorkspace* jpeg = nullptr;  // JPEG decoding (smapb_decode_jpeg), created on first use
     // RefineNet (optional post-processing step, SURVEY 8(f) f2)
     std::map<std::string, std::vector<float>> refine_raw;
     float* refine_buf = nullptr;  // folded, transposed weights + biases of the five layers
@@ -1341,6 +1343,7 @@ void smapb_destroy(smapb_handle* h) {
     if (h->roles_dev) cudaFree(h->roles_dev);
     if (h->pre_stage) cudaFree(h->pre_stage);
     for (auto& e : h->pre_cache) cudaFree(e.second.buf);
+    smapb::jpeg_workspace_destroy(h->jpeg);
     delete h;
 }
 
@@ -1698,6 +1701,14 @@ int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, i
     }
     CK(cudaMemcpyAsync(h->pre_stage, bgr_host, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return smapb_preprocess(h, h->pre_stage, img_h, img_w, out_nchw_dev, scale_row_host, stream);
+}
+
+int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                      int* status_host, void* stream) {
+    if (!h) return -1;
+    cudaSetDevice(h->device);
+    if (!h->jpeg) h->jpeg = smapb::jpeg_workspace_create();
+    return smapb::jpeg_decode(h->jpeg, n, jpeg_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
 }
 
 // host-only introspection of the resampling plan (tests compare it with the oracle over many geometries without a GPU)

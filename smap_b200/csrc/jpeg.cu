@@ -1,0 +1,1043 @@
+// Baseline (SOF0/SOF1, Huffman, 8-bit) JPEG decoding on the GPU, byte-identical to cv2.imread(path, IMREAD_COLOR).
+//
+// Host: a bounds-checked marker walk (jpeg_parse) builds the Huffman and quantisation tables, the restart segments and the
+// EXIF orientation; anything it does not accept gets a status and is left to the caller's cv2 path.  Device: one launch
+// per phase for every image of the batch:
+//   a. unstuff_kernel     removes the FF00 stuffing and the RSTn markers (restart segments are byte ranges the host found)
+//   b. huff_sync_kernel   self-synchronising Huffman decoding (Weissenberger & Schmidt, ICPP 2018 / HiPC 2021): every
+//                         segment is cut into SUB_BITS-bit subsequences, each decoded speculatively from a guessed state;
+//                         sync passes restart a subsequence from its predecessor's exit state until every start state
+//                         equals its predecessor's exit state (the state: bit position, block within the MCU, zig-zag index)
+//      huff_prefix_kernel prefix sum of the blocks each subsequence completes -> output positions; per-segment checks
+//      huff_write_kernel  the final pass: coefficients into their blocks (DC as differences)
+//      dc_scan_kernel     DC prediction: a scan per component, reset at every restart
+//   c. idct_kernel        dequantisation + accurate-integer IDCT (LL&M, 13-bit constants, 2 pass-1 bits), saturated
+//   d. colour_kernel      fancy upsampling, fixed-point YCbCr -> BGR, EXIF orientation, uint8 HWC BGR
+// oracle/jpeg_numpy.py restates every stage on the CPU.
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "../../include/smap_b200.h"
+#include "jpeg.h"
+
+namespace smapb {
+namespace {
+
+constexpr int SUB_BITS = 512;    // subsequence length of the parallel Huffman decoder
+constexpr int WARM_BITS = 1024; // speculative decoding that precedes a subsequence in the first pass
+constexpr int PASS_GROUP = 8;    // sync passes launched between two convergence checks on the host
+constexpr int GUARD = 8191;      // 16-bit-lane bound of cv2's IDCT (see idct_kernel)
+constexpr int MAX_SCAN_BYTES = 1 << 28;  // bit positions are 32-bit
+
+__constant__ uint8_t c_zigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                     41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                     30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+const uint8_t h_zigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                              41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                              30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+struct DevHuff {
+    uint16_t fast[512];  // next 9 bits -> len << 8 | symbol; 0 = the code is longer (or invalid)
+    int32_t maxcode[17];  // largest code of each length 10..16, -1 = none
+    int32_t valoff[17];   // vals index of a code of that length = valoff[len] + code
+    uint8_t vals[256];
+};
+
+struct DevImage {
+    int h, w, out_h, out_w, orientation, ncomp, hmax, vmax, mcux, mcuy, nmcu, bpm, per, nseg;
+    int seg0, sub0, nsub;
+    int blk_comp[6], blk_dx[6], blk_dy[6];
+    int comp_h[3], comp_v[3];
+    int plane_w[3], plane_h[3];
+    int64_t raw_off, raw_len, unst_off, coef_off, plane_off[3];
+    uint8_t* out;
+    int16_t qt[3][64];  // natural order (values > 32767 are rejected on the host)
+    DevHuff dc[3], ac[3];
+};
+
+struct DevSeg {
+    int img, sub0, nsub, first_mcu, nmcu;
+    uint32_t bit_begin, bit_end;  // relative to the image's unstuffed data
+};
+
+struct DevSub {
+    int img, seg;
+    uint32_t bit_begin, bit_end;
+};
+
+struct SubState {
+    unsigned long long start, exit;  // packed decoder states
+    int nblk;                        // blocks completed in this subsequence
+    int errblk;                      // blocks completed before its first error, INT_MAX = none
+};
+
+// packed decoder state: bit position | block within the MCU << 32 | zig-zag index << 40
+__host__ __device__ inline unsigned long long pack_state(uint32_t pos, int blk, int zz) {
+    return (unsigned long long)pos | ((unsigned long long)blk << 32) | ((unsigned long long)zz << 40);
+}
+
+// ---- host parser -----------------------------------------------------------------------------------------------------
+struct HuffSpec {
+    uint8_t counts[16];
+    uint8_t vals[256];
+    int nvals = 0;
+    bool defined = false;
+};
+
+struct Header {
+    int h = 0, w = 0, out_h = 0, out_w = 0, orientation = 1, ncomp = 0, hmax = 1, vmax = 1, mcux = 0, mcuy = 0, nmcu = 0;
+    int dri = 0;
+    int comp_h[3] = {1, 1, 1}, comp_v[3] = {1, 1, 1};
+    uint16_t qt[3][64];
+    const HuffSpec* dc[3];
+    const HuffSpec* ac[3];
+    HuffSpec dht[2][4];
+    std::vector<int64_t> seg_begin, seg_end;  // raw byte ranges of the restart segments
+    std::vector<int64_t> seg_stuffed;         // FF00 pairs inside each segment
+};
+
+inline int u16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
+
+// EXIF orientation from an APP1 payload: 0 = not an EXIF block, 1..8, -1 = an orientation cv2 might read otherwise
+int exif_orientation(const uint8_t* s, int64_t len) {
+    if (len < 6 || memcmp(s, "Exif\0\0", 6) != 0) return 0;
+    const uint8_t* t = s + 6;
+    const int64_t n = len - 6;
+    if (n < 8) return -1;
+    bool le;
+    if (memcmp(t, "II*\0", 4) == 0) le = true;
+    else if (memcmp(t, "MM\0*", 4) == 0) le = false;
+    else return -1;
+    auto rd = [&](int64_t i, int k, bool* ok) -> uint32_t {
+        if (i < 0 || i + k > n) {
+            *ok = false;
+            return 0;
+        }
+        uint32_t v = 0;
+        for (int j = 0; j < k; j++) v |= (uint32_t)t[i + j] << (8 * (le ? j : k - 1 - j));
+        return v;
+    };
+    bool ok = true;
+    const int64_t ifd = rd(4, 4, &ok);
+    const int cnt = (int)rd(ifd, 2, &ok);
+    if (!ok) return -1;
+    for (int e = 0; e < cnt; e++) {
+        const int64_t p = ifd + 2 + 12 * (int64_t)e;
+        const uint32_t tag = rd(p, 2, &ok);
+        if (!ok) return -1;
+        if (tag == 0x0112) {
+            const uint32_t typ = rd(p + 2, 2, &ok), c = rd(p + 4, 4, &ok), v = rd(p + 8, 2, &ok);
+            if (!ok || typ != 3 || c != 1 || v < 1 || v > 8) return -1;
+            return (int)v;
+        }
+    }
+    return 1;
+}
+
+// Validates a Huffman table (canonical codes must fit their lengths) and fills the device form.
+bool build_huff(const HuffSpec& s, DevHuff* d) {
+    memset(d, 0, sizeof(*d));
+    int code = 0, k = 0;
+    for (int l = 1; l <= 16; l++) {
+        d->valoff[l] = k - code;
+        for (int i = 0; i < s.counts[l - 1]; i++) {
+            if (code >= (1 << l)) return false;
+            if (l <= 9)
+                for (int j = 0; j < (1 << (9 - l)); j++) d->fast[(code << (9 - l)) + j] = (uint16_t)((l << 8) | s.vals[k]);
+            code++, k++;
+        }
+        d->maxcode[l] = s.counts[l - 1] ? code - 1 : -1;
+        code <<= 1;
+    }
+    memcpy(d->vals, s.vals, 256);
+    return true;
+}
+
+int jpeg_parse(const uint8_t* d, int64_t n, Header* H) {
+    if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return SMAPB_JPEG_MALFORMED;
+    int64_t p = 2;
+    const uint8_t* qt[4] = {nullptr, nullptr, nullptr, nullptr};
+    int qprec[4] = {0, 0, 0, 0};
+    bool sof = false, jfif = false, adobe = false, have_orient = false;
+    int adobe_transform = 0, ids[3] = {0, 0, 0}, tq[3] = {0, 0, 0};
+    const uint8_t* s = nullptr;
+    int64_t L = 0;
+    for (;;) {
+        if (p + 2 > n || d[p] != 0xFF) return SMAPB_JPEG_MALFORMED;
+        while (p + 1 < n && d[p + 1] == 0xFF) p++;
+        if (p + 2 > n) return SMAPB_JPEG_MALFORMED;
+        const int m = d[p + 1];
+        p += 2;
+        if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SMAPB_JPEG_MALFORMED;
+        if (p + 2 > n) return SMAPB_JPEG_MALFORMED;
+        L = u16(d + p);
+        if (L < 2 || p + L > n) return SMAPB_JPEG_MALFORMED;
+        s = d + p + 2;
+        L -= 2;
+        p += L + 2;
+        if (m == 0xDB) {
+            for (int64_t i = 0; i < L;) {
+                const int pq = s[i] >> 4, t = s[i] & 15;
+                if (pq > 1 || t > 3 || i + 1 + 64 * (pq + 1) > L) return SMAPB_JPEG_MALFORMED;
+                qt[t] = s + i + 1;
+                qprec[t] = pq;
+                i += 1 + 64 * (pq + 1);
+            }
+        } else if (m == 0xC4) {
+            for (int64_t i = 0; i < L;) {
+                if (i + 17 > L) return SMAPB_JPEG_MALFORMED;
+                const int tc = s[i] >> 4, th = s[i] & 15;
+                int tot = 0;
+                for (int j = 0; j < 16; j++) tot += s[i + 1 + j];
+                if (tc > 1 || th > 3 || tot > 256 || i + 17 + tot > L) return SMAPB_JPEG_MALFORMED;
+                HuffSpec& hs = H->dht[tc][th];
+                memcpy(hs.counts, s + i + 1, 16);
+                memset(hs.vals, 0, 256);
+                memcpy(hs.vals, s + i + 17, tot);
+                hs.nvals = tot;
+                hs.defined = true;
+                i += 17 + tot;
+            }
+        } else if (m == 0xDD) {
+            if (L != 2) return SMAPB_JPEG_MALFORMED;
+            H->dri = u16(s);
+        } else if (m == 0xC0 || m == 0xC1) {
+            if (sof || L < 6) return SMAPB_JPEG_MALFORMED;
+            sof = true;
+            const int prec = s[0], nf = s[5];
+            H->h = u16(s + 1), H->w = u16(s + 3);
+            if (L != 6 + 3 * nf) return SMAPB_JPEG_MALFORMED;
+            if (prec != 8 || H->h == 0 || H->w == 0 || (nf != 1 && nf != 3)) return SMAPB_JPEG_UNSUPPORTED;
+            H->ncomp = nf;
+            for (int c = 0; c < nf; c++) {
+                ids[c] = s[6 + 3 * c];
+                H->comp_h[c] = s[7 + 3 * c] >> 4;
+                H->comp_v[c] = s[7 + 3 * c] & 15;
+                tq[c] = s[8 + 3 * c];
+                if (tq[c] > 3) return SMAPB_JPEG_MALFORMED;
+                for (int e = 0; e < c; e++)
+                    if (ids[e] == ids[c]) return SMAPB_JPEG_MALFORMED;
+            }
+            if (nf == 1) {
+                H->comp_h[0] = H->comp_v[0] = 1;  // one component: one block per MCU whatever its factors say
+            } else {
+                const bool ok = (H->comp_h[0] == 1 || H->comp_h[0] == 2) && (H->comp_v[0] == 1 || H->comp_v[0] == 2) &&
+                                H->comp_h[1] == 1 && H->comp_v[1] == 1 && H->comp_h[2] == 1 && H->comp_v[2] == 1;
+                if (!ok) return SMAPB_JPEG_UNSUPPORTED;
+            }
+        } else if (m >= 0xC2 && m <= 0xCF) {
+            return SMAPB_JPEG_UNSUPPORTED;  // progressive, lossless, arithmetic, hierarchical, DAC, JPG
+        } else if (m == 0xE0) {
+            if (L >= 14 && memcmp(s, "JFIF\0", 5) == 0) jfif = true;
+        } else if (m == 0xEE) {
+            if (L >= 12 && memcmp(s, "Adobe", 5) == 0) adobe = true, adobe_transform = s[11];
+        } else if (m == 0xE1) {
+            const int o = exif_orientation(s, L);
+            if (o < 0) return SMAPB_JPEG_UNSUPPORTED;
+            if (o > 0) {
+                if (have_orient) return SMAPB_JPEG_UNSUPPORTED;
+                have_orient = true;
+                H->orientation = o;
+            }
+        } else if ((m >= 0xE2 && m <= 0xEF) || m == 0xFE) {
+        } else if (m == 0xDA) {
+            break;
+        } else {
+            return SMAPB_JPEG_UNSUPPORTED;
+        }
+    }
+    // SOS: one interleaved scan of every component, in frame order, sequential parameters
+    if (!sof) return SMAPB_JPEG_MALFORMED;
+    const int nf = H->ncomp;
+    if (L < 1 || s[0] != nf || L != 4 + 2 * nf) return SMAPB_JPEG_UNSUPPORTED;
+    for (int c = 0; c < nf; c++) {
+        if (s[1 + 2 * c] != ids[c]) return SMAPB_JPEG_UNSUPPORTED;
+        const int td = s[2 + 2 * c] >> 4, ta = s[2 + 2 * c] & 15;
+        if (td > 3 || ta > 3 || !H->dht[0][td].defined || !H->dht[1][ta].defined || !qt[tq[c]]) return SMAPB_JPEG_UNSUPPORTED;
+        const HuffSpec& dcs = H->dht[0][td];
+        for (int i = 0; i < dcs.nvals; i++)
+            if (dcs.vals[i] > 15) return SMAPB_JPEG_MALFORMED;
+        H->dc[c] = &H->dht[0][td];
+        H->ac[c] = &H->dht[1][ta];
+        for (int k = 0; k < 64; k++) {
+            const uint8_t* q = qt[tq[c]];
+            const int v = qprec[tq[c]] ? u16(q + 2 * k) : q[k];
+            if (v > 32767) return SMAPB_JPEG_UNSUPPORTED;
+            H->qt[c][h_zigzag[k]] = (uint16_t)v;
+        }
+    }
+    if (s[1 + 2 * nf] != 0 || s[2 + 2 * nf] != 63 || s[3 + 2 * nf] != 0) return SMAPB_JPEG_UNSUPPORTED;
+    if (nf == 3) {
+        // libjpeg's colour-space rule for 3 components: a JFIF APP0 means YCbCr; else an Adobe APP14 means RGB when its
+        // transform flag is 0 and YCbCr otherwise; else component ids 'R','G','B' mean RGB, anything else YCbCr
+        bool ycc;
+        if (jfif) ycc = true;
+        else if (adobe) ycc = adobe_transform != 0;
+        else ycc = !(ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B');
+        if (!ycc) return SMAPB_JPEG_UNSUPPORTED;
+    }
+    if ((int64_t)H->h * H->w > SMAPB_JPEG_MAX_PIXELS) return SMAPB_JPEG_TOO_LARGE;
+    H->hmax = H->comp_h[0], H->vmax = H->comp_v[0];
+    H->mcux = (H->w + 8 * H->hmax - 1) / (8 * H->hmax);
+    H->mcuy = (H->h + 8 * H->vmax - 1) / (8 * H->vmax);
+    H->nmcu = H->mcux * H->mcuy;
+    const int nseg = H->dri ? (H->nmcu + H->dri - 1) / H->dri : 1;
+    // entropy-coded data: FF00 = stuffed FF, FFD0..D7 = restart marker in sequence, FFD9 = end; anything else is refused
+    int64_t start = p, q = p, stuffed = 0;
+    for (;;) {
+        const uint8_t* f = (const uint8_t*)memchr(d + q, 0xFF, (size_t)(n - q));
+        if (!f || f + 1 >= d + n) return SMAPB_JPEG_MALFORMED;
+        q = f - d;
+        const int m = d[q + 1];
+        if (m == 0) {
+            stuffed++;
+            q += 2;
+            continue;
+        }
+        if (m >= 0xD0 && m <= 0xD7) {
+            if (!H->dri || m - 0xD0 != (int)(H->seg_begin.size() % 8) || (int)H->seg_begin.size() + 1 >= nseg)
+                return SMAPB_JPEG_CORRUPT;
+        } else if (m != 0xD9) {
+            return SMAPB_JPEG_UNSUPPORTED;
+        }
+        H->seg_begin.push_back(start);
+        H->seg_end.push_back(q);
+        H->seg_stuffed.push_back(stuffed);
+        if (m == 0xD9) break;
+        start = q = q + 2;
+        stuffed = 0;
+    }
+    if ((int)H->seg_begin.size() != nseg) return SMAPB_JPEG_CORRUPT;
+    if (H->seg_end.back() - H->seg_begin.front() > MAX_SCAN_BYTES) return SMAPB_JPEG_TOO_LARGE;
+    H->out_h = H->orientation >= 5 ? H->w : H->h;
+    H->out_w = H->orientation >= 5 ? H->h : H->w;
+    return SMAPB_JPEG_OK;
+}
+
+// ---- device helpers --------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t peek32(const uint32_t* words, uint32_t pos) {
+    const uint32_t w = pos >> 5, sh = pos & 31;
+    const uint32_t hi = __byte_perm(words[w], 0, 0x0123), lo = __byte_perm(words[w + 1], 0, 0x0123);
+    return __funnelshift_l(lo, hi, sh);
+}
+
+// Decodes from (pos, blk, zz) while pos < stop.  Every unit (a Huffman code and its extra bits) must end within seg_end.
+// Errors (a code not in the table, a run past coefficient 63, a unit past the segment's end) are recorded - `err` = blocks
+// completed before the first one, or -1 - and decoding goes on by a fixed rule (skip one bit; end the block; stop), so a
+// speculative decoder that started from a wrong state keeps going until it falls into step with the true decoder.
+// WRITE: coefficients go to coef (block `blk0` = the first block this run completes, counted within the segment); blocks at
+// or beyond `limit` are not written.
+struct RunResult {
+    uint32_t pos;
+    int blk, zz, nblk, err;
+};
+
+template <bool WRITE>
+__device__ RunResult huff_run(const DevImage& I, const uint32_t* __restrict__ words, uint32_t pos, int blk, int zz, uint32_t stop,
+                              uint32_t seg_end, int16_t* __restrict__ coef, int blk0, int limit) {
+    int nblk = 0, err = -1;
+    while (pos < stop) {
+        const int c = I.blk_comp[blk];
+        const DevHuff& T = zz == 0 ? I.dc[c] : I.ac[c];
+        const uint32_t bits = peek32(words, pos);
+        int len = 0, sym = 0;
+        const uint32_t f = T.fast[bits >> 23];
+        if (f) {
+            len = f >> 8, sym = f & 255;
+        } else {
+            for (int l = 10; l <= 16; l++) {
+                const int code = (int)(bits >> (32 - l));
+                if (code <= T.maxcode[l]) {
+                    len = l;
+                    sym = T.vals[(T.valoff[l] + code) & 255];
+                    break;
+                }
+            }
+            if (!len) {
+                if (err < 0) err = nblk;
+                pos++;
+                continue;
+            }
+        }
+        const int s = sym & 15;
+        if ((uint64_t)pos + len + s > seg_end) {
+            if (err < 0) err = nblk;
+            pos = seg_end;
+            break;
+        }
+        int v = 0;
+        if (s) {
+            v = (int)((bits << len) >> (32 - s));
+            if (v < (1 << (s - 1))) v += 1 - (1 << s);
+        }
+        int16_t* b = WRITE && blk0 + nblk < limit ? coef + (int64_t)(blk0 + nblk) * 64 : nullptr;
+        if (zz == 0) {
+            if (b) b[0] = (int16_t)v;
+            zz = 1;
+        } else if (s == 0) {
+            if ((sym >> 4) == 15) {
+                zz += 16;
+                if (zz > 64) {
+                    if (err < 0) err = nblk;
+                    zz = 64;
+                }
+            } else {
+                zz = 64;
+            }
+        } else {
+            zz += sym >> 4;
+            if (zz > 63) {
+                if (err < 0) err = nblk;
+                zz = 64;
+            } else {
+                if (b) b[c_zigzag[zz]] = (int16_t)v;
+                zz++;
+            }
+        }
+        pos += len + s;
+        if (zz == 64) {
+            zz = 0;
+            nblk++;
+            if (++blk == I.bpm) blk = 0;
+        }
+    }
+    return {pos, blk, zz, nblk, err};
+}
+
+// ---- a. unstuffing ---------------------------------------------------------------------------------------------------
+// One CTA per image walks its scan bytes: a byte is dropped when it follows an FF (the 00 of a stuffed FF, the code byte of
+// a restart marker) or when it is an FF that starts a restart marker.  Block-wide prefix sums give the output positions.
+__device__ int block_exclusive_scan(int v, int* total) {
+    __shared__ int warp_sums[32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_sums[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        const int nw = blockDim.x >> 5;
+        int t = lane < nw ? warp_sums[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, t, o);
+            if (lane >= o) t += y;
+        }
+        warp_sums[lane] = t;
+    }
+    __syncthreads();
+    const int before = (wid ? warp_sums[wid - 1] : 0) + x - v;
+    *total = warp_sums[(blockDim.x >> 5) - 1];
+    __syncthreads();
+    return before;
+}
+
+constexpr int UNSTUFF_PER_THREAD = 16;
+
+__global__ void __launch_bounds__(1024) unstuff_kernel(const DevImage* __restrict__ imgs, const uint8_t* __restrict__ raw,
+                                                       uint8_t* __restrict__ unst) {
+    const DevImage& I = imgs[blockIdx.x];
+    const uint8_t* src = raw + I.raw_off;
+    uint8_t* dst = unst + I.unst_off;
+    const int64_t n = I.raw_len;
+    int64_t out = 0;
+    for (int64_t base = 0; base < n; base += (int64_t)blockDim.x * UNSTUFF_PER_THREAD) {
+        const int64_t i0 = base + (int64_t)threadIdx.x * UNSTUFF_PER_THREAD;
+        uint8_t keep[UNSTUFF_PER_THREAD];
+        int cnt = 0;
+#pragma unroll
+        for (int k = 0; k < UNSTUFF_PER_THREAD; k++) {
+            const int64_t i = i0 + k;
+            bool kp = false;
+            if (i < n) {
+                const uint8_t b = src[i];
+                const bool after_ff = i > 0 && src[i - 1] == 0xFF;
+                const bool marker_ff = b == 0xFF && i + 1 < n && src[i + 1] != 0x00;
+                kp = !after_ff && !marker_ff;
+            }
+            keep[k] = kp;
+            cnt += kp;
+        }
+        int total;
+        const int at = block_exclusive_scan(cnt, &total);
+        int o = 0;
+#pragma unroll
+        for (int k = 0; k < UNSTUFF_PER_THREAD; k++)
+            if (keep[k]) dst[out + at + o++] = src[i0 + k];
+        out += total;
+    }
+    // zero padding behind the data: the bit reader loads whole words past a segment's last bit
+    for (int k = threadIdx.x; k < 16; k += blockDim.x) dst[out + k] = 0;
+}
+
+// ---- b. Huffman decoding ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) huff_sync_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
+                                                        const DevSub* __restrict__ subs, int nsub, const uint8_t* __restrict__ unst,
+                                                        const SubState* __restrict__ prev, SubState* __restrict__ cur,
+                                                        int* __restrict__ changed, int pass) {
+    if (pass >= 2 && changed[pass - 1] == 0) return;  // converged: the buffer of the first quiet pass is final
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nsub) return;
+    const DevSub S = subs[i];
+    const DevImage& I = imgs[S.img];
+    const DevSeg& G = segs[S.seg];
+    unsigned long long start;
+    if (pass == 0) {
+        start = pack_state(S.bit_begin, 0, 0);  // a guess, except for the first subsequence of a segment
+    } else {
+        if (G.sub0 == i) {
+            cur[i] = prev[i];
+            return;
+        }
+        start = prev[i - 1].exit;
+        if (start == prev[i].start) {
+            cur[i] = prev[i];
+            return;
+        }
+    }
+    const uint32_t* words = (const uint32_t*)(unst + I.unst_off);
+    if (pass == 0 && G.sub0 != i) {
+        // warm-up: decode up to WARM_BITS before the subsequence from the guess, so that the state at its first unit
+        // boundary has had that long to fall into step with the true decoder
+        const uint32_t from = S.bit_begin - min(S.bit_begin - G.bit_begin, (uint32_t)WARM_BITS);
+        const RunResult W = huff_run<false>(I, words, from, 0, 0, S.bit_begin, G.bit_end, nullptr, 0, 0);
+        start = pack_state(W.pos, W.blk, W.zz);
+    }
+    SubState r;
+    r.start = start;
+    const RunResult R = huff_run<false>(I, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255,
+                                        S.bit_end, G.bit_end, nullptr, 0, 0);
+    r.exit = pack_state(R.pos, R.blk, R.zz);
+    r.nblk = R.nblk;
+    r.errblk = R.err >= 0 ? R.err : 0x7fffffff;
+    cur[i] = r;
+    changed[pass] = 1;  // benign race: every writer stores 1
+}
+
+// One CTA per image: exclusive prefix sum of the blocks completed per subsequence (within its segment), and the checks
+// that make an image fall back: an error before the segment's last block, or fewer blocks than the segment's MCUs hold.
+__global__ void __launch_bounds__(1024) huff_prefix_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
+                                                           const SubState* __restrict__ st, int* __restrict__ base,
+                                                           int* __restrict__ status) {
+    const DevImage& I = imgs[blockIdx.x];
+    int carry = 0;
+    for (int j0 = 0; j0 < I.nsub; j0 += blockDim.x) {
+        const int j = j0 + threadIdx.x;
+        const int v = j < I.nsub ? st[I.sub0 + j].nblk : 0;
+        int total;
+        const int at = block_exclusive_scan(v, &total);
+        if (j < I.nsub) base[I.sub0 + j] = carry + at;  // image-wide for now
+        carry += total;
+    }
+    __syncthreads();
+    bool bad = false;
+    for (int j = threadIdx.x; j < I.nsub; j += blockDim.x) {
+        const int i = I.sub0 + j;
+        const SubState s = st[i];
+        if (s.errblk != 0x7fffffff) {
+            int lo = I.seg0, hi = I.seg0 + I.nseg - 1;
+            while (lo < hi) {
+                const int mid = (lo + hi + 1) >> 1;
+                if (segs[mid].sub0 <= i) lo = mid;
+                else hi = mid - 1;
+            }
+            const int e = base[i] - base[segs[lo].sub0] + s.errblk;  // segs[lo] holds subsequence i
+            if (e < segs[lo].nmcu * I.bpm) bad = true;
+        }
+    }
+    for (int k = I.seg0 + threadIdx.x; k < I.seg0 + I.nseg; k += blockDim.x) {
+        const DevSeg& G = segs[k];
+        const int last = G.sub0 + G.nsub - 1;
+        if (base[last] + st[last].nblk - base[G.sub0] < G.nmcu * I.bpm) bad = true;
+    }
+    if (bad) status[blockIdx.x] = SMAPB_JPEG_CORRUPT;
+}
+
+__global__ void __launch_bounds__(256) huff_write_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
+                                                         const DevSub* __restrict__ subs, int nsub, const uint8_t* __restrict__ unst,
+                                                         const SubState* __restrict__ st, const int* __restrict__ base,
+                                                         const int* __restrict__ status, int16_t* __restrict__ coef) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nsub) return;
+    const DevSub S = subs[i];
+    if (status[S.img] != SMAPB_JPEG_OK) return;
+    const DevImage& I = imgs[S.img];
+    const DevSeg& G = segs[S.seg];
+    const unsigned long long start = st[i].start;
+    const int first = G.first_mcu * I.bpm;  // block index of the segment's first block within the image
+    const int local = base[i] - base[G.sub0];
+    const uint32_t* words = (const uint32_t*)(unst + I.unst_off);
+    huff_run<true>(I, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255, S.bit_end, G.bit_end,
+                   coef + (I.coef_off + (int64_t)first) * 64, local, G.nmcu * I.bpm);
+}
+
+// DC prediction: one CTA per (image, component), a segmented scan over that component's blocks in decode order, reset at
+// every restart segment.  The sum runs in int (libjpeg's predictor), the block keeps its low 16 bits.
+__global__ void __launch_bounds__(1024) dc_scan_kernel(const DevImage* __restrict__ imgs, const int* __restrict__ status,
+                                                       int16_t* __restrict__ coef) {
+    const DevImage& I = imgs[blockIdx.x];
+    const int c = blockIdx.y;
+    if (c >= I.ncomp || status[blockIdx.x] != SMAPB_JPEG_OK) return;
+    int j0 = 0;
+    for (int j = 0; j < I.bpm; j++)
+        if (I.blk_comp[j] < c) j0++;
+    const int nc = (c == 0) ? I.bpm - (I.ncomp - 1) : 1;
+    const int total = I.nmcu * nc;
+    int16_t* cf = coef + I.coef_off * 64;
+    __shared__ int s_head[32], s_val[32];
+    int carry = 0;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    for (int t0 = 0; t0 < total; t0 += blockDim.x) {
+        const int t = t0 + threadIdx.x;
+        int v = 0, head = 0;
+        int64_t at = 0;
+        if (t < total) {
+            const int m = t / nc, k = t % nc;
+            at = ((int64_t)m * I.bpm + j0 + k) * 64;
+            v = cf[at];
+            head = (k == 0 && m % I.per == 0) ? 1 : 0;
+        }
+        // segmented inclusive scan of (head, v): (h1, v1) + (h2, v2) = (h1 | h2, h2 ? v2 : v1 + v2)
+        int x = v, hx = head;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, x, o), hy = __shfl_up_sync(0xffffffffu, hx, o);
+            if (lane >= o) {
+                if (!hx) x += y;
+                hx |= hy;
+            }
+        }
+        if (lane == 31) s_head[wid] = hx, s_val[wid] = x;
+        __syncthreads();
+        if (wid == 0) {
+            int wx = lane < nw ? s_val[lane] : 0, wh = lane < nw ? s_head[lane] : 0;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, wx, o), hy = __shfl_up_sync(0xffffffffu, wh, o);
+                if (lane >= o) {
+                    if (!wh) wx += y;
+                    wh |= hy;
+                }
+            }
+            s_val[lane] = wx, s_head[lane] = wh;
+        }
+        __syncthreads();
+        // prefix from earlier warps of this tile, then the carry of earlier tiles
+        int pre = 0, pre_head = 0;
+        if (wid > 0) pre = s_val[wid - 1], pre_head = s_head[wid - 1];
+        if (!hx) {
+            x += pre;
+            if (!pre_head) x += carry;
+        }
+        if (t < total) cf[at] = (int16_t)x;
+        const int tile_val = s_val[nw - 1], tile_head = s_head[nw - 1];
+        __syncthreads();
+        carry = tile_head ? tile_val : carry + tile_val;
+    }
+}
+
+// ---- c. dequantisation + IDCT ----------------------------------------------------------------------------------------
+// LL&M 8-point IDCT in 13-bit fixed point (the IJG "accurate integer" method): columns keep 2 extra bits, rows remove
+// 13 + 2 + 3 bits; + 128 and saturation to 0..255 (cv2's libjpeg-turbo build saturates, settled on q100 checkerboards).
+// cv2's IDCT computes in 16-bit lanes; where a dequantised coefficient or a pass-1 output leaves +-GUARD one of them could
+// overflow, and the image is left to cv2 (never happens with encoder-written quantisers).
+struct Idct8 {
+    int o[8];
+};
+
+__device__ __forceinline__ Idct8 idct8(int x0, int x1, int x2, int x3, int x4, int x5, int x6, int x7, int shift) {
+    int z1 = (x2 + x6) * 4433;
+    const int t2 = z1 - x6 * 15137, t3 = z1 + x2 * 6270;
+    const int t0 = (x0 + x4) * 8192, t1 = (x0 - x4) * 8192;
+    const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
+    int a0 = x7, a1 = x5, a2 = x3, a3 = x1;
+    z1 = a0 + a3;
+    int z2 = a1 + a2, z3 = a0 + a2, z4 = a1 + a3;
+    const int z5 = (z3 + z4) * 9633;
+    a0 *= 2446, a1 *= 16819, a2 *= 25172, a3 *= 12299;
+    z1 *= -7373, z2 *= -20995, z3 = z3 * -16069 + z5, z4 = z4 * -3196 + z5;
+    a0 += z1 + z3, a1 += z2 + z4, a2 += z2 + z3, a3 += z1 + z4;
+    const int r = 1 << (shift - 1);
+    Idct8 R;
+    R.o[0] = (t10 + a3 + r) >> shift, R.o[7] = (t10 - a3 + r) >> shift;
+    R.o[1] = (t11 + a2 + r) >> shift, R.o[6] = (t11 - a2 + r) >> shift;
+    R.o[2] = (t12 + a1 + r) >> shift, R.o[5] = (t12 - a1 + r) >> shift;
+    R.o[3] = (t13 + a0 + r) >> shift, R.o[4] = (t13 - a0 + r) >> shift;
+    return R;
+}
+
+__global__ void __launch_bounds__(128) idct_kernel(const DevImage* __restrict__ imgs, const int16_t* __restrict__ coef,
+                                                   uint8_t* __restrict__ planes, int* __restrict__ status) {
+    const DevImage& I = imgs[blockIdx.y];
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= I.nmcu * I.bpm || status[blockIdx.y] != SMAPB_JPEG_OK) return;
+    const int m = g / I.bpm, j = g % I.bpm, c = I.blk_comp[j];
+    const int bx = (m % I.mcux) * I.comp_h[c] + I.blk_dx[j], by = (m / I.mcux) * I.comp_v[c] + I.blk_dy[j];
+    const int4* src = (const int4*)(coef + (I.coef_off + g) * 64);
+    int x[64];
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const int4 q = src[r];
+        const int w4[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            x[r * 8 + 2 * k] = (int)(int16_t)(w4[k] & 0xFFFF) * I.qt[c][r * 8 + 2 * k];
+            x[r * 8 + 2 * k + 1] = (int)(int16_t)((unsigned)w4[k] >> 16) * I.qt[c][r * 8 + 2 * k + 1];
+        }
+    }
+    bool over = false;
+#pragma unroll
+    for (int k = 0; k < 64; k++) over |= x[k] > GUARD || x[k] < -GUARD;
+#pragma unroll
+    for (int col = 0; col < 8; col++) {
+        const Idct8 R = idct8(x[col], x[8 + col], x[16 + col], x[24 + col], x[32 + col], x[40 + col], x[48 + col], x[56 + col], 11);
+#pragma unroll
+        for (int r = 0; r < 8; r++) {
+            x[r * 8 + col] = R.o[r];
+            over |= R.o[r] > GUARD || R.o[r] < -GUARD;
+        }
+    }
+    if (over) {
+        status[blockIdx.y] = SMAPB_JPEG_UNSUPPORTED;
+        return;
+    }
+    uint8_t* dst = planes + I.plane_off[c] + (int64_t)by * 8 * I.plane_w[c] + bx * 8;
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const Idct8 R = idct8(x[r * 8], x[r * 8 + 1], x[r * 8 + 2], x[r * 8 + 3], x[r * 8 + 4], x[r * 8 + 5], x[r * 8 + 6],
+                              x[r * 8 + 7], 18);
+        uint32_t lo = 0, hi = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            lo |= (uint32_t)min(max(R.o[k] + 128, 0), 255) << (8 * k);
+            hi |= (uint32_t)min(max(R.o[k + 4] + 128, 0), 255) << (8 * k);
+        }
+        *(uint2*)(dst + (int64_t)r * I.plane_w[c]) = make_uint2(lo, hi);
+    }
+}
+
+// ---- d. upsampling, colour, orientation ------------------------------------------------------------------------------
+__device__ __forceinline__ int px(const uint8_t* p, int pw, int y, int x) { return p[(int64_t)y * pw + x]; }
+
+// libjpeg's fancy upsampling of a chroma plane (factors 1x1) to the luma grid at (y, x); cw x ch = the plane's real size
+__device__ int chroma_at(const uint8_t* C, int pw, int cw, int ch, int hmax, int vmax, int y, int x) {
+    if (hmax == 1 && vmax == 1) return px(C, pw, y, x);
+    const int i = x >> (hmax - 1);
+    if (hmax == 2 && cw <= 2) return px(C, pw, y >> (vmax - 1), i);  // fancy h2 filters need 3 columns: replication
+    if (vmax == 1) {  // h2v1
+        const int n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);
+        return (3 * px(C, pw, y, i) + px(C, pw, y, n) + ((x & 1) ? 2 : 1)) >> 2;
+    }
+    const int r0 = y >> 1, r1 = (y & 1) ? min(r0 + 1, ch - 1) : max(r0 - 1, 0);
+    if (hmax == 1)  // h1v2
+        return (3 * px(C, pw, r0, x) + px(C, pw, r1, x) + ((y & 1) ? 2 : 1)) >> 2;
+    const int n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);  // h2v2: column sums of the nearer and the further row
+    const int s0 = 3 * px(C, pw, r0, i) + px(C, pw, r1, i), s1 = 3 * px(C, pw, r0, n) + px(C, pw, r1, n);
+    return (3 * s0 + s1 + ((x & 1) ? 7 : 8)) >> 4;
+}
+
+__global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict__ imgs, const uint8_t* __restrict__ planes,
+                                                     const int* __restrict__ status) {
+    const DevImage& I = imgs[blockIdx.y];
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (int64_t)I.h * I.w || status[blockIdx.y] != SMAPB_JPEG_OK) return;
+    const int y = (int)(t / I.w), x = (int)(t % I.w);
+    const int Y = px(planes + I.plane_off[0], I.plane_w[0], y, x);
+    int b = Y, g = Y, r = Y;
+    if (I.ncomp == 3) {
+        const int cw = (I.w + I.hmax - 1) / I.hmax, ch = (I.h + I.vmax - 1) / I.vmax;
+        const int cb = chroma_at(planes + I.plane_off[1], I.plane_w[1], cw, ch, I.hmax, I.vmax, y, x) - 128;
+        const int cr = chroma_at(planes + I.plane_off[2], I.plane_w[2], cw, ch, I.hmax, I.vmax, y, x) - 128;
+        // JFIF YCbCr -> RGB with 16-bit fixed-point constants round(k * 2^16), rounded by adding 2^15
+        r = Y + ((91881 * cr + 32768) >> 16);
+        g = Y + ((-46802 * cr - 22554 * cb + 32768) >> 16);
+        b = Y + ((116130 * cb + 32768) >> 16);
+        r = min(max(r, 0), 255), g = min(max(g, 0), 255), b = min(max(b, 0), 255);
+    }
+    // EXIF orientation as cv2 applies it (2 flip x, 3 rotate 180, 4 flip y, 5 transpose, 6 rotate 90 cw, 7 transverse, 8 ccw)
+    int oy = y, ox = x;
+    switch (I.orientation) {
+        case 2: ox = I.w - 1 - x; break;
+        case 3: oy = I.h - 1 - y, ox = I.w - 1 - x; break;
+        case 4: oy = I.h - 1 - y; break;
+        case 5: oy = x, ox = y; break;
+        case 6: oy = x, ox = I.h - 1 - y; break;
+        case 7: oy = I.w - 1 - x, ox = I.h - 1 - y; break;
+        case 8: oy = I.w - 1 - x, ox = y; break;
+        default: break;
+    }
+    uint8_t* o = I.out + ((int64_t)oy * I.out_w + ox) * 3;
+    o[0] = (uint8_t)b, o[1] = (uint8_t)g, o[2] = (uint8_t)r;
+}
+
+template <typename T>
+cudaError_t grow(T** p, size_t* cap, size_t n) {
+    if (n <= *cap) return cudaSuccess;
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+    cudaError_t e = cudaMalloc((void**)p, n * sizeof(T));
+    if (e == cudaSuccess) *cap = n;
+    return e;
+}
+
+}  // namespace
+
+struct JpegWorkspace {
+    uint8_t* host = nullptr;  // pinned staging: descriptors + scan bytes, one upload per batch
+    size_t host_cap = 0;
+    uint8_t* dev_in = nullptr;  // device copy of the staging area
+    size_t dev_in_cap = 0;
+    uint8_t* unst = nullptr;
+    size_t unst_cap = 0;
+    SubState* st[2] = {nullptr, nullptr};
+    size_t st_cap[2] = {0, 0};
+    int* base = nullptr;
+    size_t base_cap = 0;
+    int16_t* coef = nullptr;
+    size_t coef_cap = 0;
+    uint8_t* planes = nullptr;
+    size_t planes_cap = 0;
+    int* small = nullptr;  // status[n] then changed[passes]
+    size_t small_cap = 0;
+    int* small_host = nullptr;  // pinned
+    size_t small_host_cap = 0;
+};
+
+JpegWorkspace* jpeg_workspace_create() { return new JpegWorkspace(); }
+
+void jpeg_workspace_destroy(JpegWorkspace* ws) {
+    if (!ws) return;
+    if (ws->host) cudaFreeHost(ws->host);
+    if (ws->small_host) cudaFreeHost(ws->small_host);
+    void* d[] = {ws->dev_in, ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->planes, ws->small};
+    for (void* p : d)
+        if (p) cudaFree(p);
+    delete ws;
+}
+
+static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int* status,
+                cudaStream_t st, int64_t* launches, std::string* err) {
+#define JCK(call)                                                                                             \
+    do {                                                                                                      \
+        cudaError_t e_ = (call);                                                                              \
+        if (e_ != cudaSuccess) {                                                                              \
+            *err = std::string(#call) + ": " + cudaGetErrorString(e_) + " @jpeg.cu:" + std::to_string(__LINE__); \
+            return -10;                                                                                       \
+        }                                                                                                     \
+    } while (0)
+    if (n < 0 || (n > 0 && (!jpeg || !nbytes || !bgr || !status))) {
+        *err = "smapb_decode_jpeg: null argument";
+        return -1;
+    }
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    JCK(cudaStreamIsCapturing(st, &cap));
+    if (cap != cudaStreamCaptureStatusNone) {
+        *err = "smapb_decode_jpeg: not capturable (it synchronises and may grow its workspace)";
+        return -1;
+    }
+    // host: parse, then lay out descriptors and scan bytes
+    std::vector<Header> H(n);
+    std::vector<int> idx;  // images that go to the device
+    for (int i = 0; i < n; i++) {
+        status[i] = jpeg ? jpeg_parse(jpeg[i], nbytes[i], &H[i]) : SMAPB_JPEG_MALFORMED;
+        if (status[i] == SMAPB_JPEG_OK) {
+            if (!bgr[i]) {
+                *err = "smapb_decode_jpeg: no output buffer for decodable image " + std::to_string(i);
+                return -1;
+            }
+            idx.push_back(i);
+        }
+    }
+    const int m = (int)idx.size();
+    if (m == 0) return 0;
+    std::vector<DevImage> imgs(m);
+    std::vector<DevSeg> segs;
+    std::vector<DevSub> subs;
+    int64_t raw_total = 0, unst_total = 0, coef_blocks = 0, plane_total = 0;
+    int max_blocks = 0;
+    int64_t max_px = 0;
+    int max_nsub_seg = 1;
+    for (int k = 0; k < m; k++) {
+        const Header& h = H[idx[k]];
+        DevImage& I = imgs[k];
+        memset(&I, 0, sizeof(I));
+        I.h = h.h, I.w = h.w, I.out_h = h.out_h, I.out_w = h.out_w, I.orientation = h.orientation, I.ncomp = h.ncomp;
+        I.hmax = h.hmax, I.vmax = h.vmax, I.mcux = h.mcux, I.mcuy = h.mcuy, I.nmcu = h.nmcu;
+        I.per = h.dri ? h.dri : h.nmcu;
+        I.nseg = (int)h.seg_begin.size();
+        I.out = bgr[idx[k]];
+        int j = 0;
+        for (int c = 0; c < h.ncomp; c++) {
+            for (int v = 0; v < h.comp_v[c]; v++)
+                for (int u = 0; u < h.comp_h[c]; u++) I.blk_comp[j] = c, I.blk_dx[j] = u, I.blk_dy[j] = v, j++;
+            I.comp_h[c] = h.comp_h[c], I.comp_v[c] = h.comp_v[c];
+            I.plane_w[c] = h.mcux * h.comp_h[c] * 8;
+            I.plane_h[c] = h.mcuy * h.comp_v[c] * 8;
+            I.plane_off[c] = plane_total;
+            plane_total += align_up((size_t)I.plane_w[c] * I.plane_h[c], 256);
+            for (int q = 0; q < 64; q++) I.qt[c][q] = (int16_t)h.qt[c][q];
+            if (!build_huff(*h.dc[c], &I.dc[c]) || !build_huff(*h.ac[c], &I.ac[c])) {
+                status[idx[k]] = SMAPB_JPEG_MALFORMED;
+            }
+        }
+        I.bpm = j;
+        I.raw_off = raw_total;
+        I.raw_len = h.seg_end.back() - h.seg_begin.front();
+        raw_total += align_up(I.raw_len, 16);
+        I.unst_off = unst_total;
+        I.coef_off = coef_blocks;
+        coef_blocks += (int64_t)h.nmcu * I.bpm;
+        max_blocks = std::max(max_blocks, h.nmcu * I.bpm);
+        max_px = std::max(max_px, (int64_t)h.h * h.w);
+        I.seg0 = (int)segs.size();
+        I.sub0 = (int)subs.size();
+        uint32_t bit = 0;
+        for (int s = 0; s < I.nseg; s++) {
+            const int64_t len = h.seg_end[s] - h.seg_begin[s] - h.seg_stuffed[s];
+            DevSeg G;
+            G.img = k;
+            G.first_mcu = s * I.per;
+            G.nmcu = std::min(I.per, h.nmcu - G.first_mcu);
+            G.bit_begin = bit;
+            G.bit_end = bit + (uint32_t)(len * 8);
+            G.sub0 = (int)subs.size();
+            G.nsub = std::max(1, (int)((len * 8 + SUB_BITS - 1) / SUB_BITS));
+            for (int u = 0; u < G.nsub; u++) {
+                DevSub S;
+                S.img = k;
+                S.seg = (int)segs.size();
+                S.bit_begin = std::min(G.bit_end, G.bit_begin + (uint32_t)u * SUB_BITS);
+                S.bit_end = u == G.nsub - 1 ? G.bit_end : G.bit_begin + (uint32_t)(u + 1) * SUB_BITS;
+                subs.push_back(S);
+            }
+            max_nsub_seg = std::max(max_nsub_seg, G.nsub);
+            segs.push_back(G);
+            bit = G.bit_end;
+        }
+        I.nsub = (int)subs.size() - I.sub0;
+        unst_total += align_up(bit / 8 + 16, 16);
+    }
+    // staging layout: images | segments | subsequences | scan bytes
+    const size_t o_img = 0, o_seg = align_up(o_img + sizeof(DevImage) * m, 256),
+                 o_sub = align_up(o_seg + sizeof(DevSeg) * segs.size(), 256),
+                 o_raw = align_up(o_sub + sizeof(DevSub) * subs.size(), 256), total = o_raw + raw_total;
+    if (total > ws->host_cap) {
+        if (ws->host) cudaFreeHost(ws->host);
+        ws->host = nullptr;
+        ws->host_cap = 0;
+        JCK(cudaMallocHost((void**)&ws->host, total));
+        ws->host_cap = total;
+    }
+    JCK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
+    memcpy(ws->host + o_img, imgs.data(), sizeof(DevImage) * m);
+    memcpy(ws->host + o_seg, segs.data(), sizeof(DevSeg) * segs.size());
+    memcpy(ws->host + o_sub, subs.data(), sizeof(DevSub) * subs.size());
+    for (int k = 0; k < m; k++) {
+        const Header& h = H[idx[k]];
+        memcpy(ws->host + o_raw + imgs[k].raw_off, jpeg[idx[k]] + h.seg_begin.front(), imgs[k].raw_len);
+    }
+    const int nsub = (int)subs.size();
+    const int max_passes = max_nsub_seg + 1;
+    JCK(grow(&ws->dev_in, &ws->dev_in_cap, total));
+    JCK(grow(&ws->unst, &ws->unst_cap, (size_t)unst_total));
+    JCK(grow(&ws->st[0], &ws->st_cap[0], (size_t)nsub));
+    JCK(grow(&ws->st[1], &ws->st_cap[1], (size_t)nsub));
+    JCK(grow(&ws->base, &ws->base_cap, (size_t)nsub));
+    JCK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
+    JCK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
+    JCK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
+    if ((size_t)m + PASS_GROUP > ws->small_host_cap) {
+        if (ws->small_host) cudaFreeHost(ws->small_host);
+        ws->small_host = nullptr;
+        ws->small_host_cap = 0;
+        JCK(cudaMallocHost((void**)&ws->small_host, sizeof(int) * (m + PASS_GROUP)));
+        ws->small_host_cap = m + PASS_GROUP;
+    }
+    const DevImage* d_img = (const DevImage*)(ws->dev_in + o_img);
+    const DevSeg* d_seg = (const DevSeg*)(ws->dev_in + o_seg);
+    const DevSub* d_sub = (const DevSub*)(ws->dev_in + o_sub);
+    const uint8_t* d_raw = ws->dev_in + o_raw;
+    int* d_status = ws->small;
+    int* d_changed = ws->small + m;
+    for (int k = 0; k < m; k++) ws->small_host[k] = status[idx[k]];
+    JCK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
+    JCK(cudaMemcpyAsync(d_status, ws->small_host, sizeof(int) * m, cudaMemcpyHostToDevice, st));
+    JCK(cudaMemsetAsync(d_changed, 0, sizeof(int) * (max_passes + PASS_GROUP), st));
+    JCK(cudaMemsetAsync(ws->coef, 0, (size_t)coef_blocks * 64 * sizeof(int16_t), st));
+    // a. unstuffing
+    unstuff_kernel<<<m, 1024, 0, st>>>(d_img, d_raw, ws->unst);
+    JCK(cudaGetLastError());
+    ++*launches;
+    // b. speculative pass, then sync passes until a pass changes nothing (at most one per subsequence of the longest segment)
+    const int sgrid = (nsub + 255) / 256;
+    int pass = 0, final_pass = -1;
+    while (final_pass < 0) {
+        const int stop = std::min(pass + PASS_GROUP, max_passes + 1);
+        const int first = pass;
+        for (; pass < stop; pass++) {
+            huff_sync_kernel<<<sgrid, 256, 0, st>>>(d_img, d_seg, d_sub, nsub, ws->unst, ws->st[(pass + 1) & 1], ws->st[pass & 1],
+                                                    d_changed, pass);
+            JCK(cudaGetLastError());
+            ++*launches;
+        }
+        JCK(cudaMemcpyAsync(ws->small_host, d_changed + first, sizeof(int) * (stop - first), cudaMemcpyDeviceToHost, st));
+        JCK(cudaStreamSynchronize(st));
+        for (int p = first; p < stop; p++)
+            if (p > 0 && ws->small_host[p - first] == 0) {
+                final_pass = p;
+                break;
+            }
+        if (final_pass < 0 && pass > max_passes) {
+            *err = "smapb_decode_jpeg: Huffman sync passes did not converge";
+            return -11;
+        }
+    }
+    const SubState* fin = ws->st[final_pass & 1];
+    huff_prefix_kernel<<<m, 1024, 0, st>>>(d_img, d_seg, fin, ws->base, d_status);
+    huff_write_kernel<<<sgrid, 256, 0, st>>>(d_img, d_seg, d_sub, nsub, ws->unst, fin, ws->base, d_status, ws->coef);
+    dc_scan_kernel<<<dim3(m, 3), 1024, 0, st>>>(d_img, d_status, ws->coef);
+    JCK(cudaGetLastError());
+    // c. IDCT
+    idct_kernel<<<dim3((max_blocks + 127) / 128, m), 128, 0, st>>>(d_img, ws->coef, ws->planes, d_status);
+    // d. upsampling, colour, orientation
+    colour_kernel<<<dim3((unsigned)((max_px + 255) / 256), m), 256, 0, st>>>(d_img, ws->planes, d_status);
+    JCK(cudaGetLastError());
+    *launches += 5;
+    JCK(cudaMemcpyAsync(ws->small_host, d_status, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
+    JCK(cudaStreamSynchronize(st));
+    for (int k = 0; k < m; k++)
+        if (status[idx[k]] == SMAPB_JPEG_OK) status[idx[k]] = ws->small_host[k];
+    return 0;
+#undef JCK
+}
+
+}  // namespace smapb
+
+extern "C" {
+#pragma GCC visibility push(default)
+int smapb_jpeg_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* orientation, int* status) {
+    if (!status) return -1;
+    smapb::Header H;
+    *status = smapb::jpeg_parse(data, nbytes, &H);
+    if (*status == SMAPB_JPEG_OK) {
+        for (int c = 0; c < H.ncomp; c++) {
+            smapb::DevHuff d;
+            if (!smapb::build_huff(*H.dc[c], &d) || !smapb::build_huff(*H.ac[c], &d)) *status = SMAPB_JPEG_MALFORMED;
+        }
+    }
+    const bool ok = *status == SMAPB_JPEG_OK;
+    if (h) *h = ok ? H.out_h : 0;
+    if (w) *w = ok ? H.out_w : 0;
+    if (orientation) *orientation = ok ? H.orientation : 0;
+    return 0;
+}
+#pragma GCC visibility pop
+}

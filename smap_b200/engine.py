@@ -59,6 +59,16 @@ def get_tile_table():
     return buf.value.decode()
 
 
+def jpeg_info(data):
+    """Header walk of one JPEG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
+    handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h)."""
+    h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    rc = _lib.load().smapb_jpeg_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
+    if rc != 0:
+        raise SmapB200Error("smapb_jpeg_info failed (%d)" % rc)
+    return st.value, h.value, w.value, o.value
+
+
 class Engine:
     """One handle per (process, device).  in_h/in_w: network input size (multiples of 32)."""
 
@@ -184,6 +194,26 @@ class Engine:
                                              _ptr(gt_counts.to(torch.int32).contiguous()), gt_roots.shape[1], B, _ptr(p2), _ptr(p3),
                                              _ptr(rdp), _ptr(co), self._st()), "smapb_lift3d_gt")
         return p2, p3, rdp, co
+
+    # ---- JPEG decoding -------------------------------------------------------------------------
+    def decode_jpeg(self, files):
+        """files: list of bytes (whole JPEG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
+        cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
+        n = len(files)
+        out = [None] * n
+        if n == 0:
+            return out
+        ptrs = (ctypes.c_void_p * n)()
+        for i, f in enumerate(files):
+            st, h, w = jpeg_info(f)[:3]
+            if st == 0:
+                out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
+                ptrs[i] = out[i].data_ptr()
+        data = (ctypes.c_char_p * n)(*files)
+        sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
+        status = (ctypes.c_int * n)()
+        self._check(self.lib.smapb_decode_jpeg(self._h, n, data, sizes, ptrs, status, self._st()), "smapb_decode_jpeg")
+        return [o if status[i] == 0 else None for i, o in enumerate(out)]
 
     # ---- pre-processing ------------------------------------------------------------------------
     def preprocess(self, images, out=None):
