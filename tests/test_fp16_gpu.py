@@ -1,12 +1,13 @@
 """GPU: the fp16 precision (SMAPB_PREC_FP16): fp16 operands and activations, fp32 accumulation, stores clamped to +-65504.
 
-  * single convolutions (the CASES of tests/test_conv_gpu.py) against a float64 reference built from the fp16-rounded
-    operands the device holds: |y - r| <= 1/2 ulp_fp16(y) + _acc_bound (tests/test_plan_ops_gpu.py), and the same checker
+  * single convolutions (the CASES of tests/plan_check.py) against a float64 reference built from the fp16-rounded
+    operands the device holds: |y - r| <= 1/2 ulp_fp16(y) + _acc_bound (tests/plan_check.py), and the same checker
     flags a reference built from bf16-rounded operands;
   * saturation: outputs beyond +-65504 are exactly +-65504, never inf / NaN, and counted; folded weights beyond the range
     are rejected by finalize;
-  * every op of the real plan against a float64 reference of its own layer, as tests/test_plan_ops_gpu.py does for bf16x3
-    and bf16, and plan switches that must not change a bit;
+  * every op of the real plan against a float64 reference of its own layer, by the checker of tests/plan_check.py that
+    tests/test_plan_ops_gpu.py runs for bf16x3 and bf16 (wrong references flagged, heads checked), and plan switches
+    that must not change a bit;
   * the whole backbone against the fp32 oracle next to bf16 and cuDNN with TF32 (the reference's own GPU numerics);
   * the whole path (records) on bench.py's first batch next to bf16x3.
 
@@ -26,8 +27,6 @@ Measured on one H100 80GB HBM3 (400 W power limit), max|a - b| / max|ref| agains
 fp16 lands where the reference's own cuDNN-TF32 run lands, 7x below bf16.
 
 (-s prints the table; FP16_BOUND keeps a factor >= 2 over the worst fp16 value.)"""
-import ctypes
-import math
 import os
 import sys
 
@@ -39,48 +38,22 @@ import torch.nn.functional as F
 from oracle import smap_torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_conv_gpu import CASES  # noqa: E402
-from test_plan_ops_gpu import _acc_bound, _consumers, _K, _nchw, _nhwc, op_class, plan_ops, reference, x3_error  # noqa: E402
+from plan_check import (CASES, FP16_MAX, _TILE_CASES, _K, _acc_bound, _case_tensors, _gid, _nchw, _nhwc,  # noqa: E402
+                        assert_checked, check_switches, half_ulp16, no_tf32, op_class, plan_summary)
 
 pytestmark = pytest.mark.gpu
 
-FP16_MAX = 65504.0
 FP16_BOUND = 1e-2  # backbone vs fp32 oracle, max|a - b| / max|ref| per tensor (measured <= 4.99e-3, see above)
-SEED = 5
-
-
-def _no_tf32():
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-
-
-def half_ulp16(y):
-    """Half an fp16 ulp of fp16 values y (fp64 tensor): the round-to-nearest error of the store that produced them."""
-    a = y.abs()
-    _, e = torch.frexp(a)  # a = m 2^e, m in [0.5, 1): ulp = 2^(e - 1 - 10), subnormal ulp 2^-24
-    e = torch.clamp(e - 11, min=-24)
-    return torch.ldexp(torch.full_like(a, 0.5), e)
 
 
 @pytest.fixture(scope="module")
 def eng():
     from smap_b200.engine import Engine
 
-    _no_tf32()
+    no_tf32()
     e = Engine(0, max_batch=2, in_h=64, in_w=96)
     yield e
     e.close()
-
-
-def _case_tensors(case):
-    B, H, W, Cin, Cout, k, stride, relu, use_res = case
-    g = torch.Generator(device="cpu").manual_seed(hash(case) % (2 ** 31))
-    x = torch.randn(B, H, W, Cin, generator=g).cuda()
-    w = (torch.randn(Cout, Cin, k, k, generator=g) / (Cin * k * k) ** 0.5).cuda()
-    b = torch.randn(Cout, generator=g).cuda()
-    Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
-    res = torch.randn(B, Ho, Wo, Cout, generator=g).cuda() if use_res else None
-    return x, w, b, res
 
 
 def _conv_reference(case, x, w, b, res, rnd):
@@ -133,19 +106,10 @@ def test_checker_flags_a_bf16_operand_reference(eng):
     assert over.double().mean().item() > 0.05
 
 
-_TILE_CASES = [(8, 32, 52, 256, 256, 3, 1, False), (8, 32, 52, 1024, 256, 1, 1, False), (2, 16, 26, 512, 512, 3, 2, False),
-               (4, 64, 104, 128, 512, 1, 1, True), (2, 128, 208, 256, 64, 1, 1, False)]
-
-
 @pytest.mark.parametrize("case", _TILE_CASES)
 def test_fp16_every_tile_width_and_every_run_gives_the_same_bits(eng, monkeypatch, case):
     B, H, W, Cin, Cout, k, stride, use_res = case
-    g = torch.Generator(device="cpu").manual_seed(11)
-    x = torch.randn(B, H, W, Cin, generator=g).cuda()
-    w = (torch.randn(Cout, Cin, k, k, generator=g) / (Cin * k * k) ** 0.5).cuda()
-    b = torch.randn(Cout, generator=g).cuda()
-    Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
-    res = torch.randn(B, Ho, Wo, Cout, generator=g).cuda() if use_res else None
+    x, w, b, res = _case_tensors(case, seed=11)
     first, n = None, 0
     for tile in ("128,1", "64,1", "32,1"):
         if Cout % int(tile.split(",")[0]):
@@ -224,172 +188,22 @@ def test_finalize_rejects_weights_beyond_the_fp16_range():
 PLAN_GEOMS = [(64, 96, 2), (512, 832, 2), (1024, 1024, 1)]
 
 
-class Weights16:
-    """Per-unit (W, bias, None) as the device holds them in fp16: folded in float64, rounded to fp32 (fold_unit), weights
-    rounded to fp16, biases fp32."""
-
-    mode = "fp16"
-
-    def __init__(self, sd):
-        self.sd, self.cache = sd, {}
-
-    def unit(self, name):
-        if name not in self.cache:
-            g = lambda k: self.sd[name + k].double().cuda()  # noqa: E731
-            s = g(".bn.weight") / torch.sqrt(g(".bn.running_var") + smap_torch.BN_EPS)
-            W = (g(".conv.weight") * s.view(-1, 1, 1, 1)).float().half().double()
-            bias = ((g(".conv.bias") - g(".bn.running_mean")) * s + g(".bn.bias")).float()
-            self.cache[name] = (W, bias, None)
-        return self.cache[name]
-
-    def bias_sum(self, b1, b2):
-        return (b1 + b2).double()
-
-
-def _dims(op):
-    return [int(v) for v in op["out"].split("x")]
-
-
-def dump16(eng, B, op):
-    """Op output on the device: fp16 [N, H, W, C] or fp32 [N, H, W, C] (heads)."""
-    N, H, W, C = _dims(op)
-    t = torch.empty(N, H, W, C, dtype=torch.float32 if op["kind"] == "conv_f32" else torch.float16, device="cuda")
-    nbytes = t.numel() * t.element_size()
-    got = eng.lib.smapb_debug_dump(eng._h, B, op["idx"], ctypes.c_void_p(t.data_ptr()), nbytes, 0)
-    assert got == nbytes, (op["name"], got, nbytes)
-    return t
-
-
-def _s2d_expected16(img):
-    N, _, H, W = img.shape
-    v = img.reshape(N, 3, H // 2, 2, W // 2, 2).permute(0, 2, 4, 3, 5, 1).reshape(N, H // 2, W // 2, 12)
-    return F.pad(v, (0, 4, 2, 1)).half()
-
-
-def check_plan16(H, W, B):
-    from smap_b200.engine import Engine
-
-    _no_tf32()
-    print("\n[plan ops fp16 %dx%d B=%d]" % (H, W, B))
-    sd = smap_torch.make_state_dict(SEED, "random")
-    eng = Engine(0, max_batch=B, in_h=H, in_w=W)
-    worst, failures = {}, []
-    try:
-        eng.load_state_dict(sd, "fp16")
-        eng.forward(smap_torch.make_input(B, H, W, seed=SEED + 1).cuda())
-        img = smap_torch.make_input(B, H, W, seed=SEED + 2).cuda()
-        eng.forward(img)
-        torch.cuda.synchronize()
-        _, ops = plan_ops(eng, B)
-        wts = Weights16(sd)
-        uses = _consumers(ops)
-        live = {}
-        for op in ops:
-            i, cls = op["idx"], op_class(op)
-            if op["kind"] != "conv_f32" and op.get("dtype") != "f16":
-                failures.append("op %d %s: description lacks dtype=f16" % (i, op["name"]))
-            y_raw = dump16(eng, B, op)
-            if uses.get(i):
-                live[i] = y_raw
-            get = lambda role: live[int(op[role])].double()  # noqa: E731
-            if op["kind"] == "s2d":
-                ok = torch.equal(y_raw, _s2d_expected16(img))
-                err, bad = (0.0 if ok else math.inf), ([] if ok else ["s2d not bit-exact"])
-            elif op["kind"] == "maxpool":
-                ok = torch.equal(y_raw.double(), _nhwc(F.max_pool2d(_nchw(get("a")), 3, 2, 1)))
-                err, bad = (0.0 if ok else math.inf), ([] if ok else ["max-pool not bit-exact"])
-            else:
-                y = y_raw.double()
-                r, pre, relu_last = reference(op, get, wts, img)
-                q = reference(op, get, wts, img, squares=True)[0].sqrt()
-                out_round = (lambda t: t.abs() * 2.0 ** -24) if op["kind"] == "conv_f32" else half_ulp16
-                bound = out_round(y[..., :r.shape[-1]]) + _acc_bound(op, q, r, pre)
-                _, bad = x3_error(y, r, pre, relu_last, neg=_acc_bound(op, q, pre))
-                err = ((y[..., :r.shape[-1]] - r).abs() / bound.clamp(min=1e-30)).max().item()
-                if err > 1.0:
-                    bad.append("error %.3g x the bound" % err)
-                if op["kind"] != "conv_f32" and not torch.isfinite(y).all():
-                    bad.append("non-finite activations")
-            worst[cls] = max(worst.get(cls, 0.0), err)
-            if bad:
-                failures.append("op %d %s (%s, bn %s, tw %s): %s" % (i, op["name"], cls, op.get("bn"), op.get("tw"),
-                                                                    "; ".join(bad)))
-            for j in [int(op[r]) for r in ("in", "in2", "res", "p1", "p2", "up", "a", "b") if r in op and op[r] != "x"]:
-                uses[j].remove(i)
-                if not uses[j]:
-                    live.pop(j, None)
-        assert eng.saturation_count() == 0
-    finally:
-        eng.close()
-    torch.cuda.empty_cache()
-    for k in sorted(worst):
-        print("  %-22s %.3g" % (k, worst[k]))
-    return ops, failures
-
-
-@pytest.mark.parametrize("geom", PLAN_GEOMS, ids=lambda g: "%dx%d_b%d" % g)
+@pytest.mark.parametrize("geom", PLAN_GEOMS, ids=_gid)
 def test_plan_ops_fp16(geom):
-    ops, failures = check_plan16(*geom)
-    assert not failures, "\n".join(failures)
-    seen = {op_class(o) for o in ops}
+    s = plan_summary("fp16", geom)
+    assert_checked(s, "fp16")
+    seen = {op_class(o) for o in s["ops"]}
     for need in ("conv1x1", "conv3x3", "residual", "fused_pair_s1", "fused_pair_s2", "up_residual", "res_p1_p2", "head_f32",
                  "tapexp", "stem_tc", "maxpool", "s2d"):
         assert need in seen, "no %s op checked (seen: %s)" % (need, sorted(seen))
 
 
-def _run_sums16(H, W, B, sd, x):
-    from smap_b200.engine import Engine
-
-    eng = Engine(0, max_batch=B, in_h=H, in_w=W)
-    try:
-        eng.load_state_dict(sd, "fp16")
-        outs = [o.cpu() for o in eng.forward(x)]
-        torch.cuda.synchronize()
-        sums, ops = plan_ops(eng, B)
-    finally:
-        eng.close()
-    return sums, ops, outs
-
-
-@pytest.mark.parametrize("geom", [(64, 96, 2), (512, 832, 2)], ids=lambda g: "%dx%d_b%d" % g)
+@pytest.mark.parametrize("geom", [(64, 96, 2), (512, 832, 2)], ids=_gid)
 def test_fp16_plan_switches_keep_the_bits(geom, monkeypatch):
-    from smap_b200 import _lib
     from smap_b200.engine import get_tile_table
 
-    H, W, B = geom
-    sd = smap_torch.make_state_dict(SEED, "random")
-    x = smap_torch.make_input(B, H, W, seed=SEED + 3).cuda()
-    base_sums, base_ops, base_outs = _run_sums16(H, W, B, sd, x)
-
-    def same(tag, sums, ops, outs):
-        assert [o["name"] for o in ops] == [o["name"] for o in base_ops], tag
-        diff = [o["name"] for o, a, b in zip(ops, sums, base_sums) if a != b]
-        assert not diff, "%s: %d ops differ from the default plan, first %s" % (tag, len(diff), diff[:3])
-        for a, b in zip(outs, base_outs):
-            assert torch.equal(a, b), tag
-
-    for var in ("SMAPB_SERPENTINE", "SMAPB_PDL", "SMAPB_ONE_STREAM"):
-        with monkeypatch.context() as m:
-            m.setenv(var, "1")
-            same(var, *_run_sums16(H, W, B, sd, x))
-    lib = _lib.load()
-    table = get_tile_table()
-    assert any(line.split("\t")[0].endswith(" f16") for line in table.splitlines())  # fp16 rows of their own
-    try:
-        for bn in (32, 64, 128):
-            forced = []
-            for line in table.splitlines():
-                key, tbn, cg = line.split("\t")
-                if int(key.split("/")[1]) % bn == 0:
-                    tbn = str(bn)
-                forced.append("\t".join((key, tbn, cg)))
-            lib.smapb_set_tile_table("\n".join(forced).encode() + b"\n")
-            with monkeypatch.context() as m:
-                m.setenv("SMAPB_FORCE_TILE", str(bn))
-                m.setenv("SMAPB_NO_AUTOTUNE", "1")
-                same("SMAPB_FORCE_TILE=%d" % bn, *_run_sums16(H, W, B, sd, x))
-    finally:
-        lib.smapb_set_tile_table(table.encode())
+    check_switches(geom, monkeypatch, "fp16")
+    assert any(line.split("\t")[0].endswith(" f16") for line in get_tile_table().splitlines())  # fp16 rows of their own
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -407,11 +221,11 @@ def test_backbone_fp16_vs_fp32_oracle(H, W, B, bn, capsys):
     sd = smap_torch.make_state_dict(0, bn)
     x = smap_torch.make_input(B, H, W, seed=1).cuda()
     sd_dev = {k: v.cuda() for k, v in sd.items()}
-    _no_tf32()
+    no_tf32()
     ref = smap_torch.smap_forward(sd_dev, x)
     torch.backends.cudnn.allow_tf32 = True  # PyTorch's default: the reference's own SMAP.cuda() convolutions
     tf32 = smap_torch.smap_forward(sd_dev, x)
-    _no_tf32()
+    no_tf32()
     errs = {"tf32": [rel(a, b) for a, b in zip(tf32, ref)]}
     eng = Engine(0, max_batch=B, in_h=H, in_w=W)
     try:
@@ -455,7 +269,7 @@ def test_whole_path_fp16_on_the_bench_batch(capsys):
     from smap_b200 import schema
     from smap_b200.engine import Engine, records_to_numpy, scale_row
 
-    _no_tf32()
+    no_tf32()
     B, H, W = 8, 512, 832
     sd = schema.make_state_dict(0, "identity")
     x = schema.make_input(B, H, W, seed=1).cuda()

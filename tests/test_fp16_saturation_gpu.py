@@ -3,8 +3,8 @@ in all its variants, the CUDA-core stem, s2d, upadd_relu) must store exactly +-6
 inf or NaN, and add one to the handle's saturation counter per clamped element - the counter is the only sign a user gets
 that the outputs are not the model's.
 
-The reference is the float64 one of tests/test_plan_ops_gpu.py (the value before the store, r) with its accumulation
-bound b, and the store's clamp on top.  Elements split three ways:
+The reference is the float64 one of tests/plan_check.py (the value before the store, r) with its accumulation bound b,
+and the store's clamp on top: check_ops in fp16.  Elements split three ways:
   * sure-over, |r| - b > 65504: the output is exactly sign(r) 65504 and the element is counted;
   * sure-in, |r| + b <= 65504: not counted, |y - r| <= 1/2 ulp_fp16(y) + b as before;
   * band, the rest: either outcome, |y - clamp(r)| <= 1/2 ulp_fp16(y) + b.
@@ -33,9 +33,8 @@ import torch.nn.functional as F
 from oracle import lift_numpy, smap_torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_fp16_gpu import FP16_MAX, SEED, Weights16, _no_tf32, _s2d_expected16, dump16, half_ulp16  # noqa: E402
-from test_plan_ops_gpu import (_acc_bound, _consumers, _nchw, _nhwc, check_plan, op_class, plan_ops,  # noqa: E402
-                               reference, x3_error)
+from plan_check import (FP16_MAX, ROLES, SEED, _acc_bound, _consumers, _gid, _nchw, _nhwc, check_ops,  # noqa: E402
+                        check_plan, clamp_check, no_tf32, op_class, plan_ops, split3)
 
 pytestmark = pytest.mark.gpu
 
@@ -47,99 +46,11 @@ PLANS = {
     "cuda_stem_upadd": ({"SMAPB_STEM": "cuda", "SMAPB_NO_FUSE_UP": "1"},
                         ("conv3x3", "residual", "fused_pair_s2", "res_p1_p2", "stem", "upadd")),
 }
-ROLES = ("in", "in2", "res", "p1", "p2", "up", "a", "b")
-
-
-def _gid(g):
-    return "%dx%d_b%d" % (g[1], g[0], g[2])
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the clamping reference
+# the interval of the device count
 # ---------------------------------------------------------------------------------------------------------------------
-def split3(r, b):
-    """-> (sure-over, sure-in, band) masks of reference values r with accumulation bound b."""
-    a = r.abs()
-    over = a - b > FP16_MAX
-    inside = a + b <= FP16_MAX
-    return over, inside, ~(over | inside)
-
-
-def clamp_check(y, r, b):
-    """fp16 outputs y (fp64, real channels) against r: -> (sure-over mask, band mask, worst |y - clamp(r)| / bound,
-    violated conditions)."""
-    over, _, band = split3(r, b)
-    bad = []
-    if not torch.equal(y[over], torch.sign(r[over]) * FP16_MAX):
-        bad.append("%d sure-over elements not stored as +-65504" % int((y[over].abs() != FP16_MAX).sum().item()))
-    bound = half_ulp16(y) + b
-    err = ((y - r.clamp(-FP16_MAX, FP16_MAX)).abs() / bound.clamp(min=1e-30)).max().item()
-    if err > 1.0:
-        bad.append("error %.3g x the bound" % err)
-    return over, band, err, bad
-
-
-def s2d_mapping(img):
-    """The fp32 values s2d stores (before the fp16 rounding): NaN -> -65504, beyond the range -> +-65504."""
-    return torch.where(torch.isnan(img), torch.full_like(img, -FP16_MAX), img).clamp(-FP16_MAX, FP16_MAX)
-
-
-def check_forward16(eng, B, sd, img):
-    """Every op of the batch-B plan as left by the last forward (of img), against the clamping reference.  -> summary
-    dict: sure-over per op class, negative sure-over, band, worst error per class, failures, ops."""
-    _, ops = plan_ops(eng, B)
-    wts = Weights16(sd)
-    uses = _consumers(ops)
-    live = {}
-    over_by, worst, failures = {}, {}, []
-    band = neg = 0
-    for op in ops:
-        i, cls = op["idx"], op_class(op)
-        y_raw = dump16(eng, B, op)
-        if uses.get(i):
-            live[i] = y_raw
-        get = lambda role: live[int(op[role])].double()  # noqa: E731
-        n_over, err, bad = 0, 0.0, []
-        if op["kind"] == "s2d":
-            if not torch.equal(y_raw, _s2d_expected16(s2d_mapping(img))):
-                bad.append("s2d differs from the documented mapping")
-            n_over = int((~(img.abs() <= FP16_MAX)).sum().item())
-        elif op["kind"] == "maxpool":
-            if not torch.equal(y_raw.double(), _nhwc(F.max_pool2d(_nchw(get("a")), 3, 2, 1))):
-                bad.append("max-pool not bit-exact")
-        else:
-            y = y_raw.double()
-            r, pre, relu_last = reference(op, get, wts, img)
-            q = reference(op, get, wts, img, squares=True)[0].sqrt()
-            C = r.shape[-1]
-            b = _acc_bound(op, q, r, pre)
-            _, bad = x3_error(y, r, pre, relu_last, neg=_acc_bound(op, q, pre))
-            if op["kind"] == "conv_f32":  # fp32 heads: no clamp, fed +-65504 inputs
-                err = ((y[..., :C] - r).abs() / (y[..., :C].abs() * 2.0 ** -24 + b).clamp(min=1e-30)).max().item()
-                if err > 1.0:
-                    bad.append("error %.3g x the bound" % err)
-            else:
-                if not torch.isfinite(y).all():
-                    bad.append("non-finite activations")
-                over, bnd, err, more = clamp_check(y[..., :C], r, b)
-                bad += more
-                n_over = int(over.sum().item())
-                neg += int((over & (r < 0)).sum().item())
-                band += int(bnd.sum().item())
-        if n_over:
-            over_by[cls] = over_by.get(cls, 0) + n_over
-        worst[cls] = max(worst.get(cls, 0.0), err)
-        if bad:
-            failures.append("op %d %s (%s, bn %s, tw %s): %s" % (i, op["name"], cls, op.get("bn"), op.get("tw"),
-                                                                "; ".join(bad)))
-        for j in [int(op[r]) for r in ROLES if r in op and op[r] != "x"]:
-            uses[j].remove(i)
-            if not uses[j]:
-                live.pop(j, None)
-    return {"over": over_by, "neg": neg, "band": band, "worst": worst, "failures": failures, "ops": ops,
-            "lo": sum(over_by.values()), "hi": sum(over_by.values()) + band}
-
-
 def report(tag, s, n):
     print("\n[fp16 saturation %s] device count %d in [%d, %d]: band %d, negative sure-over %d" % (tag, n, s["lo"], s["hi"],
                                                                                              s["band"], s["neg"]))
@@ -258,11 +169,11 @@ def _images(B, H, W):
 # 1-2: every fp16-storing op of whole plans
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("plan", list(PLANS))
-@pytest.mark.parametrize("geom", GEOMS, ids=_gid)
+@pytest.mark.parametrize("geom", GEOMS, ids=lambda g: _gid(g, width_first=True))
 def test_plan_saturation_is_clamped_and_counted(geom, plan, monkeypatch):
     from smap_b200.engine import Engine
 
-    _no_tf32()
+    no_tf32()
     H, W, B = geom
     for k, v in PLANS[plan][0].items():
         monkeypatch.setenv(k, v)  # read at plan build
@@ -276,13 +187,13 @@ def test_plan_saturation_is_clamped_and_counted(geom, plan, monkeypatch):
         eng.saturation_count(reset=True)
         outs = eng.forward(img)
         n = eng.saturation_count()
-        s = check_forward16(eng, B, sd, img)
+        s = check_ops(eng, B, sd, img, outs, "fp16")
         for o in outs:
             assert torch.isfinite(o).all()
     finally:
         eng.close()
     torch.cuda.empty_cache()
-    report("%s %s" % (plan, _gid(geom)), s, n)
+    report("%s %s" % (plan, _gid(geom, width_first=True)), s, n)
     print("  targets: %s" % ", ".join("%s%s" % ("-" if sg < 0 else "+", t) for t, sg in targets))
     assert_interval(s, n)
     for cls in PLANS[plan][1]:
@@ -303,7 +214,7 @@ def test_first_forward_of_a_fresh_handle_counts_one_forward(autotune, monkeypatc
     from smap_b200 import _lib
     from smap_b200.engine import Engine, get_tile_table
 
-    _no_tf32()
+    no_tf32()
     H, W, B = GEOMS[0]
     sd, _ = saturating_state_dict(op_graph(H, W, B), "default")
     _, img = _images(B, H, W)
@@ -323,15 +234,15 @@ def test_first_forward_of_a_fresh_handle_counts_one_forward(autotune, monkeypatc
             monkeypatch.setenv("SMAPB_NO_AUTOTUNE", "1")  # read at handle creation
         eng = Engine(0, max_batch=B, in_h=H, in_w=W)
         eng.load_state_dict(sd, "fp16")
-        eng.forward(img)
+        outs = eng.forward(img)
         n = eng.saturation_count()
-        s = check_forward16(eng, B, sd, img)
+        s = check_ops(eng, B, sd, img, outs, "fp16")
         tuned = n_stale - stale()
     finally:
         if eng is not None:
             eng.close()
         lib.smapb_set_tile_table(table.encode())
-    report("fresh handle %s %s" % ("autotune" if autotune else "SMAPB_NO_AUTOTUNE", _gid(GEOMS[0])), s, n)
+    report("fresh handle %s %s" % ("autotune" if autotune else "SMAPB_NO_AUTOTUNE", _gid(GEOMS[0], width_first=True)), s, n)
     print("  fp16 tile-table rows re-measured by this plan build: %d" % tuned)
     if autotune:
         assert tuned > 0, "the plan build did not autotune"
@@ -451,7 +362,7 @@ def test_conv_test_timing_and_timeline_launches_do_not_count(eng16, monkeypatch)
 def eng16():
     from smap_b200.engine import Engine
 
-    _no_tf32()
+    no_tf32()
     e = Engine(0, max_batch=2, in_h=64, in_w=96)
     yield e
     e.close()
@@ -553,7 +464,7 @@ def test_s2d_maps_non_finite_and_out_of_range_pixels():
     so no 7x7 stem window sees two of them and nothing downstream saturates."""
     from smap_b200.engine import Engine
 
-    _no_tf32()
+    no_tf32()
     H, W, B = GEOMS[0]
     sd = smap_torch.make_state_dict(SEED, "random")
     warm, img = _images(B, H, W)
@@ -567,12 +478,12 @@ def test_s2d_maps_non_finite_and_out_of_range_pixels():
         eng.saturation_count(reset=True)
         outs = eng.forward(img)
         n = eng.saturation_count()
-        s = check_forward16(eng, B, sd, img)
+        s = check_ops(eng, B, sd, img, outs, "fp16")
         for o in outs:
             assert torch.isfinite(o).all()
     finally:
         eng.close()
-    report("special pixels %s" % _gid(GEOMS[0]), s, n)
+    report("special pixels %s" % _gid(GEOMS[0], width_first=True), s, n)
     assert s["over"] == {"s2d": n_out}, s["over"]
     assert s["band"] == 0
     assert n == n_out

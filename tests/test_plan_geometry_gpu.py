@@ -1,5 +1,5 @@
-"""GPU: the per-op checkers of tests/test_plan_ops_gpu.py (check_plan) and tests/test_fp16_gpu.py (check_plan16) at the
-input geometries and plan paths no other test builds, and the association at map sizes that take its scalar NMS path.
+"""GPU: the per-op checker of tests/plan_check.py (check_plan), in bf16x3, bf16 and fp16, at the input geometries and
+plan paths no other test builds, and the association at map sizes that take its scalar NMS path.
 
   * edge geometries (in_h x in_w, B): 32x32 B=2 (deepest level 1x1, flat M = 2), 32x992 B=2 (levels one row high),
     1024x32 B=1 (levels one column wide, 64x2 levels tiled tw = 2), 224x288 B=5 (odd levels 7x9 ... 56x72, ragged flat
@@ -27,9 +27,8 @@ from smap_b200 import schema
 from smap_b200.synth import make_scene
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_fp16_gpu import check_plan16  # noqa: E402
-from test_plan_ops_gpu import (SEED, applicable_mutations, check_plan, check_switches, dump, op_class,  # noqa: E402
-                               plan_ops)
+from plan_check import (SEED, _dims, _gid, assert_checked, check_plan, check_switches, dump, op_class,  # noqa: E402
+                        plan_ops, plan_summary)
 
 pytestmark = pytest.mark.gpu
 
@@ -41,68 +40,25 @@ FALLBACK_RUNS = [("bf16x3", (32, 32, 2)), ("fp16", (32, 32, 2)), ("bf16x3", (96,
                  ("bf16x3", (512, 832, 2))]
 
 
-def _gid(g):
-    return "%dx%d_b%d" % g
-
-
-def _dims(op):
-    return [int(v) for v in op["out"].split("x")]
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # per-op parity
 # ---------------------------------------------------------------------------------------------------------------------
-_RUNS = {}
-
-
-def plan_check(precision, geom, fallback=None):
-    """{"ops", "failures", "flagged"} of one per-op check (flagged: None in fp16, whose checker has no wrong references).
-    Each check runs once per session; the coverage test reads the same runs."""
-    key = (precision, geom, fallback)
-    if key not in _RUNS:
-        try:
-            with pytest.MonkeyPatch.context() as m:
-                if fallback:
-                    m.setenv(*FALLBACKS[fallback])  # read by build_plan, on the handle's first forward
-                if precision == "fp16":
-                    ops, failures = check_plan16(*geom)
-                    _RUNS[key] = {"ops": ops, "failures": failures, "flagged": None}
-                else:
-                    _RUNS[key] = check_plan(precision, *geom)
-        except Exception as e:  # noqa: BLE001 - re-raised for every test that reads this run
-            _RUNS[key] = e
-    s = _RUNS[key]
-    if isinstance(s, Exception):
-        raise s
-    return s
-
-
-def _assert_checked(s, precision):
-    assert not s["failures"], "\n".join(s["failures"])
-    if s["flagged"] is None:
-        return
-    want = applicable_mutations(s["ops"], precision)
-    assert set(s["flagged"]) == want, "wrong references never tried: %s" % sorted(want - set(s["flagged"]))
-    missed = sorted(m for m, f in s["flagged"].items() if not f)
-    assert not missed, "wrong references the checker accepted: %s" % missed
-
-
 @pytest.mark.parametrize("geom", EDGE_GEOMS, ids=_gid)
 def test_edge_geometry_ops_bf16x3(geom):
-    _assert_checked(plan_check("bf16x3", geom), "bf16x3")
+    assert_checked(plan_summary("bf16x3", geom), "bf16x3")
 
 
 @pytest.mark.parametrize("geom", SMALL_GEOMS, ids=_gid)
 @pytest.mark.parametrize("precision", ["bf16", "fp16"])
 def test_edge_geometry_ops_bf16_fp16(precision, geom):
-    _assert_checked(plan_check(precision, geom), precision)
+    assert_checked(plan_summary(precision, geom), precision)
 
 
 @pytest.mark.parametrize("precision,geom", FALLBACK_RUNS, ids=["%s_%s" % (p, _gid(g)) for p, g in FALLBACK_RUNS])
 @pytest.mark.parametrize("fallback", sorted(FALLBACKS))
 def test_fallback_plan_ops(fallback, precision, geom):
-    s = plan_check(precision, geom, fallback)
-    _assert_checked(s, precision)
+    s = plan_summary(precision, geom, FALLBACKS[fallback])
+    assert_checked(s, precision)
     ops = s["ops"]
     kinds, classes = {o["kind"] for o in ops}, {op_class(o) for o in ops}
     if fallback == "stem_cuda":  # the CUDA-core stem replaces s2d + the tensor-core stem
@@ -117,9 +73,9 @@ def test_fallback_plan_ops(fallback, precision, geom):
 
 def test_edge_plans_cover_what_they_are_for():
     """Across this file's checked plans: 1-pixel levels, images smaller than one tile, tw = 2, and the fallback kinds."""
-    runs = [plan_check("bf16x3", g) for g in EDGE_GEOMS]
-    runs += [plan_check(p, g) for p in ("bf16", "fp16") for g in SMALL_GEOMS]
-    runs += [plan_check(p, g, f) for f in sorted(FALLBACKS) for p, g in FALLBACK_RUNS]
+    runs = [plan_summary("bf16x3", g) for g in EDGE_GEOMS]
+    runs += [plan_summary(p, g) for p in ("bf16", "fp16") for g in SMALL_GEOMS]
+    runs += [plan_summary(p, g, FALLBACKS[f]) for f in sorted(FALLBACKS) for p, g in FALLBACK_RUNS]
     seen = set()
     for s in runs:
         ops = s["ops"]
@@ -154,7 +110,7 @@ def test_edge_plans_cover_what_they_are_for():
 def test_edge_geometry_plan_switches_keep_the_bits(geom, monkeypatch):
     """Reverse tile order, PDL, one stream and every forced tile width (tile table rewritten, autotuner off) give the
     bits of the autotuned plan."""
-    check_switches(geom, monkeypatch)
+    check_switches(geom, monkeypatch, "bf16x3")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -195,7 +151,7 @@ def test_smaller_batches_give_every_op_the_same_bits(H, W):
             for a, b in zip(outs, outs5):
                 assert torch.equal(_bits(a), _bits(b[lo:hi])), "B=%d: returned tensors differ" % B
         del full
-        _assert_checked(check_plan("bf16x3", H, W, 3, eng=eng), "bf16x3")
+        assert_checked(check_plan("bf16x3", H, W, 3, eng=eng), "bf16x3")
     finally:
         eng.close()
     torch.cuda.empty_cache()
