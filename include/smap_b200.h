@@ -93,6 +93,16 @@ int smapb_jpeg_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* or
  * captured into a CUDA graph. */
 int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
                       int* status_host, void* stream);
+/* Flags of the _ex forms; 0 = exactly smapb_jpeg_info / smapb_decode_jpeg.
+ * SMAPB_JPEG_SCANS also accepts sequential files (SOF0/SOF1) with several scans (every component in exactly one) and
+ * progressive Huffman files (SOF2) whose progression libjpeg accepts without a warning and whose coefficients 1..9 are
+ * fully refined in every component (otherwise libjpeg-turbo smooths the output, and the file is left to cv2), with at
+ * most 64 scans and no DQT redefining a table a scan already used.  One call decodes a mixed batch (single-scan,
+ * multi-scan and refused files); the status codes, the shape rule and the synchronisation are those of the plain forms. */
+#define SMAPB_JPEG_SCANS 1
+int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status);
+int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                         int flags, int* status_host, void* stream);
 
 /* ---- backbone -------------------------------------------------------------------------------- */
 /* Replaces: SMAP.forward inference branch (model/smap.py:403-419).

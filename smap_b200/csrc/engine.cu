@@ -1703,12 +1703,24 @@ int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, i
     return smapb_preprocess(h, h->pre_stage, img_h, img_w, out_nchw_dev, scale_row_host, stream);
 }
 
-int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
-                      int* status_host, void* stream) {
+int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                         int flags, int* status_host, void* stream) {
     if (!h) return -1;
+    if (flags & ~SMAPB_JPEG_SCANS) {
+        h->err = "smapb_decode_jpeg_ex: unknown flags";
+        return -1;
+    }
     cudaSetDevice(h->device);
     if (!h->jpeg) h->jpeg = smapb::jpeg_workspace_create();
+    if (flags & SMAPB_JPEG_SCANS)
+        return smapb::jpeg_decode_scans(h->jpeg, n, jpeg_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches,
+                                        &h->err);
     return smapb::jpeg_decode(h->jpeg, n, jpeg_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                      int* status_host, void* stream) {
+    return smapb_decode_jpeg_ex(h, n, jpeg_host, nbytes, bgr_dev, 0, status_host, stream);
 }
 
 // host-only introspection of the resampling plan (tests compare it with the oracle over many geometries without a GPU)

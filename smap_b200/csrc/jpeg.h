@@ -17,5 +17,9 @@ void jpeg_workspace_destroy(JpegWorkspace* ws);
 // -1 for bad arguments, with the text in *err.  *launches is incremented by the number of kernels launched.
 int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int* status,
                 cudaStream_t st, int64_t* launches, std::string* err);
+// The same for a batch that may also hold sequential files with several scans and progressive Huffman files
+// (SMAPB_JPEG_SCANS): the scans run in rounds, the r-th scan of every image in round r.
+int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr,
+                      int* status, cudaStream_t st, int64_t* launches, std::string* err);
 
 }  // namespace smapb

@@ -59,13 +59,22 @@ def get_tile_table():
     return buf.value.decode()
 
 
-def jpeg_info(data):
+JPEG_SCANS = 1  # SMAPB_JPEG_SCANS
+
+
+def jpeg_info(data, scans=False):
     """Header walk of one JPEG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
-    handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h)."""
+    handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h).
+    scans=True: the walk of Engine.decode_jpeg_ex, which also takes multi-scan sequential and progressive files."""
     h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    rc = _lib.load().smapb_jpeg_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
+    lib = _lib.load()
+    if scans:
+        rc = lib.smapb_jpeg_info_ex(bytes(data), len(data), JPEG_SCANS, ctypes.byref(h), ctypes.byref(w), ctypes.byref(o),
+                                    ctypes.byref(st))
+    else:
+        rc = lib.smapb_jpeg_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
     if rc != 0:
-        raise SmapB200Error("smapb_jpeg_info failed (%d)" % rc)
+        raise SmapB200Error("%s failed (%d)" % ("smapb_jpeg_info_ex" if scans else "smapb_jpeg_info", rc))
     return st.value, h.value, w.value, o.value
 
 
@@ -213,6 +222,28 @@ class Engine:
         sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
         status = (ctypes.c_int * n)()
         self._check(self.lib.smapb_decode_jpeg(self._h, n, data, sizes, ptrs, status, self._st()), "smapb_decode_jpeg")
+        return [o if status[i] == 0 else None for i, o in enumerate(out)]
+
+    def decode_jpeg_ex(self, files, scans=True):
+        """decode_jpeg for a batch that may also hold progressive Huffman files and sequential files with several scans
+        (smapb_decode_jpeg_ex with SMAPB_JPEG_SCANS; scans=False is decode_jpeg).  -> per file a CUDA uint8 BGR [H,W,3]
+        tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None (cv2 must read it)."""
+        n = len(files)
+        out = [None] * n
+        if n == 0:
+            return out
+        ptrs = (ctypes.c_void_p * n)()
+        for i, f in enumerate(files):
+            st, h, w = jpeg_info(f, scans)[:3]
+            if st == 0:
+                out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
+                ptrs[i] = out[i].data_ptr()
+        data = (ctypes.c_char_p * n)(*files)
+        sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
+        status = (ctypes.c_int * n)()
+        flags = JPEG_SCANS if scans else 0
+        self._check(self.lib.smapb_decode_jpeg_ex(self._h, n, data, sizes, ptrs, flags, status, self._st()),
+                    "smapb_decode_jpeg_ex")
         return [o if status[i] == 0 else None for i, o in enumerate(out)]
 
     # ---- pre-processing ------------------------------------------------------------------------

@@ -4,7 +4,9 @@ A seeded in-memory corpus of q90 4:2:0 frames written by cv2 (1920x1080 and 4032
 photo-like entropy of roughly 1-2 bits per pixel) is decoded
   1. by Engine.decode_jpeg in batches of --batch (host parse, upload, every phase, status read-back: the whole call),
   2. by cv2.imdecode on one thread, and on a pool of all host cores,
-in images/s and Mpixel/s; then the run_inference loop from file bytes to skeleton records (decode, preprocess, infer_device,
+in images/s and Mpixel/s.  The same q90 4:2:0 frames written progressive by cv2 (libjpeg's default 10-scan script) are
+decoded by Engine.decode_jpeg_ex against cv2, with the share of kernel time that goes to the AC refinement scans (one
+thread per restart segment; these files have no restart markers) from torch.profiler.  Then the run_inference loop from file bytes to skeleton records (decode, preprocess, infer_device,
 records to the host) is timed in bf16x3 and fp16 with each decoder (cv2 on one thread is what the CLI did before).  The
 GPU's name and power limit are read in the same call.
 
@@ -28,6 +30,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from jpeg_corpus import content, cv2_jpeg  # noqa: E402
+from jpeg_scans import cv2_progressive  # noqa: E402
 from smap_b200 import schema  # noqa: E402
 from smap_b200.engine import RECORD_BYTES, Engine  # noqa: E402
 
@@ -39,9 +42,34 @@ def gpu_info():
     return name.strip() or torch.cuda.get_device_name(0), power.strip()
 
 
-def make_corpus(h, w, n, seed):
+def sm_clock():
+    """SM clock (MHz) now, read right after a timed loop."""
+    q = subprocess.run(["nvidia-smi", "-i", os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0],
+                        "--query-gpu=clocks.sm", "--format=csv,noheader,nounits"], capture_output=True, text=True)
+    return q.stdout.strip()
+
+
+def make_corpus(h, w, n, seed, progressive=False):
     rng = np.random.default_rng(seed)
-    return [cv2_jpeg(content("smooth", h, w, rng), 90, "420") for _ in range(n)]
+    enc = cv2_progressive if progressive else cv2_jpeg
+    return [enc(content("smooth", h, w, rng), 90, "420") for _ in range(n)]
+
+
+def refine_share(eng, files):
+    """Share of the decode call's kernel time spent in ac_refine_kernel (torch.profiler, one call)."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        eng.decode_jpeg_ex(files)
+        torch.cuda.synchronize()
+    tot = ref = 0.0
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+        if "kernel" in e.key and "Memcpy" not in e.key and "Memset" not in e.key:
+            tot += t
+            if "ac_refine_kernel" in e.key:
+                ref += t
+    return round(ref / tot, 3) if tot else None
 
 
 def cv2_decode(b):
@@ -84,18 +112,33 @@ def main():
             t = timed(fn, a.rounds)
             row[arm] = {"images_per_s": round(len(files) / t, 1), "mpixel_per_s": round(mpx / t, 1)}
         out["decode"][key] = row
+    for key, (h, w, seed) in {"prog_1920x1080": (1080, 1920, 3), "prog_4032x3024": (3024, 4032, 4)}.items():
+        files = make_corpus(h, w, B, seed, progressive=True)
+        mpx = sum(int(np.prod(cv2_decode(f).shape[:2])) for f in files) / 1e6
+        assert all(o is not None for o in eng.decode_jpeg_ex(files))
+        row = {"mbytes_per_image": round(sum(map(len, files)) / len(files) / 1e6, 3)}
+        for arm, fn in (("gpu", lambda: eng.decode_jpeg_ex(files)),
+                        ("cv2_1_thread", lambda: [cv2_decode(f) for f in files]),
+                        ("cv2_%d_threads" % cores, lambda: list(pool.map(cv2_decode, files)))):
+            t = timed(fn, a.rounds)
+            row[arm] = {"images_per_s": round(len(files) / t, 1), "mpixel_per_s": round(mpx / t, 1)}
+        eng.decode_jpeg_ex(files)
+        row["sm_clock_mhz_after_gpu_arm"] = sm_clock()
+        row["ac_refine_share_of_kernel_time"] = refine_share(eng, files)
+        out["decode"][key] = row
     # the CLI loop: bytes -> records, 4 batches of 1920x1080 frames per round
     files = corpora["1920x1080"] * 4
+    prog = make_corpus(1080, 1920, B, 3, progressive=True) * 4
     host = torch.empty(B, RECORD_BYTES, dtype=torch.uint8).pin_memory()
     sd = schema.make_state_dict(0, "identity")
     for prec in ("bf16x3", "fp16"):
         eng.load_state_dict(sd, prec)
 
-        def loop(gpu_decode):
+        def loop(gpu_decode, files=files, decode=eng.decode_jpeg):
             for lo in range(0, len(files), B):
                 chunk = files[lo:lo + B]
                 if gpu_decode:
-                    frames = eng.decode_jpeg(chunk)
+                    frames = decode(chunk)
                 else:
                     frames = [torch.from_numpy(cv2_decode(f)) for f in chunk]
                 imgs, scales = eng.preprocess(frames)
@@ -107,6 +150,9 @@ def main():
         for arm, flag in (("gpu_decode", True), ("cv2_1_thread", False)):
             t = timed(lambda: loop(flag), a.rounds)
             row[arm] = {"frames_per_s": round(len(files) / t, 1)}
+        for arm, flag in (("progressive_gpu_decode", True), ("progressive_cv2_1_thread", False)):
+            t = timed(lambda: loop(flag, prog, eng.decode_jpeg_ex), a.rounds)
+            row[arm] = {"frames_per_s": round(len(prog) / t, 1)}
         out["cli"][prec] = row
     eng.close()
     pool.shutdown()
