@@ -44,8 +44,9 @@ int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dim
  *                             real step (tools/roles_plan.py)
  *   SMAPB_TIMELINE=1          clock64 time line of CTA 0 of one launch in smapb_conv_test (set-up, first operands, last main loop end,
  *                             epilogue done, exit)
- *   SMAPB_JPEG_SUB_BITS=n     subsequence length (bits, a multiple of 32) of multi-scan JPEG decoding (smapb_decode_jpeg_ex);
- *                             default 512; short ones make blocks and EOB runs cross subsequence boundaries in tests
+ *   SMAPB_JPEG_SUB_BITS=n     subsequence length (bits, a multiple of 32) of the Huffman passes of every JPEG decode
+ *                             (smapb_decode_jpeg[_ex]); default 512; short ones make blocks and EOB runs cross subsequence
+ *                             boundaries in tests
  *   SMAPB_LIB=path (Python)   load another build of the library (A/B runs: tools/ab_hash.py) */
 
 #ifdef __cplusplus

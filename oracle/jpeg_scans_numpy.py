@@ -3,7 +3,7 @@ several scans and progressive Huffman files (ITU-T T.81 Annex G: DC first and re
 refinement, non-interleaved scans on the component's own block grid).  The IDCT, upsampling, colour conversion and
 orientation are jpeg_numpy's; so is the coefficient layout (frame MCU by frame MCU) that feeds them.
 
-    hd = parse(data)                  # every scan up to EOI, the acceptance rules of jpeg_parse_scans; NotDecoded otherwise
+    hd = parse(data)                  # every scan up to EOI, jpeg_parse's rules with SMAPB_JPEG_SCANS; NotDecoded otherwise
     coef = entropy_decode(data, hd)   # int16 [nmcu * blocks_per_mcu, 64] after every scan
     decode(data)                      # -> uint8 BGR as cv2.imread returns it
 """

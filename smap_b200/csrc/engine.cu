@@ -1712,10 +1712,8 @@ int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host
     }
     cudaSetDevice(h->device);
     if (!h->jpeg) h->jpeg = smapb::jpeg_workspace_create();
-    if (flags & SMAPB_JPEG_SCANS)
-        return smapb::jpeg_decode_scans(h->jpeg, n, jpeg_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches,
-                                        &h->err);
-    return smapb::jpeg_decode(h->jpeg, n, jpeg_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
+    return smapb::jpeg_decode(h->jpeg, n, jpeg_host, nbytes, bgr_dev, flags, status_host, (cudaStream_t)stream, &h->launches,
+                              &h->err);
 }
 
 int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,

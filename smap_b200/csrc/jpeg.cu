@@ -1,30 +1,31 @@
-// Baseline (SOF0/SOF1, Huffman, 8-bit) JPEG decoding on the GPU, byte-identical to cv2.imread(path, IMREAD_COLOR).
+// Huffman, 8-bit JPEG decoding on the GPU, byte-identical to cv2.imread(path, IMREAD_COLOR).
 //
-// Host: a bounds-checked marker walk (jpeg_parse) builds the Huffman and quantisation tables, the restart segments and the
-// EXIF orientation; anything it does not accept gets a status and is left to the caller's cv2 path.  Device: one launch
-// per phase for every image of the batch:
-//   a. unstuff_kernel     removes the FF00 stuffing and the RSTn markers (restart segments are byte ranges the host found)
-//   b. huff_sync_kernel   self-synchronising Huffman decoding (Weissenberger & Schmidt, ICPP 2018 / HiPC 2021): every
-//                         segment is cut into SUB_BITS-bit subsequences, each decoded speculatively from a guessed state;
+// Host: one bounds-checked marker walk (jpeg_parse) yields the frame (geometry, quantisers, EXIF orientation) and one
+// ScanSpec per scan (the tables in force at its SOS, its band, its restart segments); anything it does not accept gets a
+// status and is left to the caller's cv2 path.  Without SMAPB_JPEG_SCANS it accepts baseline files only: one interleaved
+// sequential scan (SOF0/SOF1) of every component, then EOI.  With it, it also accepts sequential files with several scans
+// and progressive Huffman files (SOF2): it walks every scan up to EOI, checks the progression as libjpeg does, latches each
+// component's quantiser at its first scan, refuses what libjpeg-turbo would smooth (coefficients 1..9 not fully refined)
+// and caps the scans at 64.
+//
+// Device: the coefficient buffer is zeroed once, then the scans run in rounds: round r decodes the r-th scan of every image
+// (a baseline batch is one round), one launch per phase:
+//   a. unstuff_kernel     removes the FF00 stuffing and the RSTn markers of every scan (restart segments are byte ranges
+//                         the host found)
+//   b. Huffman scans (sequential, DC first, AC first with EOB runs), on the scan's own MCU (a non-interleaved scan walks
+//      the component's block grid):
+//      scan_sync_kernel   self-synchronising Huffman decoding (Weissenberger & Schmidt, ICPP 2018 / HiPC 2021): every
+//                         segment is cut into sub_bits-bit subsequences, each decoded speculatively from a guessed state;
 //                         sync passes restart a subsequence from its predecessor's exit state until every start state
 //                         equals its predecessor's exit state (the state: bit position, block within the MCU, zig-zag index)
-//      huff_prefix_kernel prefix sum of the blocks each subsequence completes -> output positions; per-segment checks
-//      huff_write_kernel  the final pass: coefficients into their blocks (DC as differences)
-//      dc_scan_kernel     DC prediction: a scan per component, reset at every restart
+//      scan_prefix_kernel prefix sum of the blocks each subsequence completes -> output positions; per-segment checks
+//      scan_write_kernel  the final pass: coefficients into their blocks (DC as differences)
+//      scan_dc_kernel     DC prediction: a scan per component, reset at every restart
+//      dc_refine_kernel   one raw bit per block at a position known from the block's index in its restart segment
+//      ac_refine_kernel   one thread per restart segment: the bits a block takes depend on its nonzero history
 //   c. idct_kernel        dequantisation + accurate-integer IDCT (LL&M, 13-bit constants, 2 pass-1 bits), saturated
 //   d. colour_kernel      fancy upsampling, fixed-point YCbCr -> BGR, EXIF orientation, uint8 HWC BGR
-// oracle/jpeg_numpy.py restates every stage on the CPU.
-//
-// Multi-scan files (smapb_decode_jpeg_ex with SMAPB_JPEG_SCANS; jpeg_decode_scans): jpeg_parse_scans walks every scan up
-// to EOI and checks the progression as libjpeg does. It keeps the Huffman tables in force at each SOS and latches each
-// component's quantiser at its first scan. It refuses what libjpeg-turbo would smooth (coefficients 1..9 not fully
-// refined), and caps the scans at 64. The coefficient buffer is zeroed once, then the scans run in rounds: round r
-// decodes the r-th scan of every image, one launch per phase:
-//   Huffman scans (sequential, DC first, AC first with EOB runs): scan_sync / scan_prefix / scan_write, as in b, on the
-//                         scan's own MCU (a non-interleaved scan walks the component's block grid), then scan_dc
-//   dc_refine_kernel      one raw bit per block at a position known from the block's index in its restart segment
-//   ac_refine_kernel      one thread per restart segment: the bits a block takes depend on its nonzero history
-// then c and d as above.  oracle/jpeg_scans_numpy.py restates the multi-scan entropy decoding.
+// oracle/jpeg_numpy.py restates every stage on the CPU, oracle/jpeg_scans_numpy.py the multi-scan entropy decoding.
 #include <stdlib.h>
 #include <string.h>
 
@@ -58,29 +59,26 @@ struct DevHuff {
 };
 
 struct DevImage {
-    int h, w, out_h, out_w, orientation, ncomp, hmax, vmax, mcux, mcuy, nmcu, bpm, per, nseg;
-    int seg0, sub0, nsub;
+    int h, w, out_h, out_w, orientation, ncomp, hmax, vmax, mcux, mcuy, nmcu, bpm;
     int blk_comp[6], blk_dx[6], blk_dy[6];
     int comp_h[3], comp_v[3];
     int plane_w[3], plane_h[3];
-    int64_t raw_off, raw_len, unst_off, coef_off, plane_off[3];
+    int64_t coef_off, plane_off[3];
     uint8_t* out;
     int16_t qt[3][64];  // natural order (values > 32767 are rejected on the host)
-    DevHuff dc[3], ac[3];
 };
 
+// A restart segment of a scan; first_mcu / nmcu count the scan's MCUs (single blocks when it is not interleaved).
 struct DevSeg {
-    int img, sub0, nsub, first_mcu, nmcu;
-    uint32_t bit_begin, bit_end;  // relative to the image's unstuffed data
+    int scan, sub0, nsub, first_mcu, nmcu;
+    uint32_t bit_begin, bit_end;  // relative to the scan's unstuffed data
 };
 
 struct DevSub {
-    int img, seg;
+    int scan, seg;
     uint32_t bit_begin, bit_end;
 };
 
-// One scan of a multi-scan decode (SMAPB_JPEG_SCANS).  In that path DevSeg::img and DevSub::img hold the scan's index, and
-// DevSeg::first_mcu / nmcu count the scan's MCUs (single blocks when it is not interleaved).
 enum ScanKind { SCAN_HUFF = 0, SCAN_DC_REFINE = 1, SCAN_AC_REFINE = 2 };
 
 struct DevScan {
@@ -88,7 +86,7 @@ struct DevScan {
     int ss, se, al;
     int h, v, j0;                 // not interleaved: the component's sampling factors and first block within the frame's MCU
     int blk_comp[6], blk_map[6];  // block of the scan's MCU -> scan component, -> block of the frame's MCU (interleaved)
-    int dc[3], ac[3];             // tables of each scan component (indices into the batch's table array)
+    int blk_dc[6], blk_ac[6];     // -> its tables (indices into the batch's table array)
     int seg0, nseg, sub0, nsub;
     int64_t raw_off, raw_len, unst_off;
 };
@@ -117,11 +115,7 @@ struct Header {
     int dri = 0;
     int comp_h[3] = {1, 1, 1}, comp_v[3] = {1, 1, 1};
     uint16_t qt[3][64];
-    const HuffSpec* dc[3];
-    const HuffSpec* ac[3];
-    HuffSpec dht[2][4];
-    std::vector<int64_t> seg_begin, seg_end;  // raw byte ranges of the restart segments
-    std::vector<int64_t> seg_stuffed;         // FF00 pairs inside each segment
+    HuffSpec dht[2][4];  // the tables defined so far
 };
 
 inline int u16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
@@ -181,168 +175,6 @@ bool build_huff(const HuffSpec& s, DevHuff* d) {
     return true;
 }
 
-int jpeg_parse(const uint8_t* d, int64_t n, Header* H) {
-    if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return SMAPB_JPEG_MALFORMED;
-    int64_t p = 2;
-    const uint8_t* qt[4] = {nullptr, nullptr, nullptr, nullptr};
-    int qprec[4] = {0, 0, 0, 0};
-    bool sof = false, jfif = false, adobe = false, have_orient = false;
-    int adobe_transform = 0, ids[3] = {0, 0, 0}, tq[3] = {0, 0, 0};
-    const uint8_t* s = nullptr;
-    int64_t L = 0;
-    for (;;) {
-        if (p + 2 > n || d[p] != 0xFF) return SMAPB_JPEG_MALFORMED;
-        while (p + 1 < n && d[p + 1] == 0xFF) p++;
-        if (p + 2 > n) return SMAPB_JPEG_MALFORMED;
-        const int m = d[p + 1];
-        p += 2;
-        if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SMAPB_JPEG_MALFORMED;
-        if (p + 2 > n) return SMAPB_JPEG_MALFORMED;
-        L = u16(d + p);
-        if (L < 2 || p + L > n) return SMAPB_JPEG_MALFORMED;
-        s = d + p + 2;
-        L -= 2;
-        p += L + 2;
-        if (m == 0xDB) {
-            for (int64_t i = 0; i < L;) {
-                const int pq = s[i] >> 4, t = s[i] & 15;
-                if (pq > 1 || t > 3 || i + 1 + 64 * (pq + 1) > L) return SMAPB_JPEG_MALFORMED;
-                qt[t] = s + i + 1;
-                qprec[t] = pq;
-                i += 1 + 64 * (pq + 1);
-            }
-        } else if (m == 0xC4) {
-            for (int64_t i = 0; i < L;) {
-                if (i + 17 > L) return SMAPB_JPEG_MALFORMED;
-                const int tc = s[i] >> 4, th = s[i] & 15;
-                int tot = 0;
-                for (int j = 0; j < 16; j++) tot += s[i + 1 + j];
-                if (tc > 1 || th > 3 || tot > 256 || i + 17 + tot > L) return SMAPB_JPEG_MALFORMED;
-                HuffSpec& hs = H->dht[tc][th];
-                memcpy(hs.counts, s + i + 1, 16);
-                memset(hs.vals, 0, 256);
-                memcpy(hs.vals, s + i + 17, tot);
-                hs.nvals = tot;
-                hs.defined = true;
-                i += 17 + tot;
-            }
-        } else if (m == 0xDD) {
-            if (L != 2) return SMAPB_JPEG_MALFORMED;
-            H->dri = u16(s);
-        } else if (m == 0xC0 || m == 0xC1) {
-            if (sof || L < 6) return SMAPB_JPEG_MALFORMED;
-            sof = true;
-            const int prec = s[0], nf = s[5];
-            H->h = u16(s + 1), H->w = u16(s + 3);
-            if (L != 6 + 3 * nf) return SMAPB_JPEG_MALFORMED;
-            if (prec != 8 || H->h == 0 || H->w == 0 || (nf != 1 && nf != 3)) return SMAPB_JPEG_UNSUPPORTED;
-            H->ncomp = nf;
-            for (int c = 0; c < nf; c++) {
-                ids[c] = s[6 + 3 * c];
-                H->comp_h[c] = s[7 + 3 * c] >> 4;
-                H->comp_v[c] = s[7 + 3 * c] & 15;
-                tq[c] = s[8 + 3 * c];
-                if (tq[c] > 3) return SMAPB_JPEG_MALFORMED;
-                for (int e = 0; e < c; e++)
-                    if (ids[e] == ids[c]) return SMAPB_JPEG_MALFORMED;
-            }
-            if (nf == 1) {
-                H->comp_h[0] = H->comp_v[0] = 1;  // one component: one block per MCU whatever its factors say
-            } else {
-                const bool ok = (H->comp_h[0] == 1 || H->comp_h[0] == 2) && (H->comp_v[0] == 1 || H->comp_v[0] == 2) &&
-                                H->comp_h[1] == 1 && H->comp_v[1] == 1 && H->comp_h[2] == 1 && H->comp_v[2] == 1;
-                if (!ok) return SMAPB_JPEG_UNSUPPORTED;
-            }
-        } else if (m >= 0xC2 && m <= 0xCF) {
-            return SMAPB_JPEG_UNSUPPORTED;  // progressive, lossless, arithmetic, hierarchical, DAC, JPG
-        } else if (m == 0xE0) {
-            if (L >= 14 && memcmp(s, "JFIF\0", 5) == 0) jfif = true;
-        } else if (m == 0xEE) {
-            if (L >= 12 && memcmp(s, "Adobe", 5) == 0) adobe = true, adobe_transform = s[11];
-        } else if (m == 0xE1) {
-            const int o = exif_orientation(s, L);
-            if (o < 0) return SMAPB_JPEG_UNSUPPORTED;
-            if (o > 0) {
-                if (have_orient) return SMAPB_JPEG_UNSUPPORTED;
-                have_orient = true;
-                H->orientation = o;
-            }
-        } else if ((m >= 0xE2 && m <= 0xEF) || m == 0xFE) {
-        } else if (m == 0xDA) {
-            break;
-        } else {
-            return SMAPB_JPEG_UNSUPPORTED;
-        }
-    }
-    // SOS: one interleaved scan of every component, in frame order, sequential parameters
-    if (!sof) return SMAPB_JPEG_MALFORMED;
-    const int nf = H->ncomp;
-    if (L < 1 || s[0] != nf || L != 4 + 2 * nf) return SMAPB_JPEG_UNSUPPORTED;
-    for (int c = 0; c < nf; c++) {
-        if (s[1 + 2 * c] != ids[c]) return SMAPB_JPEG_UNSUPPORTED;
-        const int td = s[2 + 2 * c] >> 4, ta = s[2 + 2 * c] & 15;
-        if (td > 3 || ta > 3 || !H->dht[0][td].defined || !H->dht[1][ta].defined || !qt[tq[c]]) return SMAPB_JPEG_UNSUPPORTED;
-        const HuffSpec& dcs = H->dht[0][td];
-        for (int i = 0; i < dcs.nvals; i++)
-            if (dcs.vals[i] > 15) return SMAPB_JPEG_MALFORMED;
-        H->dc[c] = &H->dht[0][td];
-        H->ac[c] = &H->dht[1][ta];
-        for (int k = 0; k < 64; k++) {
-            const uint8_t* q = qt[tq[c]];
-            const int v = qprec[tq[c]] ? u16(q + 2 * k) : q[k];
-            if (v > 32767) return SMAPB_JPEG_UNSUPPORTED;
-            H->qt[c][h_zigzag[k]] = (uint16_t)v;
-        }
-    }
-    if (s[1 + 2 * nf] != 0 || s[2 + 2 * nf] != 63 || s[3 + 2 * nf] != 0) return SMAPB_JPEG_UNSUPPORTED;
-    if (nf == 3) {
-        // libjpeg's colour-space rule for 3 components: a JFIF APP0 means YCbCr; else an Adobe APP14 means RGB when its
-        // transform flag is 0 and YCbCr otherwise; else component ids 'R','G','B' mean RGB, anything else YCbCr
-        bool ycc;
-        if (jfif) ycc = true;
-        else if (adobe) ycc = adobe_transform != 0;
-        else ycc = !(ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B');
-        if (!ycc) return SMAPB_JPEG_UNSUPPORTED;
-    }
-    if ((int64_t)H->h * H->w > SMAPB_JPEG_MAX_PIXELS) return SMAPB_JPEG_TOO_LARGE;
-    H->hmax = H->comp_h[0], H->vmax = H->comp_v[0];
-    H->mcux = (H->w + 8 * H->hmax - 1) / (8 * H->hmax);
-    H->mcuy = (H->h + 8 * H->vmax - 1) / (8 * H->vmax);
-    H->nmcu = H->mcux * H->mcuy;
-    const int nseg = H->dri ? (H->nmcu + H->dri - 1) / H->dri : 1;
-    // entropy-coded data: FF00 = stuffed FF, FFD0..D7 = restart marker in sequence, FFD9 = end; anything else is refused
-    int64_t start = p, q = p, stuffed = 0;
-    for (;;) {
-        const uint8_t* f = (const uint8_t*)memchr(d + q, 0xFF, (size_t)(n - q));
-        if (!f || f + 1 >= d + n) return SMAPB_JPEG_MALFORMED;
-        q = f - d;
-        const int m = d[q + 1];
-        if (m == 0) {
-            stuffed++;
-            q += 2;
-            continue;
-        }
-        if (m >= 0xD0 && m <= 0xD7) {
-            if (!H->dri || m - 0xD0 != (int)(H->seg_begin.size() % 8) || (int)H->seg_begin.size() + 1 >= nseg)
-                return SMAPB_JPEG_CORRUPT;
-        } else if (m != 0xD9) {
-            return SMAPB_JPEG_UNSUPPORTED;
-        }
-        H->seg_begin.push_back(start);
-        H->seg_end.push_back(q);
-        H->seg_stuffed.push_back(stuffed);
-        if (m == 0xD9) break;
-        start = q = q + 2;
-        stuffed = 0;
-    }
-    if ((int)H->seg_begin.size() != nseg) return SMAPB_JPEG_CORRUPT;
-    if (H->seg_end.back() - H->seg_begin.front() > MAX_SCAN_BYTES) return SMAPB_JPEG_TOO_LARGE;
-    H->out_h = H->orientation >= 5 ? H->w : H->h;
-    H->out_w = H->orientation >= 5 ? H->h : H->w;
-    return SMAPB_JPEG_OK;
-}
-
-// ---- host parser of multi-scan files (SMAPB_JPEG_SCANS) ---------------------------------------------------------------
 constexpr int MAX_SCANS = 64;
 
 struct ScanSpec {
@@ -350,18 +182,28 @@ struct ScanSpec {
     int ss = 0, se = 63, ah = 0, al = 0, dri = 0;
     int mcux = 0, nmcu = 0, bpm = 0;     // the scan's MCU grid: the frame's when interleaved, the component's block grid if not
     HuffSpec dc[3], ac[3];               // the tables in force at this SOS (optimised progressive files redefine them per scan)
-    std::vector<int64_t> seg_begin, seg_end, seg_stuffed;
+    std::vector<int64_t> seg_begin, seg_end;  // raw byte ranges of the restart segments
+    std::vector<int64_t> seg_stuffed;         // FF00 pairs inside each segment
 };
 
 struct ScanHeader {
-    Header f;  // frame geometry, latched quantisers, orientation (f.dc / f.ac / f.seg_* are unused)
+    Header f;  // frame geometry, latched quantisers, orientation
     std::vector<ScanSpec> scans;
 };
 
-// Walks every scan up to EOI.  Accepts baseline files, sequential files with several scans (every component in exactly
-// one scan) and progressive Huffman files (SOF2) whose progression libjpeg accepts without a warning and whose output
-// libjpeg-turbo does not smooth; everything else gets a status and goes to cv2.
-int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
+bool huff_ok(const HuffSpec& s) {
+    DevHuff d;
+    return build_huff(s, &d);
+}
+
+// Walks the markers up to EOI.  Without SMAPB_JPEG_SCANS it accepts one interleaved sequential scan (SOF0/SOF1) of every
+// component in frame order, followed by EOI.  With it, it also accepts sequential files with several scans (every
+// component in exactly one scan) and progressive Huffman files (SOF2) whose progression libjpeg accepts without a warning
+// and whose output libjpeg-turbo does not smooth.  Everything else gets a status and goes to cv2.  The two modes report
+// some defects at different points (the `!multi` checks), so a file with two defects keeps the status each mode always
+// gave it.
+int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
+    const bool multi = flags & SMAPB_JPEG_SCANS;
     Header* H = &M->f;
     if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return SMAPB_JPEG_MALFORMED;
     int64_t p = 2;
@@ -373,6 +215,14 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
     int coef_bits[3][64];  // libjpeg's progression record: -1 = never coded, else the Al of the last scan that coded it
     int nscanned[3] = {0, 0, 0};
     memset(coef_bits, 0xFF, sizeof(coef_bits));
+    // libjpeg's colour-space rule for 3 components: a JFIF APP0 means YCbCr; else an Adobe APP14 means RGB when its
+    // transform flag is 0 and YCbCr otherwise; else component ids 'R','G','B' mean RGB, anything else YCbCr
+    auto ycc = [&]() {
+        if (H->ncomp != 3 || jfif) return true;
+        if (adobe) return adobe_transform != 0;
+        return !(ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B');
+    };
+    auto too_large = [&]() { return (int64_t)H->h * H->w > SMAPB_JPEG_MAX_PIXELS; };
     for (;;) {
         if (p + 2 > n || d[p] != 0xFF) return SMAPB_JPEG_MALFORMED;
         while (p + 1 < n && d[p + 1] == 0xFF) p++;
@@ -418,7 +268,7 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
         } else if (m == 0xDD) {
             if (L != 2) return SMAPB_JPEG_MALFORMED;
             H->dri = u16(s);
-        } else if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
+        } else if (m == 0xC0 || m == 0xC1 || (m == 0xC2 && multi)) {
             if (sof || L < 6) return SMAPB_JPEG_MALFORMED;
             sof = true;
             progressive = m == 0xC2;
@@ -437,19 +287,19 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
                     if (ids[e] == ids[c]) return SMAPB_JPEG_MALFORMED;
             }
             if (nf == 1) {
-                H->comp_h[0] = H->comp_v[0] = 1;
+                H->comp_h[0] = H->comp_v[0] = 1;  // one component: one block per MCU whatever its factors say
             } else {
                 const bool ok = (H->comp_h[0] == 1 || H->comp_h[0] == 2) && (H->comp_v[0] == 1 || H->comp_v[0] == 2) &&
                                 H->comp_h[1] == 1 && H->comp_v[1] == 1 && H->comp_h[2] == 1 && H->comp_v[2] == 1;
                 if (!ok) return SMAPB_JPEG_UNSUPPORTED;
             }
-            if ((int64_t)H->h * H->w > SMAPB_JPEG_MAX_PIXELS) return SMAPB_JPEG_TOO_LARGE;
+            if (multi && too_large()) return SMAPB_JPEG_TOO_LARGE;  // without SMAPB_JPEG_SCANS: at the SOS
             H->hmax = H->comp_h[0], H->vmax = H->comp_v[0];
             H->mcux = (H->w + 8 * H->hmax - 1) / (8 * H->hmax);
             H->mcuy = (H->h + 8 * H->vmax - 1) / (8 * H->vmax);
             H->nmcu = H->mcux * H->mcuy;
-        } else if (m >= 0xC3 && m <= 0xCF) {
-            return SMAPB_JPEG_UNSUPPORTED;  // lossless, arithmetic, hierarchical, DAC, JPG
+        } else if (m >= 0xC2 && m <= 0xCF) {
+            return SMAPB_JPEG_UNSUPPORTED;  // progressive (without SMAPB_JPEG_SCANS), lossless, arithmetic, hierarchical, DAC, JPG
         } else if (m == 0xE0 || m == 0xE1 || m == 0xEE) {
             if (after_scan) return SMAPB_JPEG_UNSUPPORTED;  // colour-space and orientation markers belong before the first scan
             if (m == 0xE0) {
@@ -471,41 +321,51 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
             if ((int)M->scans.size() == MAX_SCANS) return SMAPB_JPEG_UNSUPPORTED;
             const int nf = H->ncomp;
             const int ns = L >= 1 ? s[0] : 0;
+            if (!multi && (ns != nf || L != 4 + 2 * nf)) return SMAPB_JPEG_UNSUPPORTED;
             if (ns < 1 || ns > nf || L != 4 + 2 * ns) return SMAPB_JPEG_MALFORMED;
             M->scans.emplace_back();
             ScanSpec& S = M->scans.back();
             S.ncomp = ns;
             S.ss = s[1 + 2 * ns], S.se = s[2 + 2 * ns], S.ah = s[3 + 2 * ns] >> 4, S.al = s[3 + 2 * ns] & 15;
             S.dri = H->dri;
-            for (int k = 0; k < ns; k++) {
-                int c = 0;
-                while (c < nf && ids[c] != s[1 + 2 * k]) c++;
-                if (c == nf || (k > 0 && c <= S.comp[k - 1])) return SMAPB_JPEG_UNSUPPORTED;  // unknown id, or not in frame order
-                S.comp[k] = c;
-            }
-            if (!progressive) {
-                if (S.ss != 0 || S.se != 63 || S.ah != 0 || S.al != 0) return SMAPB_JPEG_UNSUPPORTED;
-                for (int k = 0; k < ns; k++)
-                    if (nscanned[S.comp[k]]++) return SMAPB_JPEG_UNSUPPORTED;
-            } else {
-                // libjpeg's checks (start_pass_phuff_decoder): the first group is fatal there, the second a warning
-                // ("bogus progression"); both are left to cv2
-                const bool dc_band = S.ss == 0;
-                if (dc_band ? S.se != 0 : (S.ss > S.se || S.se > 63 || ns != 1)) return SMAPB_JPEG_UNSUPPORTED;
-                if ((S.ah != 0 && S.al != S.ah - 1) || S.al > 13) return SMAPB_JPEG_UNSUPPORTED;
+            if (multi) {
                 for (int k = 0; k < ns; k++) {
-                    int* cb = coef_bits[S.comp[k]];
-                    if (!dc_band && cb[0] < 0) return SMAPB_JPEG_UNSUPPORTED;
-                    for (int i = S.ss; i <= S.se; i++) {
-                        if (S.ah != (cb[i] < 0 ? 0 : cb[i])) return SMAPB_JPEG_UNSUPPORTED;
-                        cb[i] = S.al;
+                    int c = 0;
+                    while (c < nf && ids[c] != s[1 + 2 * k]) c++;
+                    if (c == nf || (k > 0 && c <= S.comp[k - 1])) return SMAPB_JPEG_UNSUPPORTED;  // unknown id, or not in frame order
+                    S.comp[k] = c;
+                }
+                if (!progressive) {
+                    if (S.ss != 0 || S.se != 63 || S.ah != 0 || S.al != 0) return SMAPB_JPEG_UNSUPPORTED;
+                    for (int k = 0; k < ns; k++)
+                        if (nscanned[S.comp[k]]++) return SMAPB_JPEG_UNSUPPORTED;
+                } else {
+                    // libjpeg's checks (start_pass_phuff_decoder): the first group is fatal there, the second a warning
+                    // ("bogus progression"); both are left to cv2
+                    const bool dc_band = S.ss == 0;
+                    if (dc_band ? S.se != 0 : (S.ss > S.se || S.se > 63 || ns != 1)) return SMAPB_JPEG_UNSUPPORTED;
+                    if ((S.ah != 0 && S.al != S.ah - 1) || S.al > 13) return SMAPB_JPEG_UNSUPPORTED;
+                    for (int k = 0; k < ns; k++) {
+                        int* cb = coef_bits[S.comp[k]];
+                        if (!dc_band && cb[0] < 0) return SMAPB_JPEG_UNSUPPORTED;
+                        for (int i = S.ss; i <= S.se; i++) {
+                            if (S.ah != (cb[i] < 0 ? 0 : cb[i])) return SMAPB_JPEG_UNSUPPORTED;
+                            cb[i] = S.al;
+                        }
                     }
                 }
             }
-            const bool dc_first = S.ss == 0 && S.ah == 0, uses_ac = S.se > 0;
+            // without SMAPB_JPEG_SCANS each component is checked in turn (id, tables, quantiser), both tables whatever
+            // the band, and the band after them
+            const bool dc_first = !multi || (S.ss == 0 && S.ah == 0), uses_ac = !multi || S.se > 0;
             for (int k = 0; k < ns; k++) {
+                if (!multi) {
+                    if (s[1 + 2 * k] != ids[k]) return SMAPB_JPEG_UNSUPPORTED;
+                    S.comp[k] = k;
+                }
                 const int c = S.comp[k];
                 const int td = s[2 + 2 * k] >> 4, ta = s[2 + 2 * k] & 15;
+                if (!multi && (ta > 3 || !H->dht[1][ta].defined || !qt[tq[c]])) return SMAPB_JPEG_UNSUPPORTED;
                 if (dc_first) {
                     if (td > 3 || !H->dht[0][td].defined) return SMAPB_JPEG_UNSUPPORTED;
                     for (int i = 0; i < H->dht[0][td].nvals; i++)
@@ -516,8 +376,7 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
                     if (ta > 3 || !H->dht[1][ta].defined) return SMAPB_JPEG_UNSUPPORTED;
                     S.ac[k] = H->dht[1][ta];
                 }
-                DevHuff tmp;
-                if ((dc_first && !build_huff(S.dc[k], &tmp)) || (uses_ac && !build_huff(S.ac[k], &tmp))) return SMAPB_JPEG_MALFORMED;
+                if (multi && ((dc_first && !huff_ok(S.dc[k])) || (uses_ac && !huff_ok(S.ac[k])))) return SMAPB_JPEG_MALFORMED;
                 if (!latched[c]) {  // libjpeg latches a component's quantiser at its first scan
                     if (!qt[tq[c]]) return SMAPB_JPEG_UNSUPPORTED;
                     for (int i = 0; i < 64; i++) {
@@ -528,6 +387,11 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
                     latched[c] = true;
                     qt_used[tq[c]] = true;
                 }
+            }
+            if (!multi) {
+                if (S.ss != 0 || S.se != 63 || S.ah != 0 || S.al != 0) return SMAPB_JPEG_UNSUPPORTED;
+                if (!ycc()) return SMAPB_JPEG_UNSUPPORTED;
+                if (too_large()) return SMAPB_JPEG_TOO_LARGE;
             }
             if (ns == 1) {  // non-interleaved: the component's own block grid
                 const int c = S.comp[0];
@@ -542,7 +406,8 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
                 for (int k = 0; k < ns; k++) S.bpm += H->comp_h[S.comp[k]] * H->comp_v[S.comp[k]];
             }
             const int nseg = S.dri ? (S.nmcu + S.dri - 1) / S.dri : 1;
-            // entropy-coded data up to the next marker that is not a restart marker
+            // entropy-coded data: FF00 = stuffed FF, FFD0..D7 = restart marker in sequence; any other marker ends the scan,
+            // and without SMAPB_JPEG_SCANS it must be EOI
             int64_t start = p, q = p, stuffed = 0;
             for (;;) {
                 const uint8_t* f = (const uint8_t*)memchr(d + q, 0xFF, (size_t)(n - q));
@@ -557,6 +422,7 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
                 const bool rst = mk >= 0xD0 && mk <= 0xD7;
                 if (rst && (!S.dri || mk - 0xD0 != (int)(S.seg_begin.size() % 8) || (int)S.seg_begin.size() + 1 >= nseg))
                     return SMAPB_JPEG_CORRUPT;
+                if (!rst && !multi && mk != 0xD9) return SMAPB_JPEG_UNSUPPORTED;
                 S.seg_begin.push_back(start);
                 S.seg_end.push_back(q);
                 S.seg_stuffed.push_back(stuffed);
@@ -571,24 +437,24 @@ int jpeg_parse_scans(const uint8_t* d, int64_t n, ScanHeader* M) {
             return SMAPB_JPEG_UNSUPPORTED;
         }
     }
-    const int nf = H->ncomp;
-    for (int c = 0; c < nf; c++) {
-        if (!progressive) {
-            if (nscanned[c] != 1) return SMAPB_JPEG_UNSUPPORTED;
-            continue;
+    if (multi) {
+        for (int c = 0; c < H->ncomp; c++) {
+            if (!progressive) {
+                if (nscanned[c] != 1) return SMAPB_JPEG_UNSUPPORTED;
+                continue;
+            }
+            // libjpeg-turbo smooths the output (block smoothing, smoothing_ok) when a component's DC was coded and one of
+            // its coefficients 1..9 is not fully refined; those files, and components without DC, are left to cv2
+            if (coef_bits[c][0] < 0) return SMAPB_JPEG_UNSUPPORTED;
+            for (int i = 1; i <= 9; i++)
+                if (coef_bits[c][i] != 0) return SMAPB_JPEG_UNSUPPORTED;
         }
-        // libjpeg-turbo smooths the output (block smoothing, smoothing_ok) when a component's DC was coded and one of its
-        // coefficients 1..9 is not fully refined; those files, and components without DC, are left to cv2
-        if (coef_bits[c][0] < 0) return SMAPB_JPEG_UNSUPPORTED;
-        for (int i = 1; i <= 9; i++)
-            if (coef_bits[c][i] != 0) return SMAPB_JPEG_UNSUPPORTED;
-    }
-    if (nf == 3) {
-        bool ycc;
-        if (jfif) ycc = true;
-        else if (adobe) ycc = adobe_transform != 0;
-        else ycc = !(ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B');
-        if (!ycc) return SMAPB_JPEG_UNSUPPORTED;
+        if (!ycc()) return SMAPB_JPEG_UNSUPPORTED;
+    } else {
+        // the one scan covers every component and its colour space was checked at its SOS; its tables are checked last
+        const ScanSpec& S = M->scans[0];
+        for (int k = 0; k < S.ncomp; k++)
+            if (!huff_ok(S.dc[k]) || !huff_ok(S.ac[k])) return SMAPB_JPEG_MALFORMED;
     }
     H->out_h = H->orientation >= 5 ? H->w : H->h;
     H->out_w = H->orientation >= 5 ? H->h : H->w;
@@ -602,91 +468,26 @@ __device__ __forceinline__ uint32_t peek32(const uint32_t* words, uint32_t pos) 
     return __funnelshift_l(lo, hi, sh);
 }
 
-// Decodes from (pos, blk, zz) while pos < stop.  Every unit (a Huffman code and its extra bits) must end within seg_end.
-// Errors (a code not in the table, a run past coefficient 63, a unit past the segment's end) are recorded - `err` = blocks
-// completed before the first one, or -1 - and decoding goes on by a fixed rule (skip one bit; end the block; stop), so a
-// speculative decoder that started from a wrong state keeps going until it falls into step with the true decoder.
-// WRITE: coefficients go to coef (block `blk0` = the first block this run completes, counted within the segment); blocks at
-// or beyond `limit` are not written.
-struct RunResult {
-    uint32_t pos;
-    int blk, zz, nblk, err;
-};
-
-template <bool WRITE>
-__device__ RunResult huff_run(const DevImage& I, const uint32_t* __restrict__ words, uint32_t pos, int blk, int zz, uint32_t stop,
-                              uint32_t seg_end, int16_t* __restrict__ coef, int blk0, int limit) {
-    int nblk = 0, err = -1;
-    while (pos < stop) {
-        const int c = I.blk_comp[blk];
-        const DevHuff& T = zz == 0 ? I.dc[c] : I.ac[c];
-        const uint32_t bits = peek32(words, pos);
-        int len = 0, sym = 0;
-        const uint32_t f = T.fast[bits >> 23];
-        if (f) {
-            len = f >> 8, sym = f & 255;
-        } else {
-            for (int l = 10; l <= 16; l++) {
-                const int code = (int)(bits >> (32 - l));
-                if (code <= T.maxcode[l]) {
-                    len = l;
-                    sym = T.vals[(T.valoff[l] + code) & 255];
-                    break;
-                }
-            }
-            if (!len) {
-                if (err < 0) err = nblk;
-                pos++;
-                continue;
-            }
-        }
-        const int s = sym & 15;
-        if ((uint64_t)pos + len + s > seg_end) {
-            if (err < 0) err = nblk;
-            pos = seg_end;
-            break;
-        }
-        int v = 0;
-        if (s) {
-            v = (int)((bits << len) >> (32 - s));
-            if (v < (1 << (s - 1))) v += 1 - (1 << s);
-        }
-        int16_t* b = WRITE && blk0 + nblk < limit ? coef + (int64_t)(blk0 + nblk) * 64 : nullptr;
-        if (zz == 0) {
-            if (b) b[0] = (int16_t)v;
-            zz = 1;
-        } else if (s == 0) {
-            if ((sym >> 4) == 15) {
-                zz += 16;
-                if (zz > 64) {
-                    if (err < 0) err = nblk;
-                    zz = 64;
-                }
-            } else {
-                zz = 64;
-            }
-        } else {
-            zz += sym >> 4;
-            if (zz > 63) {
-                if (err < 0) err = nblk;
-                zz = 64;
-            } else {
-                if (b) b[c_zigzag[zz]] = (int16_t)v;
-                zz++;
-            }
-        }
-        pos += len + s;
-        if (zz == 64) {
-            zz = 0;
-            nblk++;
-            if (++blk == I.bpm) blk = 0;
+// The Huffman code at the top of `bits`: its length (0 = no code of the table) and *sym.  Codes of up to 9 bits come from
+// the fast table, longer ones from maxcode.
+__device__ __forceinline__ int huff_lookup(const DevHuff& T, uint32_t bits, int* sym) {
+    const uint32_t f = T.fast[bits >> 23];
+    if (f) {
+        *sym = f & 255;
+        return f >> 8;
+    }
+    for (int l = 10; l <= 16; l++) {
+        const int code = (int)(bits >> (32 - l));
+        if (code <= T.maxcode[l]) {
+            *sym = T.vals[(T.valoff[l] + code) & 255];
+            return l;
         }
     }
-    return {pos, blk, zz, nblk, err};
+    return 0;
 }
 
 // ---- a. unstuffing ---------------------------------------------------------------------------------------------------
-// One CTA per image walks its scan bytes: a byte is dropped when it follows an FF (the 00 of a stuffed FF, the code byte of
+// One CTA per scan walks its bytes: a byte is dropped when it follows an FF (the 00 of a stuffed FF, the code byte of
 // a restart marker) or when it is an FF that starts a restart marker.  Block-wide prefix sums give the output positions.
 __device__ int block_exclusive_scan(int v, int* total) {
     __shared__ int warp_sums[32];
@@ -718,10 +519,9 @@ __device__ int block_exclusive_scan(int v, int* total) {
 
 constexpr int UNSTUFF_PER_THREAD = 16;
 
-template <class Desc>  // DevImage (one scan per image) or DevScan (one CTA per scan)
-__global__ void __launch_bounds__(1024) unstuff_kernel(const Desc* __restrict__ imgs, const uint8_t* __restrict__ raw,
+__global__ void __launch_bounds__(1024) unstuff_kernel(const DevScan* __restrict__ scans, const uint8_t* __restrict__ raw,
                                                        uint8_t* __restrict__ unst) {
-    const Desc& I = imgs[blockIdx.x];
+    const DevScan& I = scans[blockIdx.x];
     const uint8_t* src = raw + I.raw_off;
     uint8_t* dst = unst + I.unst_off;
     const int64_t n = I.raw_len;
@@ -755,20 +555,176 @@ __global__ void __launch_bounds__(1024) unstuff_kernel(const Desc* __restrict__ 
     for (int k = threadIdx.x; k < 16; k += blockDim.x) dst[out + k] = 0;
 }
 
-// ---- b. Huffman decoding ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) huff_sync_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
-                                                        const DevSub* __restrict__ subs, int nsub, const uint8_t* __restrict__ unst,
-                                                        const SubState* __restrict__ prev, SubState* __restrict__ cur,
-                                                        int* __restrict__ changed, int pass) {
+// ---- b. Huffman scans and refinement ---------------------------------------------------------------------------------
+// Block counts saturate at BLOCK_SAT.  An EOB run adds up to 32767 blocks for 15 bits, so plain
+// sums over a scan could pass 2^31; every segment holds far fewer than BLOCK_SAT blocks, so a saturated count is already
+// past the segment's end (nothing is written there) and sums of two saturated counts still fit an int.
+constexpr int BLOCK_SAT = 1 << 29;
+
+__device__ __forceinline__ int sat_add(int a, int b) { return min(a + b, BLOCK_SAT); }
+
+struct SatAdd {
+    __device__ int operator()(int a, int b) const { return sat_add(a, b); }
+};
+struct IntAdd {
+    __device__ int operator()(int a, int b) const { return a + b; }
+};
+
+// Block-wide segmented inclusive scan of (head, v), one value per thread in thread order, continued from *carry (the value
+// the tiles before this one end with, updated for the next): (h1, v1) + (h2, v2) = (h1 | h2, h2 ? v2 : Add(v1, v2)).
+// Every thread of the CTA calls it.
+template <class Add>
+__device__ int block_segmented_scan(int v, int head, int* carry) {
+    __shared__ int s_head[32], s_val[32];
+    const Add add;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int x = v, hx = head;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o), hy = __shfl_up_sync(0xffffffffu, hx, o);
+        if (lane >= o) {
+            if (!hx) x = add(x, y);
+            hx |= hy;
+        }
+    }
+    if (lane == 31) s_head[wid] = hx, s_val[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        int wx = lane < nw ? s_val[lane] : 0, wh = lane < nw ? s_head[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, wx, o), hy = __shfl_up_sync(0xffffffffu, wh, o);
+            if (lane >= o) {
+                if (!wh) wx = add(wx, y);
+                wh |= hy;
+            }
+        }
+        s_val[lane] = wx, s_head[lane] = wh;
+    }
+    __syncthreads();
+    // prefix from earlier warps of this tile, then the carry of earlier tiles
+    if (!hx) {
+        if (wid > 0) x = add(x, s_val[wid - 1]);
+        if (wid == 0 || !s_head[wid - 1]) x = add(x, *carry);
+    }
+    const int tile_val = s_val[nw - 1], tile_head = s_head[nw - 1];
+    __syncthreads();
+    *carry = tile_head ? tile_val : add(*carry, tile_val);
+    return x;
+}
+
+// The coefficient buffer keeps the single-scan layout (frame MCU by frame MCU, the IDCT reads it as it is); a scan's block
+// b (in its own decode order) lands here.
+__device__ __forceinline__ int64_t scan_block(const DevScan& S, const DevImage& I, int b) {
+    const int m = b / S.bpm, j = b - m * S.bpm;
+    if (S.inter) return (int64_t)m * I.bpm + S.blk_map[j];
+    const int bx = m % S.mcux, by = m / S.mcux;
+    return ((int64_t)(by / S.v) * I.mcux + bx / S.h) * I.bpm + S.j0 + (by % S.v) * S.h + bx % S.h;
+}
+
+// Decodes coefficients Ss..Se of each block of one scan from (pos, blk, zz) while pos < stop: DC first / sequential values
+// as differences (scan_dc_kernel adds them up), AC values stored << Al.  In progressive AC scans (Ss > 0) an EOBn symbol
+// ends a run of 2^n + (n extra bits) blocks; those blocks hold no bits, so the run is counted when its symbol is read and
+// the decoder state stays (bit position, block within the MCU, zig-zag index).  Every unit (a Huffman code and its extra
+// bits) must end within seg_end.  Errors (a code not in the table, a run past Se, a unit past the segment's end) are
+// recorded - `err` = blocks completed before the first one, or -1 - and decoding goes on by a fixed rule (skip one bit; end
+// the block; stop), so a speculative decoder that started from a wrong state keeps going until it falls into step with the
+// true decoder.  WRITE: coefficients go to the scan's block blk0 + (blocks completed so far); blocks at or beyond `limit`
+// are not written.
+struct RunResult {
+    uint32_t pos;
+    int blk, zz, nblk, err;
+};
+
+template <bool WRITE>
+__device__ RunResult scan_run(const DevScan& S, const DevImage& I, const DevHuff* __restrict__ huffs,
+                              const uint32_t* __restrict__ words, uint32_t pos, int blk, int zz, uint32_t stop, uint32_t seg_end,
+                              int16_t* __restrict__ coef, int blk0, int limit) {
+    int nblk = 0, err = -1;
+    const bool eob_runs = S.ss > 0;
+    int16_t* b = nullptr;
+    int b_at = -1;
+    while (pos < stop) {
+        const DevHuff& T = huffs[zz == 0 ? S.blk_dc[blk] : S.blk_ac[blk]];
+        const uint32_t bits = peek32(words, pos);
+        int sym = 0;
+        const int len = huff_lookup(T, bits, &sym);
+        if (!len) {
+            if (err < 0) err = nblk;
+            pos++;
+            continue;
+        }
+        const int s = sym & 15, r = sym >> 4;
+        const bool eob_n = eob_runs && s == 0 && r < 15;
+        const int extra = eob_n ? r : s;
+        if ((uint64_t)pos + len + extra > seg_end) {
+            if (err < 0) err = nblk;
+            pos = seg_end;
+            break;
+        }
+        int v = 0;
+        if (extra) {
+            v = (int)((bits << len) >> (32 - extra));
+            if (!eob_n && v < (1 << (s - 1))) v += 1 - (1 << s);
+        }
+        if (WRITE && b_at != nblk) {
+            b_at = nblk;
+            b = blk0 + nblk < limit ? coef + scan_block(S, I, blk0 + nblk) * 64 : nullptr;
+        }
+        int done = 0;  // blocks this unit completes
+        if (zz == 0) {
+            if (WRITE && b) b[0] = (int16_t)v;
+            zz = 1;
+            if (S.se == 0) done = 1;
+        } else if (s == 0) {
+            if (r == 15) {
+                zz += 16;
+                if (zz > S.se + 1) {
+                    if (err < 0) err = nblk;
+                    done = 1;
+                } else if (zz == S.se + 1) {
+                    done = 1;
+                }
+            } else {
+                done = eob_n ? (1 << r) + v : 1;
+            }
+        } else {
+            zz += r;
+            if (zz > S.se) {
+                if (err < 0) err = nblk;
+                done = 1;
+            } else {
+                if (WRITE && b) b[c_zigzag[zz]] = (int16_t)((unsigned)v << S.al);
+                if (++zz > S.se) done = 1;
+            }
+        }
+        pos += len + extra;
+        if (done) {
+            zz = S.ss;
+            nblk = min(nblk + done, BLOCK_SAT);
+            if (++blk == S.bpm) blk = 0;
+        }
+    }
+    return {pos, blk, zz, nblk, err};
+}
+
+// Sync passes over the subsequences [sub_lo, sub_lo + nsub) of one round.
+__global__ void __launch_bounds__(256) scan_sync_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                        const DevHuff* __restrict__ huffs, const DevSeg* __restrict__ segs,
+                                                        const DevSub* __restrict__ subs, int sub_lo, int nsub,
+                                                        const uint8_t* __restrict__ unst, const SubState* __restrict__ prev,
+                                                        SubState* __restrict__ cur, int* __restrict__ changed, int pass) {
     if (pass >= 2 && changed[pass - 1] == 0) return;  // converged: the buffer of the first quiet pass is final
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nsub) return;
-    const DevSub S = subs[i];
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nsub) return;
+    const int i = sub_lo + t;
+    const DevSub U = subs[i];
+    const DevScan& S = scans[U.scan];
     const DevImage& I = imgs[S.img];
-    const DevSeg& G = segs[S.seg];
+    const DevSeg& G = segs[U.seg];
     unsigned long long start;
     if (pass == 0) {
-        start = pack_state(S.bit_begin, 0, 0);  // a guess, except for the first subsequence of a segment
+        start = pack_state(U.bit_begin, 0, S.ss);  // a guess, except for the first subsequence of a segment
     } else {
         if (G.sub0 == i) {
             cur[i] = prev[i];
@@ -780,18 +736,18 @@ __global__ void __launch_bounds__(256) huff_sync_kernel(const DevImage* __restri
             return;
         }
     }
-    const uint32_t* words = (const uint32_t*)(unst + I.unst_off);
+    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
     if (pass == 0 && G.sub0 != i) {
         // warm-up: decode up to WARM_BITS before the subsequence from the guess, so that the state at its first unit
         // boundary has had that long to fall into step with the true decoder
-        const uint32_t from = S.bit_begin - min(S.bit_begin - G.bit_begin, (uint32_t)WARM_BITS);
-        const RunResult W = huff_run<false>(I, words, from, 0, 0, S.bit_begin, G.bit_end, nullptr, 0, 0);
+        const uint32_t from = U.bit_begin - min(U.bit_begin - G.bit_begin, (uint32_t)WARM_BITS);
+        const RunResult W = scan_run<false>(S, I, huffs, words, from, 0, S.ss, U.bit_begin, G.bit_end, nullptr, 0, 0);
         start = pack_state(W.pos, W.blk, W.zz);
     }
     SubState r;
     r.start = start;
-    const RunResult R = huff_run<false>(I, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255,
-                                        S.bit_end, G.bit_end, nullptr, 0, 0);
+    const RunResult R = scan_run<false>(S, I, huffs, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255,
+                                        U.bit_end, G.bit_end, nullptr, 0, 0);
     r.exit = pack_state(R.pos, R.blk, R.zz);
     r.nblk = R.nblk;
     r.errblk = R.err >= 0 ? R.err : 0x7fffffff;
@@ -799,126 +755,201 @@ __global__ void __launch_bounds__(256) huff_sync_kernel(const DevImage* __restri
     changed[pass] = 1;  // benign race: every writer stores 1
 }
 
-// One CTA per image: exclusive prefix sum of the blocks completed per subsequence (within its segment), and the checks
-// that make an image fall back: an error before the segment's last block, or fewer blocks than the segment's MCUs hold.
-__global__ void __launch_bounds__(1024) huff_prefix_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
+// One CTA per scan of list[]: base[i] = blocks completed in subsequence i's restart segment up to and including i (a
+// segmented, saturating inclusive scan), and the checks that make an image fall back: an error before the segment's last
+// block, or fewer blocks than the segment's MCUs hold.
+__global__ void __launch_bounds__(1024) scan_prefix_kernel(const DevScan* __restrict__ scans, const int* __restrict__ list,
+                                                           const DevSeg* __restrict__ segs, const DevSub* __restrict__ subs,
                                                            const SubState* __restrict__ st, int* __restrict__ base,
                                                            int* __restrict__ status) {
-    const DevImage& I = imgs[blockIdx.x];
+    const DevScan& S = scans[list[blockIdx.x]];
     int carry = 0;
-    for (int j0 = 0; j0 < I.nsub; j0 += blockDim.x) {
+    for (int j0 = 0; j0 < S.nsub; j0 += blockDim.x) {
         const int j = j0 + threadIdx.x;
-        const int v = j < I.nsub ? st[I.sub0 + j].nblk : 0;
-        int total;
-        const int at = block_exclusive_scan(v, &total);
-        if (j < I.nsub) base[I.sub0 + j] = carry + at;  // image-wide for now
-        carry += total;
+        int v = 0, head = 0;
+        if (j < S.nsub) {
+            const int i = S.sub0 + j;
+            v = st[i].nblk;
+            head = segs[subs[i].seg].sub0 == i;
+        }
+        const int x = block_segmented_scan<SatAdd>(v, head, &carry);
+        if (j < S.nsub) base[S.sub0 + j] = x;
     }
     __syncthreads();
     bool bad = false;
-    for (int j = threadIdx.x; j < I.nsub; j += blockDim.x) {
-        const int i = I.sub0 + j;
+    for (int j = threadIdx.x; j < S.nsub; j += blockDim.x) {
+        const int i = S.sub0 + j;
         const SubState s = st[i];
-        if (s.errblk != 0x7fffffff) {
-            int lo = I.seg0, hi = I.seg0 + I.nseg - 1;
-            while (lo < hi) {
-                const int mid = (lo + hi + 1) >> 1;
-                if (segs[mid].sub0 <= i) lo = mid;
-                else hi = mid - 1;
-            }
-            const int e = base[i] - base[segs[lo].sub0] + s.errblk;  // segs[lo] holds subsequence i
-            if (e < segs[lo].nmcu * I.bpm) bad = true;
-        }
+        const DevSeg& G = segs[subs[i].seg];
+        if (s.errblk != 0x7fffffff && sat_add(G.sub0 == i ? 0 : base[i - 1], s.errblk) < G.nmcu * S.bpm) bad = true;
+        if (i == G.sub0 + G.nsub - 1 && base[i] < G.nmcu * S.bpm) bad = true;  // the segment ends short of its blocks
     }
-    for (int k = I.seg0 + threadIdx.x; k < I.seg0 + I.nseg; k += blockDim.x) {
-        const DevSeg& G = segs[k];
-        const int last = G.sub0 + G.nsub - 1;
-        if (base[last] + st[last].nblk - base[G.sub0] < G.nmcu * I.bpm) bad = true;
-    }
-    if (bad) status[blockIdx.x] = SMAPB_JPEG_CORRUPT;
+    if (bad) status[S.img] = SMAPB_JPEG_CORRUPT;
 }
 
-__global__ void __launch_bounds__(256) huff_write_kernel(const DevImage* __restrict__ imgs, const DevSeg* __restrict__ segs,
-                                                         const DevSub* __restrict__ subs, int nsub, const uint8_t* __restrict__ unst,
-                                                         const SubState* __restrict__ st, const int* __restrict__ base,
-                                                         const int* __restrict__ status, int16_t* __restrict__ coef) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nsub) return;
-    const DevSub S = subs[i];
+__global__ void __launch_bounds__(256) scan_write_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                         const DevHuff* __restrict__ huffs, const DevSeg* __restrict__ segs,
+                                                         const DevSub* __restrict__ subs, int sub_lo, int nsub,
+                                                         const uint8_t* __restrict__ unst, const SubState* __restrict__ st,
+                                                         const int* __restrict__ base, const int* __restrict__ status,
+                                                         int16_t* __restrict__ coef) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nsub) return;
+    const int i = sub_lo + t;
+    const DevSub U = subs[i];
+    const DevScan& S = scans[U.scan];
     if (status[S.img] != SMAPB_JPEG_OK) return;
     const DevImage& I = imgs[S.img];
-    const DevSeg& G = segs[S.seg];
+    const DevSeg& G = segs[U.seg];
     const unsigned long long start = st[i].start;
-    const int first = G.first_mcu * I.bpm;  // block index of the segment's first block within the image
-    const int local = base[i] - base[G.sub0];
-    const uint32_t* words = (const uint32_t*)(unst + I.unst_off);
-    huff_run<true>(I, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255, S.bit_end, G.bit_end,
-                   coef + (I.coef_off + (int64_t)first) * 64, local, G.nmcu * I.bpm);
+    const int first = G.first_mcu * S.bpm;
+    const int local = G.sub0 == i ? 0 : base[i - 1];  // blocks of the segment completed before this subsequence
+    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
+    scan_run<true>(S, I, huffs, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255, U.bit_end, G.bit_end,
+                   coef + I.coef_off * 64, first + local, first + G.nmcu * S.bpm);
 }
 
-// DC prediction: one CTA per (image, component), a segmented scan over that component's blocks in decode order, reset at
-// every restart segment.  The sum runs in int (libjpeg's predictor), the block keeps its low 16 bits.
-__global__ void __launch_bounds__(1024) dc_scan_kernel(const DevImage* __restrict__ imgs, const int* __restrict__ status,
+// DC prediction of a sequential or DC-first scan: one CTA per (scan, scan component), a segmented scan over that
+// component's blocks in decode order, reset at every restart.  The sum runs in int (libjpeg's predictor), the block keeps
+// the low 16 bits of (sum << Al).
+__global__ void __launch_bounds__(1024) scan_dc_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                       const int* __restrict__ list, const int* __restrict__ status,
                                                        int16_t* __restrict__ coef) {
-    const DevImage& I = imgs[blockIdx.x];
-    const int c = blockIdx.y;
-    if (c >= I.ncomp || status[blockIdx.x] != SMAPB_JPEG_OK) return;
-    int j0 = 0;
-    for (int j = 0; j < I.bpm; j++)
-        if (I.blk_comp[j] < c) j0++;
-    const int nc = (c == 0) ? I.bpm - (I.ncomp - 1) : 1;
-    const int total = I.nmcu * nc;
+    const DevScan& S = scans[list[blockIdx.x]];
+    const DevImage& I = imgs[S.img];
+    const int k = blockIdx.y;
+    if (k >= S.ncomp || status[S.img] != SMAPB_JPEG_OK) return;
+    int j0 = 0, nc = 0;
+    for (int j = 0; j < S.bpm; j++) {
+        if (S.blk_comp[j] < k) j0++;
+        if (S.blk_comp[j] == k) nc++;
+    }
+    const int total = S.nmcu * nc;
     int16_t* cf = coef + I.coef_off * 64;
-    __shared__ int s_head[32], s_val[32];
     int carry = 0;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
     for (int t0 = 0; t0 < total; t0 += blockDim.x) {
         const int t = t0 + threadIdx.x;
         int v = 0, head = 0;
         int64_t at = 0;
         if (t < total) {
-            const int m = t / nc, k = t % nc;
-            at = ((int64_t)m * I.bpm + j0 + k) * 64;
+            const int m = t / nc, kk = t % nc;
+            at = scan_block(S, I, m * S.bpm + j0 + kk) * 64;
             v = cf[at];
-            head = (k == 0 && m % I.per == 0) ? 1 : 0;
+            head = (kk == 0 && m % S.per == 0) ? 1 : 0;
         }
-        // segmented inclusive scan of (head, v): (h1, v1) + (h2, v2) = (h1 | h2, h2 ? v2 : v1 + v2)
-        int x = v, hx = head;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, x, o), hy = __shfl_up_sync(0xffffffffu, hx, o);
-            if (lane >= o) {
-                if (!hx) x += y;
-                hx |= hy;
-            }
+        const int x = block_segmented_scan<IntAdd>(v, head, &carry);
+        if (t < total) cf[at] = (int16_t)((unsigned)x << S.al);
+    }
+}
+
+// DC refinement: one raw bit per block, the n-th bit of its restart segment for the segment's n-th block; sets bit Al.
+__global__ void __launch_bounds__(256) dc_refine_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                        const int* __restrict__ list, const DevSeg* __restrict__ segs,
+                                                        const uint8_t* __restrict__ unst, int* __restrict__ status,
+                                                        int16_t* __restrict__ coef) {
+    const DevScan& S = scans[list[blockIdx.y]];
+    const DevImage& I = imgs[S.img];
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= S.nmcu * S.bpm || status[S.img] != SMAPB_JPEG_OK) return;
+    const DevSeg& G = segs[S.seg0 + t / S.bpm / S.per];
+    const uint32_t pos = G.bit_begin + (uint32_t)(t - G.first_mcu * S.bpm);
+    if (pos >= G.bit_end) {
+        status[S.img] = SMAPB_JPEG_CORRUPT;
+        return;
+    }
+    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
+    if (peek32(words, pos) >> 31) {
+        int16_t* c = coef + (I.coef_off + scan_block(S, I, t)) * 64;
+        c[0] = (int16_t)(c[0] | (1 << S.al));
+    }
+}
+
+// AC refinement (libjpeg's decode_mcu_AC_refine): the bits a block takes depend on which of its coefficients are already
+// nonzero, so no speculative decoder can start mid-segment; one thread decodes one restart segment.  It reads and writes
+// only the current block's coefficients, at or after its zig-zag position.
+__global__ void __launch_bounds__(128) ac_refine_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                        const DevHuff* __restrict__ huffs, const int* __restrict__ list, int n,
+                                                        const DevSeg* __restrict__ segs, const uint8_t* __restrict__ unst,
+                                                        int* __restrict__ status, int16_t* __restrict__ coef) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const DevSeg& G = segs[list[t]];
+    const DevScan& S = scans[G.scan];
+    const DevImage& I = imgs[S.img];
+    if (status[S.img] != SMAPB_JPEG_OK) return;
+    const DevHuff& T = huffs[S.blk_ac[0]];
+    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
+    int16_t* cf = coef + I.coef_off * 64;
+    const int p1 = 1 << S.al, m1 = -(1 << S.al);
+    uint32_t pos = G.bit_begin;
+    const uint32_t end = G.bit_end;
+    bool bad = false;
+    int eobrun = 0;
+    auto bit = [&]() -> int {
+        if (pos >= end) {
+            bad = true;
+            return 0;
         }
-        if (lane == 31) s_head[wid] = hx, s_val[wid] = x;
-        __syncthreads();
-        if (wid == 0) {
-            int wx = lane < nw ? s_val[lane] : 0, wh = lane < nw ? s_head[lane] : 0;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, wx, o), hy = __shfl_up_sync(0xffffffffu, wh, o);
-                if (lane >= o) {
-                    if (!wh) wx += y;
-                    wh |= hy;
+        return (int)(peek32(words, pos++) >> 31);
+    };
+    for (int q = 0; q < G.nmcu && !bad; q++) {
+        int16_t* blk = cf + scan_block(S, I, G.first_mcu + q) * 64;
+        int k = S.ss;
+        if (eobrun == 0) {
+            for (; k <= S.se && !bad; k++) {
+                int sym = 0;
+                const int len = huff_lookup(T, peek32(words, pos), &sym);
+                if (!len || pos + len > end) {
+                    bad = true;
+                    break;
+                }
+                pos += len;
+                int r = sym >> 4, s = sym & 15, sv = 0;
+                if (s) {
+                    if (s != 1) {
+                        bad = true;
+                        break;
+                    }
+                    sv = bit() ? p1 : m1;
+                } else if (r != 15) {
+                    eobrun = 1 << r;
+                    if (r) {
+                        if (pos + r > end) {
+                            bad = true;
+                            break;
+                        }
+                        eobrun += (int)(peek32(words, pos) >> (32 - r));
+                        pos += r;
+                    }
+                    break;
+                }
+                do {
+                    int16_t* c = blk + c_zigzag[k];
+                    if (*c != 0) {
+                        if (bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
+                    } else if (--r < 0) {
+                        break;
+                    }
+                    k++;
+                } while (k <= S.se);
+                if (sv) {
+                    if (k > S.se) {
+                        bad = true;
+                        break;
+                    }
+                    blk[c_zigzag[k]] = (int16_t)sv;
                 }
             }
-            s_val[lane] = wx, s_head[lane] = wh;
         }
-        __syncthreads();
-        // prefix from earlier warps of this tile, then the carry of earlier tiles
-        int pre = 0, pre_head = 0;
-        if (wid > 0) pre = s_val[wid - 1], pre_head = s_head[wid - 1];
-        if (!hx) {
-            x += pre;
-            if (!pre_head) x += carry;
+        if (eobrun > 0) {
+            for (; k <= S.se; k++) {
+                int16_t* c = blk + c_zigzag[k];
+                if (*c != 0 && bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
+            }
+            eobrun--;
         }
-        if (t < total) cf[at] = (int16_t)x;
-        const int tile_val = s_val[nw - 1], tile_head = s_head[nw - 1];
-        __syncthreads();
-        carry = tile_head ? tile_val : carry + tile_val;
     }
+    if (bad) status[S.img] = SMAPB_JPEG_CORRUPT;
 }
 
 // ---- c. dequantisation + IDCT ----------------------------------------------------------------------------------------
@@ -1055,431 +1086,6 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict_
     o[0] = (uint8_t)b, o[1] = (uint8_t)g, o[2] = (uint8_t)r;
 }
 
-// ---- multi-scan phases (SMAPB_JPEG_SCANS) ----------------------------------------------------------------------------
-// Block counts of the multi-scan path saturate at BLOCK_SAT.  An EOB run adds up to 32767 blocks for 15 bits, so plain
-// sums over a scan could pass 2^31; every segment holds far fewer than BLOCK_SAT blocks, so a saturated count is already
-// past the segment's end (nothing is written there) and sums of two saturated counts still fit an int.
-constexpr int BLOCK_SAT = 1 << 29;
-
-__device__ __forceinline__ int sat_add(int a, int b) { return min(a + b, BLOCK_SAT); }
-
-// The coefficient buffer keeps the single-scan layout (frame MCU by frame MCU, the IDCT reads it as it is); a scan's block
-// b (in its own decode order) lands here.
-__device__ __forceinline__ int64_t scan_block(const DevScan& S, const DevImage& I, int b) {
-    const int m = b / S.bpm, j = b - m * S.bpm;
-    if (S.inter) return (int64_t)m * I.bpm + S.blk_map[j];
-    const int bx = m % S.mcux, by = m / S.mcux;
-    return ((int64_t)(by / S.v) * I.mcux + bx / S.h) * I.bpm + S.j0 + (by % S.v) * S.h + bx % S.h;
-}
-
-// huff_run for one scan of a multi-scan file: coefficients Ss..Se of each block, DC first / sequential values as
-// differences (scan_dc_kernel adds them up), AC values stored << Al.  In progressive AC scans (Ss > 0) an EOBn symbol ends
-// a run of 2^n + (n extra bits) blocks; those blocks hold no bits, so the run is counted when its symbol is read and the
-// decoder state stays (bit position, block within the MCU, zig-zag index).
-template <bool WRITE>
-__device__ RunResult scan_run(const DevScan& S, const DevImage& I, const DevHuff* __restrict__ huffs,
-                              const uint32_t* __restrict__ words, uint32_t pos, int blk, int zz, uint32_t stop, uint32_t seg_end,
-                              int16_t* __restrict__ coef, int blk0, int limit) {
-    int nblk = 0, err = -1;
-    const bool eob_runs = S.ss > 0;
-    int16_t* b = nullptr;
-    int b_at = -1;
-    while (pos < stop) {
-        const int k = S.blk_comp[blk];
-        const DevHuff& T = huffs[zz == 0 ? S.dc[k] : S.ac[k]];
-        const uint32_t bits = peek32(words, pos);
-        int len = 0, sym = 0;
-        const uint32_t f = T.fast[bits >> 23];
-        if (f) {
-            len = f >> 8, sym = f & 255;
-        } else {
-            for (int l = 10; l <= 16; l++) {
-                const int code = (int)(bits >> (32 - l));
-                if (code <= T.maxcode[l]) {
-                    len = l;
-                    sym = T.vals[(T.valoff[l] + code) & 255];
-                    break;
-                }
-            }
-            if (!len) {
-                if (err < 0) err = nblk;
-                pos++;
-                continue;
-            }
-        }
-        const int s = sym & 15, r = sym >> 4;
-        const bool eob_n = eob_runs && s == 0 && r < 15;
-        const int extra = eob_n ? r : s;
-        if ((uint64_t)pos + len + extra > seg_end) {
-            if (err < 0) err = nblk;
-            pos = seg_end;
-            break;
-        }
-        int v = 0;
-        if (extra) {
-            v = (int)((bits << len) >> (32 - extra));
-            if (!eob_n && v < (1 << (s - 1))) v += 1 - (1 << s);
-        }
-        if (WRITE && b_at != nblk) {
-            b_at = nblk;
-            b = blk0 + nblk < limit ? coef + scan_block(S, I, blk0 + nblk) * 64 : nullptr;
-        }
-        int done = 0;  // blocks this unit completes
-        if (zz == 0) {
-            if (WRITE && b) b[0] = (int16_t)v;
-            zz = 1;
-            if (S.se == 0) done = 1;
-        } else if (s == 0) {
-            if (r == 15) {
-                zz += 16;
-                if (zz > S.se + 1) {
-                    if (err < 0) err = nblk;
-                    done = 1;
-                } else if (zz == S.se + 1) {
-                    done = 1;
-                }
-            } else {
-                done = eob_n ? (1 << r) + v : 1;
-            }
-        } else {
-            zz += r;
-            if (zz > S.se) {
-                if (err < 0) err = nblk;
-                done = 1;
-            } else {
-                if (WRITE && b) b[c_zigzag[zz]] = (int16_t)((unsigned)v << S.al);
-                if (++zz > S.se) done = 1;
-            }
-        }
-        pos += len + extra;
-        if (done) {
-            zz = S.ss;
-            nblk = min(nblk + done, BLOCK_SAT);
-            if (++blk == S.bpm) blk = 0;
-        }
-    }
-    return {pos, blk, zz, nblk, err};
-}
-
-// Sync passes over the subsequences [sub_lo, sub_lo + nsub) of one round: huff_sync_kernel on scan descriptors.
-__global__ void __launch_bounds__(256) scan_sync_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                        const DevHuff* __restrict__ huffs, const DevSeg* __restrict__ segs,
-                                                        const DevSub* __restrict__ subs, int sub_lo, int nsub,
-                                                        const uint8_t* __restrict__ unst, const SubState* __restrict__ prev,
-                                                        SubState* __restrict__ cur, int* __restrict__ changed, int pass) {
-    if (pass >= 2 && changed[pass - 1] == 0) return;
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= nsub) return;
-    const int i = sub_lo + t;
-    const DevSub U = subs[i];
-    const DevScan& S = scans[U.img];
-    const DevImage& I = imgs[S.img];
-    const DevSeg& G = segs[U.seg];
-    unsigned long long start;
-    if (pass == 0) {
-        start = pack_state(U.bit_begin, 0, S.ss);
-    } else {
-        if (G.sub0 == i) {
-            cur[i] = prev[i];
-            return;
-        }
-        start = prev[i - 1].exit;
-        if (start == prev[i].start) {
-            cur[i] = prev[i];
-            return;
-        }
-    }
-    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
-    if (pass == 0 && G.sub0 != i) {
-        const uint32_t from = U.bit_begin - min(U.bit_begin - G.bit_begin, (uint32_t)WARM_BITS);
-        const RunResult W = scan_run<false>(S, I, huffs, words, from, 0, S.ss, U.bit_begin, G.bit_end, nullptr, 0, 0);
-        start = pack_state(W.pos, W.blk, W.zz);
-    }
-    SubState r;
-    r.start = start;
-    const RunResult R = scan_run<false>(S, I, huffs, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255,
-                                        U.bit_end, G.bit_end, nullptr, 0, 0);
-    r.exit = pack_state(R.pos, R.blk, R.zz);
-    r.nblk = R.nblk;
-    r.errblk = R.err >= 0 ? R.err : 0x7fffffff;
-    cur[i] = r;
-    changed[pass] = 1;
-}
-
-// One CTA per scan of list[]: base[i] = blocks completed in subsequence i's restart segment up to and including i (a
-// segmented, saturating inclusive scan), and the checks of huff_prefix_kernel; a failed check marks the image corrupt.
-__global__ void __launch_bounds__(1024) scan_prefix_kernel(const DevScan* __restrict__ scans, const int* __restrict__ list,
-                                                           const DevSeg* __restrict__ segs, const DevSub* __restrict__ subs,
-                                                           const SubState* __restrict__ st, int* __restrict__ base,
-                                                           int* __restrict__ status) {
-    const DevScan& S = scans[list[blockIdx.x]];
-    __shared__ int s_head[32], s_val[32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    int carry = 0;
-    for (int j0 = 0; j0 < S.nsub; j0 += blockDim.x) {
-        const int j = j0 + threadIdx.x;
-        int x = 0, hx = 0;
-        if (j < S.nsub) {
-            const int i = S.sub0 + j;
-            x = st[i].nblk;
-            hx = segs[subs[i].seg].sub0 == i;
-        }
-        // (h1, v1) + (h2, v2) = (h1 | h2, h2 ? v2 : sat(v1 + v2)), as in dc_scan_kernel
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, x, o), hy = __shfl_up_sync(0xffffffffu, hx, o);
-            if (lane >= o) {
-                if (!hx) x = sat_add(x, y);
-                hx |= hy;
-            }
-        }
-        if (lane == 31) s_head[wid] = hx, s_val[wid] = x;
-        __syncthreads();
-        if (wid == 0) {
-            int wx = lane < nw ? s_val[lane] : 0, wh = lane < nw ? s_head[lane] : 0;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, wx, o), hy = __shfl_up_sync(0xffffffffu, wh, o);
-                if (lane >= o) {
-                    if (!wh) wx = sat_add(wx, y);
-                    wh |= hy;
-                }
-            }
-            s_val[lane] = wx, s_head[lane] = wh;
-        }
-        __syncthreads();
-        if (!hx) {
-            if (wid > 0) x = sat_add(x, s_val[wid - 1]);
-            if (wid == 0 || !s_head[wid - 1]) x = sat_add(x, carry);
-        }
-        if (j < S.nsub) base[S.sub0 + j] = x;
-        const int tile_val = s_val[nw - 1], tile_head = s_head[nw - 1];
-        __syncthreads();
-        carry = tile_head ? tile_val : sat_add(carry, tile_val);
-    }
-    __syncthreads();
-    bool bad = false;
-    for (int j = threadIdx.x; j < S.nsub; j += blockDim.x) {
-        const int i = S.sub0 + j;
-        const SubState s = st[i];
-        const DevSeg& G = segs[subs[i].seg];
-        if (s.errblk != 0x7fffffff && sat_add(G.sub0 == i ? 0 : base[i - 1], s.errblk) < G.nmcu * S.bpm) bad = true;
-        if (i == G.sub0 + G.nsub - 1 && base[i] < G.nmcu * S.bpm) bad = true;  // the segment ends short of its blocks
-    }
-    if (bad) status[S.img] = SMAPB_JPEG_CORRUPT;
-}
-
-__global__ void __launch_bounds__(256) scan_write_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                         const DevHuff* __restrict__ huffs, const DevSeg* __restrict__ segs,
-                                                         const DevSub* __restrict__ subs, int sub_lo, int nsub,
-                                                         const uint8_t* __restrict__ unst, const SubState* __restrict__ st,
-                                                         const int* __restrict__ base, const int* __restrict__ status,
-                                                         int16_t* __restrict__ coef) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= nsub) return;
-    const int i = sub_lo + t;
-    const DevSub U = subs[i];
-    const DevScan& S = scans[U.img];
-    if (status[S.img] != SMAPB_JPEG_OK) return;
-    const DevImage& I = imgs[S.img];
-    const DevSeg& G = segs[U.seg];
-    const unsigned long long start = st[i].start;
-    const int first = G.first_mcu * S.bpm;
-    const int local = G.sub0 == i ? 0 : base[i - 1];  // blocks of the segment completed before this subsequence
-    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
-    scan_run<true>(S, I, huffs, words, (uint32_t)start, (int)(start >> 32) & 255, (int)(start >> 40) & 255, U.bit_end, G.bit_end,
-                   coef + I.coef_off * 64, first + local, first + G.nmcu * S.bpm);
-}
-
-// DC prediction of a sequential or DC-first scan: dc_scan_kernel over the scan's blocks of one scan component (grid.y),
-// reset at every restart; the block keeps the low 16 bits of (sum << Al).
-__global__ void __launch_bounds__(1024) scan_dc_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                       const int* __restrict__ list, const int* __restrict__ status,
-                                                       int16_t* __restrict__ coef) {
-    const DevScan& S = scans[list[blockIdx.x]];
-    const DevImage& I = imgs[S.img];
-    const int k = blockIdx.y;
-    if (k >= S.ncomp || status[S.img] != SMAPB_JPEG_OK) return;
-    int j0 = 0, nc = 0;
-    for (int j = 0; j < S.bpm; j++) {
-        if (S.blk_comp[j] < k) j0++;
-        if (S.blk_comp[j] == k) nc++;
-    }
-    const int total = S.nmcu * nc;
-    int16_t* cf = coef + I.coef_off * 64;
-    __shared__ int s_head[32], s_val[32];
-    int carry = 0;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    for (int t0 = 0; t0 < total; t0 += blockDim.x) {
-        const int t = t0 + threadIdx.x;
-        int v = 0, head = 0;
-        int64_t at = 0;
-        if (t < total) {
-            const int m = t / nc, kk = t % nc;
-            at = scan_block(S, I, m * S.bpm + j0 + kk) * 64;
-            v = cf[at];
-            head = (kk == 0 && m % S.per == 0) ? 1 : 0;
-        }
-        int x = v, hx = head;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, x, o), hy = __shfl_up_sync(0xffffffffu, hx, o);
-            if (lane >= o) {
-                if (!hx) x += y;
-                hx |= hy;
-            }
-        }
-        if (lane == 31) s_head[wid] = hx, s_val[wid] = x;
-        __syncthreads();
-        if (wid == 0) {
-            int wx = lane < nw ? s_val[lane] : 0, wh = lane < nw ? s_head[lane] : 0;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, wx, o), hy = __shfl_up_sync(0xffffffffu, wh, o);
-                if (lane >= o) {
-                    if (!wh) wx += y;
-                    wh |= hy;
-                }
-            }
-            s_val[lane] = wx, s_head[lane] = wh;
-        }
-        __syncthreads();
-        int pre = 0, pre_head = 0;
-        if (wid > 0) pre = s_val[wid - 1], pre_head = s_head[wid - 1];
-        if (!hx) {
-            x += pre;
-            if (!pre_head) x += carry;
-        }
-        if (t < total) cf[at] = (int16_t)((unsigned)x << S.al);
-        const int tile_val = s_val[nw - 1], tile_head = s_head[nw - 1];
-        __syncthreads();
-        carry = tile_head ? tile_val : carry + tile_val;
-    }
-}
-
-// DC refinement: one raw bit per block, the n-th bit of its restart segment for the segment's n-th block; sets bit Al.
-__global__ void __launch_bounds__(256) dc_refine_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                        const int* __restrict__ list, const DevSeg* __restrict__ segs,
-                                                        const uint8_t* __restrict__ unst, int* __restrict__ status,
-                                                        int16_t* __restrict__ coef) {
-    const DevScan& S = scans[list[blockIdx.y]];
-    const DevImage& I = imgs[S.img];
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= S.nmcu * S.bpm || status[S.img] != SMAPB_JPEG_OK) return;
-    const DevSeg& G = segs[S.seg0 + t / S.bpm / S.per];
-    const uint32_t pos = G.bit_begin + (uint32_t)(t - G.first_mcu * S.bpm);
-    if (pos >= G.bit_end) {
-        status[S.img] = SMAPB_JPEG_CORRUPT;
-        return;
-    }
-    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
-    if (peek32(words, pos) >> 31) {
-        int16_t* c = coef + (I.coef_off + scan_block(S, I, t)) * 64;
-        c[0] = (int16_t)(c[0] | (1 << S.al));
-    }
-}
-
-// AC refinement (libjpeg's decode_mcu_AC_refine): the bits a block takes depend on which of its coefficients are already
-// nonzero, so no speculative decoder can start mid-segment; one thread decodes one restart segment.  It reads and writes
-// only the current block's coefficients, at or after its zig-zag position.
-__global__ void __launch_bounds__(128) ac_refine_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                        const DevHuff* __restrict__ huffs, const int* __restrict__ list, int n,
-                                                        const DevSeg* __restrict__ segs, const uint8_t* __restrict__ unst,
-                                                        int* __restrict__ status, int16_t* __restrict__ coef) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    const DevSeg& G = segs[list[t]];
-    const DevScan& S = scans[G.img];
-    const DevImage& I = imgs[S.img];
-    if (status[S.img] != SMAPB_JPEG_OK) return;
-    const DevHuff& T = huffs[S.ac[0]];
-    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
-    int16_t* cf = coef + I.coef_off * 64;
-    const int p1 = 1 << S.al, m1 = -(1 << S.al);
-    uint32_t pos = G.bit_begin;
-    const uint32_t end = G.bit_end;
-    bool bad = false;
-    int eobrun = 0;
-    auto bit = [&]() -> int {
-        if (pos >= end) {
-            bad = true;
-            return 0;
-        }
-        return (int)(peek32(words, pos++) >> 31);
-    };
-    for (int q = 0; q < G.nmcu && !bad; q++) {
-        int16_t* blk = cf + scan_block(S, I, G.first_mcu + q) * 64;
-        int k = S.ss;
-        if (eobrun == 0) {
-            for (; k <= S.se && !bad; k++) {
-                const uint32_t bits = peek32(words, pos);
-                int len = 0, sym = 0;
-                const uint32_t f = T.fast[bits >> 23];
-                if (f) {
-                    len = f >> 8, sym = f & 255;
-                } else {
-                    for (int l = 10; l <= 16; l++) {
-                        const int code = (int)(bits >> (32 - l));
-                        if (code <= T.maxcode[l]) {
-                            len = l;
-                            sym = T.vals[(T.valoff[l] + code) & 255];
-                            break;
-                        }
-                    }
-                }
-                if (!len || pos + len > end) {
-                    bad = true;
-                    break;
-                }
-                pos += len;
-                int r = sym >> 4, s = sym & 15, sv = 0;
-                if (s) {
-                    if (s != 1) {
-                        bad = true;
-                        break;
-                    }
-                    sv = bit() ? p1 : m1;
-                } else if (r != 15) {
-                    eobrun = 1 << r;
-                    if (r) {
-                        if (pos + r > end) {
-                            bad = true;
-                            break;
-                        }
-                        eobrun += (int)(peek32(words, pos) >> (32 - r));
-                        pos += r;
-                    }
-                    break;
-                }
-                do {
-                    int16_t* c = blk + c_zigzag[k];
-                    if (*c != 0) {
-                        if (bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
-                    } else if (--r < 0) {
-                        break;
-                    }
-                    k++;
-                } while (k <= S.se);
-                if (sv) {
-                    if (k > S.se) {
-                        bad = true;
-                        break;
-                    }
-                    blk[c_zigzag[k]] = (int16_t)sv;
-                }
-            }
-        }
-        if (eobrun > 0) {
-            for (; k <= S.se; k++) {
-                int16_t* c = blk + c_zigzag[k];
-                if (*c != 0 && bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
-            }
-            eobrun--;
-        }
-    }
-    if (bad) status[S.img] = SMAPB_JPEG_CORRUPT;
-}
-
 template <typename T>
 cudaError_t grow(T** p, size_t* cap, size_t n) {
     if (n <= *cap) return cudaSuccess;
@@ -1512,7 +1118,7 @@ struct JpegWorkspace {
     size_t small_cap = 0;
     int* small_host = nullptr;  // pinned
     size_t small_host_cap = 0;
-    int sub_bits = SUB_BITS;  // subsequence length of multi-scan decoding (SMAPB_JPEG_SUB_BITS)
+    int sub_bits = SUB_BITS;  // subsequence length of the Huffman passes (SMAPB_JPEG_SUB_BITS)
 };
 
 JpegWorkspace* jpeg_workspace_create() {
@@ -1536,202 +1142,6 @@ void jpeg_workspace_destroy(JpegWorkspace* ws) {
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int* status,
-                cudaStream_t st, int64_t* launches, std::string* err) {
-#define JCK(call)                                                                                             \
-    do {                                                                                                      \
-        cudaError_t e_ = (call);                                                                              \
-        if (e_ != cudaSuccess) {                                                                              \
-            *err = std::string(#call) + ": " + cudaGetErrorString(e_) + " @jpeg.cu:" + std::to_string(__LINE__); \
-            return -10;                                                                                       \
-        }                                                                                                     \
-    } while (0)
-    if (n < 0 || (n > 0 && (!jpeg || !nbytes || !bgr || !status))) {
-        *err = "smapb_decode_jpeg: null argument";
-        return -1;
-    }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    JCK(cudaStreamIsCapturing(st, &cap));
-    if (cap != cudaStreamCaptureStatusNone) {
-        *err = "smapb_decode_jpeg: not capturable (it synchronises and may grow its workspace)";
-        return -1;
-    }
-    // host: parse, then lay out descriptors and scan bytes
-    std::vector<Header> H(n);
-    std::vector<int> idx;  // images that go to the device
-    for (int i = 0; i < n; i++) {
-        status[i] = jpeg ? jpeg_parse(jpeg[i], nbytes[i], &H[i]) : SMAPB_JPEG_MALFORMED;
-        if (status[i] == SMAPB_JPEG_OK) {
-            if (!bgr[i]) {
-                *err = "smapb_decode_jpeg: no output buffer for decodable image " + std::to_string(i);
-                return -1;
-            }
-            idx.push_back(i);
-        }
-    }
-    const int m = (int)idx.size();
-    if (m == 0) return 0;
-    std::vector<DevImage> imgs(m);
-    std::vector<DevSeg> segs;
-    std::vector<DevSub> subs;
-    int64_t raw_total = 0, unst_total = 0, coef_blocks = 0, plane_total = 0;
-    int max_blocks = 0;
-    int64_t max_px = 0;
-    int max_nsub_seg = 1;
-    for (int k = 0; k < m; k++) {
-        const Header& h = H[idx[k]];
-        DevImage& I = imgs[k];
-        memset(&I, 0, sizeof(I));
-        I.h = h.h, I.w = h.w, I.out_h = h.out_h, I.out_w = h.out_w, I.orientation = h.orientation, I.ncomp = h.ncomp;
-        I.hmax = h.hmax, I.vmax = h.vmax, I.mcux = h.mcux, I.mcuy = h.mcuy, I.nmcu = h.nmcu;
-        I.per = h.dri ? h.dri : h.nmcu;
-        I.nseg = (int)h.seg_begin.size();
-        I.out = bgr[idx[k]];
-        int j = 0;
-        for (int c = 0; c < h.ncomp; c++) {
-            for (int v = 0; v < h.comp_v[c]; v++)
-                for (int u = 0; u < h.comp_h[c]; u++) I.blk_comp[j] = c, I.blk_dx[j] = u, I.blk_dy[j] = v, j++;
-            I.comp_h[c] = h.comp_h[c], I.comp_v[c] = h.comp_v[c];
-            I.plane_w[c] = h.mcux * h.comp_h[c] * 8;
-            I.plane_h[c] = h.mcuy * h.comp_v[c] * 8;
-            I.plane_off[c] = plane_total;
-            plane_total += align_up((size_t)I.plane_w[c] * I.plane_h[c], 256);
-            for (int q = 0; q < 64; q++) I.qt[c][q] = (int16_t)h.qt[c][q];
-            if (!build_huff(*h.dc[c], &I.dc[c]) || !build_huff(*h.ac[c], &I.ac[c])) {
-                status[idx[k]] = SMAPB_JPEG_MALFORMED;
-            }
-        }
-        I.bpm = j;
-        I.raw_off = raw_total;
-        I.raw_len = h.seg_end.back() - h.seg_begin.front();
-        raw_total += align_up(I.raw_len, 16);
-        I.unst_off = unst_total;
-        I.coef_off = coef_blocks;
-        coef_blocks += (int64_t)h.nmcu * I.bpm;
-        max_blocks = std::max(max_blocks, h.nmcu * I.bpm);
-        max_px = std::max(max_px, (int64_t)h.h * h.w);
-        I.seg0 = (int)segs.size();
-        I.sub0 = (int)subs.size();
-        uint32_t bit = 0;
-        for (int s = 0; s < I.nseg; s++) {
-            const int64_t len = h.seg_end[s] - h.seg_begin[s] - h.seg_stuffed[s];
-            DevSeg G;
-            G.img = k;
-            G.first_mcu = s * I.per;
-            G.nmcu = std::min(I.per, h.nmcu - G.first_mcu);
-            G.bit_begin = bit;
-            G.bit_end = bit + (uint32_t)(len * 8);
-            G.sub0 = (int)subs.size();
-            G.nsub = std::max(1, (int)((len * 8 + SUB_BITS - 1) / SUB_BITS));
-            for (int u = 0; u < G.nsub; u++) {
-                DevSub S;
-                S.img = k;
-                S.seg = (int)segs.size();
-                S.bit_begin = std::min(G.bit_end, G.bit_begin + (uint32_t)u * SUB_BITS);
-                S.bit_end = u == G.nsub - 1 ? G.bit_end : G.bit_begin + (uint32_t)(u + 1) * SUB_BITS;
-                subs.push_back(S);
-            }
-            max_nsub_seg = std::max(max_nsub_seg, G.nsub);
-            segs.push_back(G);
-            bit = G.bit_end;
-        }
-        I.nsub = (int)subs.size() - I.sub0;
-        unst_total += align_up(bit / 8 + 16, 16);
-    }
-    // staging layout: images | segments | subsequences | scan bytes
-    const size_t o_img = 0, o_seg = align_up(o_img + sizeof(DevImage) * m, 256),
-                 o_sub = align_up(o_seg + sizeof(DevSeg) * segs.size(), 256),
-                 o_raw = align_up(o_sub + sizeof(DevSub) * subs.size(), 256), total = o_raw + raw_total;
-    if (total > ws->host_cap) {
-        if (ws->host) cudaFreeHost(ws->host);
-        ws->host = nullptr;
-        ws->host_cap = 0;
-        JCK(cudaMallocHost((void**)&ws->host, total));
-        ws->host_cap = total;
-    }
-    JCK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
-    memcpy(ws->host + o_img, imgs.data(), sizeof(DevImage) * m);
-    memcpy(ws->host + o_seg, segs.data(), sizeof(DevSeg) * segs.size());
-    memcpy(ws->host + o_sub, subs.data(), sizeof(DevSub) * subs.size());
-    for (int k = 0; k < m; k++) {
-        const Header& h = H[idx[k]];
-        memcpy(ws->host + o_raw + imgs[k].raw_off, jpeg[idx[k]] + h.seg_begin.front(), imgs[k].raw_len);
-    }
-    const int nsub = (int)subs.size();
-    const int max_passes = max_nsub_seg + 1;
-    JCK(grow(&ws->dev_in, &ws->dev_in_cap, total));
-    JCK(grow(&ws->unst, &ws->unst_cap, (size_t)unst_total));
-    JCK(grow(&ws->st[0], &ws->st_cap[0], (size_t)nsub));
-    JCK(grow(&ws->st[1], &ws->st_cap[1], (size_t)nsub));
-    JCK(grow(&ws->base, &ws->base_cap, (size_t)nsub));
-    JCK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
-    JCK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
-    JCK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
-    if ((size_t)m + PASS_GROUP > ws->small_host_cap) {
-        if (ws->small_host) cudaFreeHost(ws->small_host);
-        ws->small_host = nullptr;
-        ws->small_host_cap = 0;
-        JCK(cudaMallocHost((void**)&ws->small_host, sizeof(int) * (m + PASS_GROUP)));
-        ws->small_host_cap = m + PASS_GROUP;
-    }
-    const DevImage* d_img = (const DevImage*)(ws->dev_in + o_img);
-    const DevSeg* d_seg = (const DevSeg*)(ws->dev_in + o_seg);
-    const DevSub* d_sub = (const DevSub*)(ws->dev_in + o_sub);
-    const uint8_t* d_raw = ws->dev_in + o_raw;
-    int* d_status = ws->small;
-    int* d_changed = ws->small + m;
-    for (int k = 0; k < m; k++) ws->small_host[k] = status[idx[k]];
-    JCK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
-    JCK(cudaMemcpyAsync(d_status, ws->small_host, sizeof(int) * m, cudaMemcpyHostToDevice, st));
-    JCK(cudaMemsetAsync(d_changed, 0, sizeof(int) * (max_passes + PASS_GROUP), st));
-    JCK(cudaMemsetAsync(ws->coef, 0, (size_t)coef_blocks * 64 * sizeof(int16_t), st));
-    // a. unstuffing
-    unstuff_kernel<DevImage><<<m, 1024, 0, st>>>(d_img, d_raw, ws->unst);
-    JCK(cudaGetLastError());
-    ++*launches;
-    // b. speculative pass, then sync passes until a pass changes nothing (at most one per subsequence of the longest segment)
-    const int sgrid = (nsub + 255) / 256;
-    int pass = 0, final_pass = -1;
-    while (final_pass < 0) {
-        const int stop = std::min(pass + PASS_GROUP, max_passes + 1);
-        const int first = pass;
-        for (; pass < stop; pass++) {
-            huff_sync_kernel<<<sgrid, 256, 0, st>>>(d_img, d_seg, d_sub, nsub, ws->unst, ws->st[(pass + 1) & 1], ws->st[pass & 1],
-                                                    d_changed, pass);
-            JCK(cudaGetLastError());
-            ++*launches;
-        }
-        JCK(cudaMemcpyAsync(ws->small_host, d_changed + first, sizeof(int) * (stop - first), cudaMemcpyDeviceToHost, st));
-        JCK(cudaStreamSynchronize(st));
-        for (int p = first; p < stop; p++)
-            if (p > 0 && ws->small_host[p - first] == 0) {
-                final_pass = p;
-                break;
-            }
-        if (final_pass < 0 && pass > max_passes) {
-            *err = "smapb_decode_jpeg: Huffman sync passes did not converge";
-            return -11;
-        }
-    }
-    const SubState* fin = ws->st[final_pass & 1];
-    huff_prefix_kernel<<<m, 1024, 0, st>>>(d_img, d_seg, fin, ws->base, d_status);
-    huff_write_kernel<<<sgrid, 256, 0, st>>>(d_img, d_seg, d_sub, nsub, ws->unst, fin, ws->base, d_status, ws->coef);
-    dc_scan_kernel<<<dim3(m, 3), 1024, 0, st>>>(d_img, d_status, ws->coef);
-    JCK(cudaGetLastError());
-    // c. IDCT
-    idct_kernel<<<dim3((max_blocks + 127) / 128, m), 128, 0, st>>>(d_img, ws->coef, ws->planes, d_status);
-    // d. upsampling, colour, orientation
-    colour_kernel<<<dim3((unsigned)((max_px + 255) / 256), m), 256, 0, st>>>(d_img, ws->planes, d_status);
-    JCK(cudaGetLastError());
-    *launches += 5;
-    JCK(cudaMemcpyAsync(ws->small_host, d_status, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
-    JCK(cudaStreamSynchronize(st));
-    for (int k = 0; k < m; k++)
-        if (status[idx[k]] == SMAPB_JPEG_OK) status[idx[k]] = ws->small_host[k];
-    return 0;
-#undef JCK
-}
-
 namespace {
 // What one round (the r-th scan of every image that has one) launches: subsequences [sub_lo, sub_lo + nsub) of its
 // Huffman scans, and ranges of the batch's index list (scans, or segments for AC refinement).
@@ -1741,8 +1151,8 @@ struct Round {
 };
 }  // namespace
 
-int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr,
-                      int* status, cudaStream_t st, int64_t* launches, std::string* err) {
+int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int flags,
+                int* status, cudaStream_t st, int64_t* launches, std::string* err) {
 #define JCK(call)                                                                                             \
     do {                                                                                                      \
         cudaError_t e_ = (call);                                                                              \
@@ -1761,10 +1171,11 @@ int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, cons
         *err = "smapb_decode_jpeg_ex: not capturable (it synchronises and may grow its workspace)";
         return -1;
     }
+    // host: parse, then lay out descriptors and scan bytes
     std::vector<ScanHeader> H(n);
-    std::vector<int> idx;
+    std::vector<int> idx;  // images that go to the device
     for (int i = 0; i < n; i++) {
-        status[i] = jpeg ? jpeg_parse_scans(jpeg[i], nbytes[i], &H[i]) : SMAPB_JPEG_MALFORMED;
+        status[i] = jpeg ? jpeg_parse(jpeg[i], nbytes[i], flags, &H[i]) : SMAPB_JPEG_MALFORMED;
         if (status[i] == SMAPB_JPEG_OK) {
             if (!bgr[i]) {
                 *err = "smapb_decode_jpeg_ex: no output buffer for decodable image " + std::to_string(i);
@@ -1832,21 +1243,23 @@ int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, cons
             int j = 0;
             for (int q = 0; q < P.ncomp; q++) {
                 const int c = P.comp[q];
-                int j0c = 0;
-                for (int e = 0; e < c; e++) j0c += h.comp_h[e] * h.comp_v[e];
-                for (int v = 0; v < h.comp_v[c]; v++)
-                    for (int u = 0; u < h.comp_h[c]; u++) D.blk_comp[j] = q, D.blk_map[j] = j0c + v * h.comp_h[c] + u, j++;
-                D.h = h.comp_h[c], D.v = h.comp_v[c], D.j0 = j0c;  // used when the scan has one component
+                int dc = 0, ac = 0;
                 if (D.kind == SCAN_HUFF && P.ss == 0) {
-                    D.dc[q] = (int)huffs.size();
+                    dc = (int)huffs.size();
                     huffs.emplace_back();
                     build_huff(P.dc[q], &huffs.back());
                 }
                 if (D.kind != SCAN_DC_REFINE && P.se > 0) {
-                    D.ac[q] = (int)huffs.size();
+                    ac = (int)huffs.size();
                     huffs.emplace_back();
                     build_huff(P.ac[q], &huffs.back());
                 }
+                int j0c = 0;
+                for (int e = 0; e < c; e++) j0c += h.comp_h[e] * h.comp_v[e];
+                for (int v = 0; v < h.comp_v[c]; v++)
+                    for (int u = 0; u < h.comp_h[c]; u++)
+                        D.blk_comp[j] = q, D.blk_map[j] = j0c + v * h.comp_h[c] + u, D.blk_dc[j] = dc, D.blk_ac[j] = ac, j++;
+                D.h = h.comp_h[c], D.v = h.comp_v[c], D.j0 = j0c;  // used when the scan has one component
             }
             if (!D.inter) D.bpm = 1;
             D.raw_off = raw_total;
@@ -1860,7 +1273,7 @@ int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, cons
             for (int s = 0; s < D.nseg; s++) {
                 const int64_t len = P.seg_end[s] - P.seg_begin[s] - P.seg_stuffed[s];
                 DevSeg G;
-                G.img = si;
+                G.scan = si;
                 G.first_mcu = s * D.per;
                 G.nmcu = std::min(D.per, D.nmcu - G.first_mcu);
                 G.bit_begin = bit;
@@ -1871,7 +1284,7 @@ int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, cons
                     G.nsub = std::max(1, (int)((len * 8 + ws->sub_bits - 1) / ws->sub_bits));
                     for (int u = 0; u < G.nsub; u++) {
                         DevSub U;
-                        U.img = si;
+                        U.scan = si;
                         U.seg = (int)segs.size();
                         U.bit_begin = std::min(G.bit_end, G.bit_begin + (uint32_t)u * ws->sub_bits);
                         U.bit_end = u == G.nsub - 1 ? G.bit_end : G.bit_begin + (uint32_t)(u + 1) * ws->sub_bits;
@@ -1969,7 +1382,7 @@ int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, cons
     JCK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
     JCK(cudaMemcpyAsync(d_status, ws->small_host, sizeof(int) * m, cudaMemcpyHostToDevice, st));
     JCK(cudaMemsetAsync(ws->coef, 0, (size_t)coef_blocks * 64 * sizeof(int16_t), st));
-    unstuff_kernel<DevScan><<<nscan, 1024, 0, st>>>(d_scan, d_raw, ws->unst);
+    unstuff_kernel<<<nscan, 1024, 0, st>>>(d_scan, d_raw, ws->unst);
     JCK(cudaGetLastError());
     ++*launches;
     for (const Round& R : rounds) {
@@ -2043,18 +1456,8 @@ extern "C" {
 int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status) {
     if (!status || (flags & ~SMAPB_JPEG_SCANS)) return -1;
     smapb::ScanHeader M;
-    smapb::Header& H = M.f;
-    if (flags & SMAPB_JPEG_SCANS) {
-        *status = smapb::jpeg_parse_scans(data, nbytes, &M);  // checks the tables of every scan
-    } else {
-        *status = smapb::jpeg_parse(data, nbytes, &H);
-        if (*status == SMAPB_JPEG_OK) {
-            for (int c = 0; c < H.ncomp; c++) {
-                smapb::DevHuff d;
-                if (!smapb::build_huff(*H.dc[c], &d) || !smapb::build_huff(*H.ac[c], &d)) *status = SMAPB_JPEG_MALFORMED;
-            }
-        }
-    }
+    *status = smapb::jpeg_parse(data, nbytes, flags, &M);
+    const smapb::Header& H = M.f;
     const bool ok = *status == SMAPB_JPEG_OK;
     if (h) *h = ok ? H.out_h : 0;
     if (w) *w = ok ? H.out_w : 0;

@@ -1,4 +1,4 @@
-// Baseline JPEG decoding on the GPU (jpeg.cu): host marker parser + batched device phases.
+// Huffman JPEG decoding on the GPU (jpeg.cu): host marker walk + batched device phases.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,14 +12,12 @@ struct JpegWorkspace;  // handle-owned device / pinned buffers, grown on demand
 JpegWorkspace* jpeg_workspace_create();
 void jpeg_workspace_destroy(JpegWorkspace* ws);
 
-// Decodes the images whose headers the decoder supports into bgr[i] (uint8 [out_h, out_w, 3], device), and reports
-// status[i] (SMAPB_JPEG_*) for every image.  Synchronises `st` before returning.  0 on success; otherwise a CUDA error or
-// -1 for bad arguments, with the text in *err.  *launches is incremented by the number of kernels launched.
-int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int* status,
-                cudaStream_t st, int64_t* launches, std::string* err);
-// The same for a batch that may also hold sequential files with several scans and progressive Huffman files
-// (SMAPB_JPEG_SCANS): the scans run in rounds, the r-th scan of every image in round r.
-int jpeg_decode_scans(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr,
-                      int* status, cudaStream_t st, int64_t* launches, std::string* err);
+// Decodes the images whose headers the decoder accepts into bgr[i] (uint8 [out_h, out_w, 3], device), and reports
+// status[i] (SMAPB_JPEG_*) for every image.  flags = 0 accepts baseline files only; SMAPB_JPEG_SCANS also accepts
+// sequential files with several scans and progressive Huffman files.  The scans run in rounds, the r-th scan of every
+// image in round r.  Synchronises `st` before returning.  0 on success; otherwise a CUDA error or -1 for bad arguments,
+// with the text in *err.  *launches is incremented by the number of kernels launched.
+int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int flags,
+                int* status, cudaStream_t st, int64_t* launches, std::string* err);
 
 }  // namespace smapb
