@@ -17,10 +17,10 @@ extern "C" {
  *   name=<unit name>  kind=conv | conv_f32 | stem_tc | stem | s2d | maxpool | upadd
  *     conv: tensor-core conv with split-bf16 output; conv_f32: fp32 NHWC output (heads, *.tapexp); stem_tc: the 7x7/s2
  *     stem as a 4x1-tap conv over the s2d view; stem: the CUDA-core stem; s2d: space-to-depth of the image
- *   inputs by role, as dump indices, absent roles left out: in= in2= res= p1= p2= up= (convs), a= b= (maxpool, upadd);
+ *   inputs by role, as dump indices, absent roles left out: in= res= p1= p2= in2= up= (convs), a= b= (maxpool, upadd);
  *     in=x is the network input image
  *   convs:  tw= (patch width; 128 on the flat path) rev= (reverse tile order) k=<kh>x<kw> s= pad=<y>x<x> cin= cin2= s2=
- *           cout= (padded) out=NxHxWxC bn= cg= relu= hasres= post= upmode= tiles= nterms=
+ *           cout= (padded) out=NxHxWxC bn= relu= hasres= post= upmode= tiles= nterms=
  *   others: out=NxHxWxC nterms= */
 int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int max_ops, char* desc, int desc_stride);
 /* Raw copy (both bf16 planes, or fp32 for head outputs) of op `idx`'s output into host or device memory (the copy direction
@@ -36,7 +36,8 @@ int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dim
 /* Environment switches read when a handle / plan is built (never on the per-call path):
  *   SMAPB_DEBUG_STOP=n        run only the first n ops of the plan
  *   SMAPB_DEBUG_SYNC=1        synchronise the stream after every launch
- *   SMAPB_FORCE_TILE=bn[,1]   force a tile width (32, 64, 128) wherever it is valid;  SMAPB_NO_AUTOTUNE=1  cost model only
+ *   SMAPB_FORCE_TILE=bn       force a tile width (32, 64, 128) wherever it is valid, except where the tile table or the
+ *                             autotuner picks one;  SMAPB_NO_AUTOTUNE=1  cost model only
  *   SMAPB_ONE_STREAM=1        no side stream;  SMAPB_NO_GRAPH=1  no CUDA graph replay;  SMAPB_PDL=1  programmatic dependent launch
  *   SMAPB_STEM=cuda           CUDA-core stem;  SMAPB_NO_FUSE_DS=1 / SMAPB_NO_FUSE_UP=1  unfused downsample / up-residual
  *   SMAPB_ROLES=1             per-role wait-cycle counters in smapb_conv_test

@@ -1,0 +1,235 @@
+// Internal to libsmap_b200 (not installed): the handle and plan types shared by engine.cu (handle, inference paths, C ABI)
+// and plan.cu (conv set-up, tile choice, weights, execution plan).
+#pragma once
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <stdlib.h>
+
+#include <map>
+#include <memory>
+#include <string>
+#include <vector>
+
+#include "../../include/smap_b200.h"
+#include "conv_tc.cuh"
+#include "jpeg.h"
+#include "preprocess.h"
+#include "refine.h"
+
+namespace smapb {
+
+// split-bf16 NHWC activation tensor: plane 0 = hi, plane 1 = lo
+struct Act {
+    __nv_bfloat16* ptr = nullptr;
+    int N = 0, H = 0, W = 0, C = 0;
+    long long plane() const { return (long long)N * H * W * C; }
+};
+struct ActF32 {
+    float* ptr = nullptr;
+    int N = 0, H = 0, W = 0, C = 0;
+};
+
+struct ConvLayer {
+    std::string name;
+    int Cin = 0, Cout = 0, Cout_pad = 0, k = 1, stride = 1, pad = 0;
+    int Cin2 = 0, stride2 = 1;  // K-concatenated second 1x1 input (weights hold Cin + Cin2 columns)
+    __nv_bfloat16* w_dev = nullptr;  // [T][taps][Cout_pad][Cin]
+    float* bias_dev = nullptr;       // [Cout_pad]
+};
+
+enum OpKind { OP_STEM, OP_S2D, OP_MAXPOOL, OP_CONV, OP_UPADD, OP_HEADMERGE, OP_TAPSUM };
+struct Op {
+    OpKind kind;
+    // conv
+    ConvParams cp;
+    int block_n = 0;
+    double flops = 0;
+    // generic tensors
+    Act a, b, out;
+    ActF32 f4, f3, f2;
+    int cout = 0;  // head merge real channel count
+    int which_out = 0;  // tap sum output: 1 detd, 2 rootd
+    const float* bias = nullptr;  // tap-sum bias
+    // two-stream execution: side-branch ops (skip convs, heads) run on stream 1 and overlap the main chain
+    int stream = 0;
+    std::vector<int> waits;  // indices of producer ops on the OTHER stream this op must wait for
+    bool record = false;     // some op on the other stream consumes this op's output
+    cudaEvent_t ev = nullptr;
+    std::string name;  // reference unit name (NVTX range, profiles)
+    // debug descriptions (smapb_debug_checksums): the tensors the op reads, in the order PlanBuilder::wire received them
+    // (conv: ConvIO::inputs; null = role absent), and the output shape N, H, W, C of a conv
+    std::vector<const void*> inputs;
+    int dims[4] = {0, 0, 0, 0};
+};
+
+struct Plan {
+    int B = 0;
+    std::vector<Op> ops;
+    std::vector<void*> allocs;
+    int n_conv = 0;
+    double conv_flops = 0;
+    std::map<const void*, int> producer;  // tensor -> index of the op that writes it (build time)
+    int last_side = -1;
+};
+
+}  // namespace smapb
+
+struct smapb_handle {
+    int device = 0, max_batch = 0, in_h = 0, in_w = 0, h = 0, w = 0;
+    int sm_count = 132;
+    int sm_reserve = 0;  // SMs the persistent conv grids leave to concurrent kernels
+    std::string err;
+    int64_t launches = 0;
+    // weights
+    std::map<std::string, std::vector<float>> raw;
+    std::map<std::string, std::vector<int64_t>> raw_shape;
+    std::map<std::string, smapb::ConvLayer> layers;
+    float* stem_w = nullptr;  // [147][64]
+    smapb::ConvLayer stem_tc;  // space-to-depth tensor-core stem (4 ky-blocks x 64 k)
+    int stem_tc_ok = -1;      // -1 untested, 0 overlapped TMA view rejected (CUDA-core stem), 1 in use
+    float* stem_b = nullptr;
+    int nterms = 3;  // MMA terms (3 = bf16x3, 1 = bf16 or fp16)
+    int planes = 2;  // activation planes (2 or 1)
+    bool f16 = false;  // element format of weights and activations: fp16 (SMAPB_PREC_FP16) instead of bf16
+    unsigned long long* sat_dev = nullptr;  // fp16: activation elements clamped to +-65504 (smapb_saturation_count)
+    bool finalized = false;
+    std::map<int, std::unique_ptr<smapb::Plan>> plans;
+    // association workspace (sized for max_batch)
+    float* peaks = nullptr;
+    float* scores = nullptr;
+    float* bodies = nullptr;
+    int* counts = nullptr;
+    uint32_t* nms_masks = nullptr;  // one ballot bit per pixel of the key-point planes
+    // whole-path workspace
+    float* imgs_dev = nullptr;
+    float* imgs_flip = nullptr;
+    float* hm = nullptr;
+    float* hm_flip = nullptr;
+    float* detd = nullptr;
+    float* rootd = nullptr;
+    float* scratch_detd = nullptr;
+    float* scratch_rootd = nullptr;
+    double* scales_dev = nullptr;
+    smapb_record* records_dev = nullptr;
+    bool use_pdl = getenv("SMAPB_PDL") != nullptr;  // programmatic dependent launch between conv kernels
+    // host-facing pipeline (smapb_submit_host / smapb_wait): two slots, H2D of slot s+1 overlaps the compute of slot s
+    struct Slot {
+        float* imgs = nullptr;
+        double* scales = nullptr;
+        smapb_record* records = nullptr;
+        smapb_record* records_all = nullptr;  // [comm_world * max_batch], gathered variant
+        cudaEvent_t h2d = nullptr, done = nullptr, rec_ready = nullptr;
+        bool used = false;
+    } slots[2];
+    cudaStream_t copy_stream = nullptr;
+    bool autotune = getenv("SMAPB_NO_AUTOTUNE") == nullptr;
+    bool two_streams = getenv("SMAPB_ONE_STREAM") == nullptr;  // side branches (heads, skip convs) on a second stream
+    cudaStream_t aux_stream = nullptr;  // side branches of the decoder (skip convs, heads) run here
+    // Stream used when the caller passes NULL (= the legacy default stream).  It is NON-blocking - a blocking stream would
+    // be fenced by every legacy-stream operation of the process (e.g. a collective issued by the host framework) - and is
+    // ordered against the legacy stream explicitly with the two bridge events (on_stream in engine.cu).
+    cudaStream_t own_stream = nullptr;
+    cudaEvent_t bridge_in = nullptr, bridge_out = nullptr;
+    struct GraphEntry {
+        int B, flip, gather;
+        const void* imgs;
+        const void* scales;
+        cudaGraphExec_t exec;
+        uint64_t stamp;  // last use (LRU eviction)
+    };
+    std::vector<GraphEntry> graphs;  // whole-path CUDA graphs keyed by (B, flip, gather, input pointers)
+    uint64_t graph_clock = 0;
+    // skeleton-record exchange (SURVEY 8(e)): one ncclAllGather per batch on the compute stream, inside the graph
+    void* comm = nullptr;  // ncclComm_t
+    bool comm_owned = false;
+    int comm_rank = 0, comm_world = 1;
+    smapb_record* gather_dev = nullptr;  // [comm_world * max_batch]
+    // decoupled exchange (smapb_infer_device_gather_async / smapb_submit_host_gather): the all-gather runs on its own stream
+    // behind an event, so a rank's compute stream never waits for its peers
+    cudaStream_t gather_stream = nullptr;
+    cudaEvent_t rec_ready[2] = {nullptr, nullptr}, gather_done[2] = {nullptr, nullptr};
+    smapb_record* rec_buf[2] = {nullptr, nullptr};  // [max_batch] each: the records of the two most recent async calls
+    bool gather_used[2] = {false, false};
+    int gather_idx = 0;
+    double* gt_dist = nullptr;           // [max_batch][127*127] distance matrices of the GT-matching lift
+    bool nccl_in_graph = getenv("SMAPB_NCCL_EAGER") == nullptr;
+    bool nvtx_ops = getenv("SMAPB_NVTX") != nullptr;  // one NVTX range per plan op (phase ranges are always emitted)
+    bool serpentine = getenv("SMAPB_SERPENTINE") != nullptr;
+    // pre-processing (SURVEY 8(f) f1): resampling tables per source geometry, staging for host images
+    struct PreEntry {
+        smapb::ResizePlan plan;
+        smapb::ResizeTablesDev tab{};
+        void* buf = nullptr;
+    };
+    std::map<std::pair<int, int>, PreEntry> pre_cache;
+    uint8_t* pre_stage = nullptr;
+    size_t pre_stage_bytes = 0;
+    smapb::JpegWorkspace* jpeg = nullptr;  // JPEG decoding (smapb_decode_jpeg), created on first use
+    // RefineNet (optional post-processing step, SURVEY 8(f) f2)
+    std::map<std::string, std::vector<float>> refine_raw;
+    float* refine_buf = nullptr;  // folded, transposed weights + biases of the five layers
+    smapb::RefineWeights refine_w{};
+    bool refine_ready = false, refine_on = false;
+    std::map<std::pair<int, int>, int> eager_runs;  // (B, flip) -> number of eager executions so far
+    // profiling (per-op CUDA events on the launching stream)
+    bool profiling = false;
+    std::vector<cudaEvent_t> prof_events;
+    std::vector<int> prof_kind;          // kind of the op that ended at event i (-1 = interval start)
+    std::vector<std::string> prof_desc;  // description of that op
+    std::vector<double> prof_flops;
+    size_t prof_used = 0;
+    // per-launch role counters of the conv kernels inside a profiled (eager) run: SMAPB_ROLES_PLAN=<csv path>
+    long long* roles_dev = nullptr;  // [ROLES_CAP][16]
+    size_t roles_used = 0;
+    std::vector<std::string> roles_desc;
+};
+
+namespace smapb {
+
+constexpr size_t ROLES_CAP = 4096;
+
+inline int fail(smapb_handle* h, int code, const std::string& msg) {
+    if (h) h->err = msg;
+    return code;
+}
+#define CK(call)                                                                                          \
+    do {                                                                                                  \
+        cudaError_t e_ = (call);                                                                          \
+        if (e_ != cudaSuccess)                                                                            \
+            return fail(h, -10, std::string(#call) + ": " + cudaGetErrorString(e_) + " @" + std::to_string(__LINE__)); \
+    } while (0)
+
+template <typename T>
+int dev_alloc(smapb_handle* h, T** p, size_t count) {
+    CK(cudaMalloc((void**)p, count * sizeof(T)));
+    return 0;
+}
+
+enum ProfKind { PK_START = -1, PK_CONV = 0, PK_STEM = 1, PK_ELEM = 2, PK_ASSOC = 3, PK_LIFT = 4, PK_COPY = 5 };
+inline void prof_mark(smapb_handle* h, int kind, cudaStream_t st, const char* desc = "", double flops = 0) {
+    if (!h->profiling) return;
+    if (h->prof_used == h->prof_events.size()) {
+        cudaEvent_t e;
+        cudaEventCreate(&e);
+        h->prof_events.push_back(e);
+        h->prof_kind.push_back(0);
+        h->prof_desc.emplace_back();
+        h->prof_flops.push_back(0);
+    }
+    cudaEventRecord(h->prof_events[h->prof_used], st);
+    h->prof_kind[h->prof_used] = kind;
+    h->prof_desc[h->prof_used] = desc;
+    h->prof_flops[h->prof_used] = flops;
+    h->prof_used++;
+}
+
+// plan.cu
+int build_plan(smapb_handle* h, int B, Plan** out_plan);
+int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float* detd, float* rootd, cudaStream_t st);
+void free_plan(Plan* plan);
+void free_layers(smapb_handle* h);  // the device weights of every conv layer, the tensor-core stem's included
+// engine.cu
+void drop_graphs(smapb_handle* h, bool gather_only = false);  // destroys the cached whole-path graphs (or those with the all-gather)
+
+}  // namespace smapb

@@ -66,7 +66,7 @@ def test_conv_residual_and_post_adds_deterministic(eng, B, H, W, Cin, Cout):
         assert (y - ref).abs().max().item() / ref.abs().max().item() < 2e-5
 
 
-_TILES = ("128,1", "64,1", "32,1")
+_TILES = ("128", "64", "32")
 
 
 @pytest.mark.parametrize("case", _TILE_CASES)
@@ -80,7 +80,7 @@ def test_every_tile_shape_gives_the_same_bits(eng, monkeypatch, case):
     ref = F.relu(ref + res if use_res else ref)
     first, n = None, 0
     for tile in _TILES:
-        bn = int(tile.split(",")[0])
+        bn = int(tile)
         if Cout % bn:
             continue
         monkeypatch.setenv("SMAPB_FORCE_TILE", tile)

@@ -1,6 +1,6 @@
 """Small-shape workload for compute-sanitizer (tools/gpu_sanitize.sh): every kernel family of the library once or twice -
 tensor-core convs in every pipeline configuration (plain, residual ring, post-adds, K-concatenated pair, bilinear residual
-via a whole forward, CTA pairs, thin heads), the elementwise kernels, NMS / PAF / grouping / lift, RefineNet, pre-processing -
+via a whole forward, every tile width, thin heads), the elementwise kernels, NMS / PAF / grouping / lift, RefineNet, pre-processing -
 at sizes the sanitizer's ~100x slowdown tolerates.  Not a test (no numerical check) and not a bench."""
 import os
 import sys
@@ -20,7 +20,7 @@ if which in ("all", "conv"):
     cases = [(1, 16, 24, 64, 64, 1, 1, False), (1, 16, 24, 64, 256, 1, 1, True), (2, 16, 26, 128, 128, 3, 1, False),
              (1, 16, 26, 128, 128, 3, 2, False), (2, 16, 26, 256, 64, 1, 1, False), (1, 16, 24, 256, 14, 3, 1, False),
              (3, 20, 26, 64, 64, 3, 1, False)]
-    for tile in (None, "256,2", "128,2", "64,2", "64,1"):
+    for tile in (None, "128", "64", "32"):
         if tile:
             os.environ["SMAPB_FORCE_TILE"] = tile
         for (B, H, W, Cin, Cout, k, s, res) in cases:

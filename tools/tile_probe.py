@@ -24,7 +24,7 @@ SHAPES = {
     "l4_c3": (8, 16, 26, 512, 2048, 1, 1, True, True),
     "l4_c1": (8, 16, 26, 2048, 512, 1, 1, True, False),
 }
-TILES = ("128,1", "64,1", "32,1")
+TILES = ("128", "64", "32")
 names = sys.argv[1:] or list(SHAPES)
 eng = Engine(0, max_batch=1, in_h=64, in_w=96)
 g = torch.Generator(device="cpu").manual_seed(5)
@@ -39,7 +39,7 @@ for n in names:
     base = None
     out = []
     for t in TILES:
-        if Cout % int(t.split(",")[0]):
+        if Cout % int(t):
             continue
         os.environ["SMAPB_FORCE_TILE"] = t
         try:
