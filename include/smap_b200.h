@@ -55,8 +55,10 @@ int smapb_finalize_weights(smapb_handle* h, int precision);
 
 /* ---- pre-processing (the step in front of the backbone) ------------------------------------------------------ */
 /* Replaces: CustomDataset.__getitem__ after cv2.imread (dataset/custom_dataset.py:27-68): scale = min(net_w/W, net_h/H),
- * cv2.resize(img, (0,0), fx=scale, fy=scale) (8-bit INTER_LINEAR, bit-exact incl. the 1/2-scale INTER_AREA reroute),
- * gray-128 letterbox to net_w x net_h, torchvision ToTensor + Normalize(cfg.INPUT.MEANS, cfg.INPUT.STDS).
+ * cv2.resize(img, (0,0), fx=scale, fy=scale) (8-bit INTER_LINEAR, bit-exact incl. the 1/2-scale INTER_AREA reroute and
+ * its partial blocks at an odd last column or row), gray-128 letterbox to net_w x net_h, torchvision ToTensor +
+ * Normalize(cfg.INPUT.MEANS, cfg.INPUT.STDS).  img_w and img_h: 1 to 16384.  Returns -1 (smapb_last_error names the
+ * geometry) where cv2.resize raises: when rint(img_w * scale) or rint(img_h * scale) is 0, e.g. 16x16384 into 832x512.
  * bgr_dev: uint8 [img_h, img_w, 3] (BGR, as cv2.imread returns); out_nchw_dev: fp32 [3, in_h, in_w] - one image slot of the
  * batch handed to smapb_backbone_forward / smapb_infer_device.  scale_row_host (may be NULL): the image's 9 scale values
  * in SMAPB_SCALE_LEN order, including the default intrinsics of exps/stage3_root2/test.py:99-103. */

@@ -29,7 +29,8 @@ long long smapb_debug_dump(smapb_handle* h, int B, int idx, void* host, long lon
 
 /* Host-only: the resampling plan smapb_preprocess uses for a src_w x src_h image (no GPU work).  dims6 = {dst_w, dst_h,
  * pad_left, pad_top, mode (0 fixed-point bilinear, 1 exact 1/2 scale = 2x2 rounded mean, 2 copy), 0}; the tables (may be
- * NULL) must hold dst_w, 2*dst_w, 2*dst_h and 2*dst_h entries (dst <= net size). */
+ * NULL) must hold dst_w, 2*dst_w, 2*dst_h and 2*dst_h entries (dst <= net size).  Returns -1 for a geometry
+ * smapb_preprocess refuses. */
 int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dims6, double* scale, int* xofs, short* xcoef,
                             int* yofs, short* ycoef);
 

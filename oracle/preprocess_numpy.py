@@ -13,8 +13,9 @@ cv2.resize is a third-party dependency of the reference (opencv-python, unpinned
 VResizeLinear<uchar,int,short,FixedPtCast<int,uchar,22>>): coefficients are float32 weights rounded (half to even) to
 1/2048 steps, the horizontal pass keeps 32-bit sums and the vertical pass computes
 ((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2.  An exact 1/2 scale is rerouted to INTER_AREA, i.e. the
-rounded mean of each 2x2 block.  tests/test_oracle_preprocess.py pins this restatement against cv2 itself and against
-digests of the reference pipeline's outputs (tests/golden/make_golden.py).
+rounded mean of each 2x2 block (of the pixels inside it where the image's last odd column or row cuts the block).  A side
+that rounds to 0 pixels is refused, as cv2 refuses it.  tests/test_oracle_preprocess.py pins this restatement against cv2
+itself and against digests of the reference pipeline's outputs (tests/golden/make_golden.py).
 """
 import numpy as np
 
@@ -49,15 +50,29 @@ def linear_tables(src, dst, inv_scale):
 
 
 def resize_linear_u8(img, fx):
-    """cv2.resize(img, (0, 0), fx=fx, fy=fx) for uint8 HWC images."""
+    """cv2.resize(img, (0, 0), fx=fx, fy=fx) for uint8 HWC images.  Raises ValueError where cv2 raises (!dsize.empty()):
+    a side that rounds to 0 pixels."""
     H, W = img.shape[:2]
     dw, dh = cv_round(W * fx), cv_round(H * fx)
+    if dw <= 0 or dh <= 0:
+        raise ValueError("a %dx%d image resizes to %dx%d at scale %r" % (W, H, dw, dh, fx))
     if (dw, dh) == (W, H):
         return img.copy()
     scale = 1.0 / fx
     if int(scale) == 2 and abs(2 - scale) < np.finfo(np.float64).eps:   # INTER_LINEAR -> INTER_AREA (fast 2x2 mean)
-        s = img[: dh * 2, : dw * 2].astype(np.int32)
-        return ((s[0::2, 0::2] + s[0::2, 1::2] + s[1::2, 0::2] + s[1::2, 1::2] + 2) >> 2).astype(np.uint8)
+        # dw = rint(W / 2) rounds up when W = 3 (mod 4) (likewise H): the last column's (row's) windows are cut by the image
+        # edge.  resizeAreaFast_Invoker averages the pixels inside such a window as saturate_cast<uchar>((float)sum / count),
+        # i.e. the float quotient rounded half to even; full windows keep the SIMD path's (sum + 2) >> 2.
+        s = img.astype(np.int32)
+        acc = np.zeros((dh, dw, 3), np.int32)
+        cnt = np.zeros((dh, dw, 1), np.int32)
+        for oy in (0, 1):
+            for ox in (0, 1):
+                p = s[oy::2, ox::2][:dh, :dw]
+                acc[:p.shape[0], :p.shape[1]] += p
+                cnt[:p.shape[0], :p.shape[1]] += 1
+        part = np.rint(acc.astype(np.float32) / cnt.astype(np.float32))
+        return np.where(cnt == 4, (acc + 2) >> 2, part).astype(np.uint8)
     xo, xa = linear_tables(W, dw, fx)
     yo, yb = linear_tables(H, dh, fx)
     # the vertical taps of the generic resizer are clamped row indices around floor(fy) WITHOUT the f=0 snap used for x:

@@ -312,17 +312,23 @@ int smapb_lift3d_gt(smapb_handle* h, const float* bodies, const int* counts, con
 
 // ---- pre-processing (SURVEY 8(f) f1) ---------------------------------------------------------------------------
 static int pre_entry(smapb_handle* h, int img_h, int img_w, smapb_handle::PreEntry** out) {
-    if (img_h < 2 || img_w < 2 || img_h > 16384 || img_w > 16384) return fail(h, -1, "smapb_preprocess: image size outside [2, 16384]");
     auto key = std::make_pair(img_w, img_h);
     auto it = h->pre_cache.find(key);
     if (it == h->pre_cache.end()) {
+        smapb_handle::PreEntry E;
+        if (!make_resize_plan(img_w, img_h, h->in_w, h->in_h, &E.plan)) {
+            char msg[256];
+            snprintf(msg, sizeof msg,
+                     "smapb_preprocess: a %dx%d image (W x H) does not fit a %dx%d input: sides must be in [1, 16384] and "
+                     "resize to at least 1 pixel (cv2.resize refuses an empty size)",
+                     img_w, img_h, h->in_w, h->in_h);
+            return fail(h, -1, msg);
+        }
         if (h->pre_cache.size() >= 256) {  // bound the cache: drop everything (streams are idle after the sync)
             cudaDeviceSynchronize();
             for (auto& e : h->pre_cache) cudaFree(e.second.buf);
             h->pre_cache.clear();
         }
-        smapb_handle::PreEntry E;
-        make_resize_plan(img_w, img_h, h->in_w, h->in_h, &E.plan);
         const ResizePlan& P = E.plan;
         const size_t nx = P.xofs.size(), ny = P.yofs.size();  // ny = 2 * dst_h
         const size_t bytes = nx * 4 + ny * 4 + nx * 2 * 2 + ny * 2 + 64;
@@ -377,6 +383,9 @@ int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, i
                           double* scale_row_host, void* stream) {
     if (!h || !bgr_host || !out_nchw_dev) return -1;
     cudaSetDevice(h->device);
+    smapb_handle::PreEntry* E = nullptr;
+    int rc = pre_entry(h, img_h, img_w, &E);  // refuse the geometry before staging its pixels
+    if (rc) return rc;
     const size_t bytes = (size_t)img_h * img_w * 3;
     if (bytes > h->pre_stage_bytes) {
         cudaDeviceSynchronize();
@@ -411,9 +420,8 @@ int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, c
 // host-only introspection of the resampling plan (tests compare it with the oracle over many geometries without a GPU)
 int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dims6, double* scale, int* xofs, short* xcoef,
                             int* yofs, short* ycoef) {
-    if (src_w < 2 || src_h < 2 || net_w < 1 || net_h < 1 || !dims6) return -1;
     ResizePlan P;
-    make_resize_plan(src_w, src_h, net_w, net_h, &P);
+    if (!dims6 || !make_resize_plan(src_w, src_h, net_w, net_h, &P)) return -1;
     dims6[0] = P.dst_w, dims6[1] = P.dst_h, dims6[2] = P.pad_l, dims6[3] = P.pad_t, dims6[4] = P.mode, dims6[5] = 0;
     if (scale) *scale = P.scale;
     if (xofs) memcpy(xofs, P.xofs.data(), P.xofs.size() * sizeof(int));

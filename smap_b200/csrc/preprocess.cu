@@ -4,7 +4,8 @@
 // cv2's 8-bit bilinear resize is fixed point (OpenCV modules/imgproc/src/resize.cpp): float32 weights rounded (half to
 // even) to multiples of 1/2048, 32-bit horizontal sums, vertical pass
 //   (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2
-// and an exact 1/2 scale is rerouted to INTER_AREA (rounded mean of 2x2 blocks).  The tables are built on the host with the
+// and an exact 1/2 scale is rerouted to INTER_AREA (rounded mean of 2x2 blocks, or of the pixels inside a block cut by an
+// odd last column or row).  The tables are built on the host with the
 // same float/double operations (make_resize_plan); the kernel does the integer arithmetic and the normalisation with
 // IEEE division, one thread per output pixel (3 channels), fully coalesced fp32 stores.  HBM-bound: reads the source
 // image once (through L1/L2, each source pixel is touched by <= 2x2 output pixels when down-scaling), writes 5.1 MB.
@@ -16,13 +17,15 @@ namespace smapb {
 
 static inline int cv_round(double v) { return (int)lrint(v); }  // round half to even (default rounding mode)
 
-void make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* P) {
+bool make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* P) {
+    if (src_w < 1 || src_h < 1 || src_w > 16384 || src_h > 16384 || net_w < 1 || net_h < 1) return false;
     P->src_w = src_w;
     P->src_h = src_h;
     const double s = fmin((double)net_w / src_w, (double)net_h / src_h);  // custom_dataset.py:46
     P->scale = s;
     P->dst_w = cv_round(src_w * s);  // cv::resize: dsize = Size(saturate_cast<int>(ssize.width * fx), ...)
     P->dst_h = cv_round(src_h * s);
+    if (P->dst_w == 0 || P->dst_h == 0) return false;  // cv::resize asserts !dsize.empty(): e.g. 16x16384 -> rint(0.5) = 0
     P->pad_l = P->pad_t = 0;
     if (P->dst_w < net_w) P->pad_l = (net_w - P->dst_w) / 2;       // custom_dataset.py:55-60
     else if (P->dst_h < net_h) P->pad_t = (net_h - P->dst_h) / 2;  // custom_dataset.py:61-66
@@ -38,7 +41,7 @@ void make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* P)
     P->xcoef.assign((size_t)P->dst_w * 2, 0);
     P->yofs.assign((size_t)P->dst_h * 2, 0);
     P->ycoef.assign((size_t)P->dst_h * 2, 0);
-    if (P->mode != 0) return;
+    if (P->mode != 0) return true;
     for (int d = 0; d < P->dst_w; d++) {
         float f = (float)((d + 0.5) * inv - 0.5);
         int sx = (int)floorf(f);
@@ -58,6 +61,7 @@ void make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* P)
         P->ycoef[2 * d] = (short)lrintf((1.f - f) * 2048.f);
         P->ycoef[2 * d + 1] = (short)lrintf(f * 2048.f);
     }
+    return true;
 }
 
 __global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restrict__ src, int src_w, int src_h, int dst_w,
@@ -72,10 +76,21 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restri
             const uint8_t* p = src + ((size_t)dy * src_w + dx) * 3;
             v[0] = p[0], v[1] = p[1], v[2] = p[2];
         } else if (mode == 1) {
+            const int nx = min(2, src_w - 2 * dx), ny = min(2, src_h - 2 * dy);  // 1 where rint(src / 2) rounded up
             const uint8_t* p = src + ((size_t)(2 * dy) * src_w + 2 * dx) * 3;
             const uint8_t* q = p + (size_t)src_w * 3;
+            if (nx == 2 && ny == 2) {
 #pragma unroll
-            for (int c = 0; c < 3; c++) v[c] = ((int)p[c] + (int)p[3 + c] + (int)q[c] + (int)q[3 + c] + 2) >> 2;
+                for (int c = 0; c < 3; c++) v[c] = ((int)p[c] + (int)p[3 + c] + (int)q[c] + (int)q[3 + c] + 2) >> 2;
+            } else {  // window cut by the last column / row: cv2's saturate_cast<uchar>((float)sum / count), half to even
+#pragma unroll
+                for (int c = 0; c < 3; c++) {
+                    int sum = p[c];
+                    if (nx == 2) sum += p[3 + c];
+                    if (ny == 2) sum += q[c];
+                    v[c] = __float2int_rn(__fdiv_rn((float)sum, (float)(nx * ny)));
+                }
+            }
         } else {
             const int sx = tab.xofs[dx];
             const int sx1 = min(sx + 1, src_w - 1);

@@ -18,8 +18,9 @@ struct ResizePlan {
     std::vector<short> xcoef, ycoef;                 // [dst_w][2], [dst_h][2]  (weights * 2048, rounded half to even)
 };
 
-// fills `plan` for a src_w x src_h image going into a net_w x net_h input
-void make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* plan);
+// fills `plan` for a src_w x src_h image going into a net_w x net_h input; false (plan unusable) for sides outside
+// [1, 16384] and where cv2.resize refuses the image: a resized side that rounds to 0 pixels
+bool make_resize_plan(int src_w, int src_h, int net_w, int net_h, ResizePlan* plan);
 
 struct ResizeTablesDev {
     const int* xofs;

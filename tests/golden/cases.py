@@ -58,6 +58,90 @@ def preprocess_case_image(ci):
     return np.clip(np.rint(img), 0, 255).astype(np.uint8)
 
 
+# Network input sizes (net_w, net_h) the resize sweep runs at: the default, config 5, and the edge sizes of the plan
+# tests (levels one row high, one column wide, the smallest tiled input).
+RESIZE_NETS = [(832, 512), (1024, 1024), (96, 64), (992, 32), (32, 1024)]
+RESIZE_KINDS = ("noise", "check", "flat")
+
+
+def resize_geoms(net_w=832, net_h=512, n_random=None, seed=21):
+    """Source geometries (W, H) that reach every regime of cv2.resize(img, (0,0), fx=s, fy=s), s = min(net_w/W, net_h/H),
+    for a net_w x net_h input.  Includes geometries cv2 refuses (a resized side rounds to 0).
+      * exact 1/2 scale with every parity of W mod 4 (H = 2 net_h) and of H mod 4 (W = 2 net_w): rint(W / 2) rounds up
+        at W = 3 (mod 4), so the last column's 2x2 INTER_AREA window is cut by the image edge (likewise rows);
+      * identity (s = 1 with nothing to resize) and near-identity;
+      * up-scaling from 1-, 2- and few-pixel images;
+      * extreme aspect ratios: a side resized to one pixel, or to rint(0.5) = 0 (refused);
+      * exact 1/3 and 1/4 scales;
+      * seeded random sizes (n_random; default: enough for more than 256 accepted geometries at 832x512, past the
+        library's per-handle plan cache)."""
+    hw, hh = 2 * net_w, 2 * net_h
+
+    def sides(n):  # runs of 4 or more consecutive sides (every residue mod 4) at the small, middle and top end
+        return sorted(set(range(2, 18)) | set(range(n // 2 - 2, n // 2 + 2)) | set(range(3 * n // 4 - 2, 3 * n // 4 + 2))
+                      | set(range(n - 7, n + 1)))
+
+    g = [(w, hh) for w in sides(hw)] + [(hw, h) for h in sides(hh)]
+    if (net_w, net_h) == (832, 512):  # odd crops of a 1024-high photo (last column cut), and neighbours just off 1/2 scale
+        g += [(767, 1024), (1363, 1024), (1663, 1023), (1665, 1024), (1664, 1025)]
+    g += [(net_w, net_h), (net_w - 1, net_h), (net_w + 1, net_h + 1), (net_w - 1, net_h - 1)]
+    g += [(1, 1), (1, 2), (2, 1), (2, 2), (5, 7), (17, 9), (1, 300), (5, 1), (net_w, 1), (1, net_h)]
+    g += [(16384, 16), (17, 16384), (16, 16384), (16384, 9), (2, 16384), (1, hh), (5000, 40), (40, 5000)]
+    g += [(3 * net_w, 3 * net_h), (3 * net_w, 3 * net_h - 1), (3 * net_w - 1, 3 * net_h), (4 * net_w, 4 * net_h),
+          (4 * net_w + 1, 4 * net_h), (4 * net_w, 4 * net_h - 3), (3 * net_w + 2, 2 * net_h + 1)]
+    g = [(w, h) for (w, h) in dict.fromkeys(g) if 1 <= w <= 16384 and 1 <= h <= 16384]
+    if n_random is None:
+        n_random = max(0, 280 - len(g))
+    rng = np.random.default_rng(seed)
+    while n_random > 0:
+        w, h = int(rng.integers(1, 2600)), int(rng.integers(1, 2000))
+        if (w, h) not in g:
+            g.append((w, h))
+            n_random -= 1
+    return g
+
+
+def resize_refused(W, H, net_w=832, net_h=512):
+    """cv2.resize raises !dsize.empty() where a resized side rounds (half to even) to 0."""
+    s = min(net_w / W, net_h / H)
+    return int(np.rint(W * s)) == 0 or int(np.rint(H * s)) == 0
+
+
+def resize_image(kind, W, H, seed):
+    """uint8 BGR [H,W,3]: full-range noise (odd 2x2 and 1x2 sums, so round-half-to-even occurs), a 0/255 checkerboard
+    (neighbours differ by the whole range) or flat 255 (the saturation edge)."""
+    if kind == "noise":
+        return np.random.default_rng(seed).integers(0, 256, (H, W, 3), dtype=np.uint8)
+    if kind == "check":
+        c = ((np.add.outer(np.arange(H), np.arange(W)) % 2) * 255).astype(np.uint8)
+        return np.stack([c, 255 - c, c], 2)
+    return np.full((H, W, 3), 255, np.uint8)
+
+
+def cv2_preprocess(img, net_w=832, net_h=512):
+    """The reference loader with cv2 itself (dataset/custom_dataset.py:42-68, 23-24; exps/stage3_root2/test.py:99-103):
+    cv2.resize(img, (0,0), fx=s, fy=s), gray-128 letterbox to net_w x net_h, ToTensor + Normalize in float32.
+    -> (float32 [3, net_h, net_w], scale dict).  Raises cv2.error where cv2 refuses the size."""
+    import cv2
+
+    H, W = img.shape[:2]
+    s = min(net_w / W, net_h / H)
+    r = cv2.resize(img, (0, 0), fx=s, fy=s)
+    h, w = r.shape[:2]
+    out = np.full((net_h, net_w, 3), 128, np.uint8)
+    if w < net_w:
+        assert h == net_h
+        out[:, (net_w - w) // 2:(net_w - w) // 2 + w] = r
+    else:
+        assert w == net_w and h <= net_h
+        out[(net_h - h) // 2:(net_h - h) // 2 + h] = r
+    x = out.astype(np.float32) / np.float32(255)
+    x = (x - np.array([0.406, 0.456, 0.485], np.float32)) / np.array([0.225, 0.224, 0.229], np.float32)  # BGR, config.py:34-35
+    scale = {"scale": s, "img_width": W, "img_height": H, "net_width": net_w, "net_height": net_h,
+             "f_x": W, "f_y": W, "cx": W / 2, "cy": H / 2}
+    return np.ascontiguousarray(x.transpose(2, 0, 1)), scale
+
+
 N_GT_CASES = 12
 
 

@@ -126,6 +126,17 @@ def large_frames(seed=9):
     return out
 
 
+def resize_edge_files(seed=12):
+    """Files whose frames hit the resizer's edges at an 832x512 input: the 1x1, 7x5 and 17x9 (w x h) corpus files
+    (up-scaling from 1-pixel sides), a 1663x1024 frame (exact 1/2 scale, last column cut) and an EXIF-6 file stored
+    1023x1664 whose displayed frame is 1664x1023 (last row cut)."""
+    rng = np.random.default_rng(seed)
+    out = [(n, b) for n, b in corpus() if n.split("_")[0] in ("1x1", "7x5", "17x9")]
+    out.append(("1663x1024_noise_q90_420", cv2_jpeg(content("noise", 1024, 1663, rng), 90, "420")))
+    out.append(("exif6_1664x1023_q90_420", pil_jpeg(content("noise", 1664, 1023, rng), 90, 2, 6)))
+    return out
+
+
 def not_decoded(seed=6):
     """-> list of (name, bytes) the decoder must leave to cv2: progressive, CMYK, 4:1:1, PNG, RGB (Adobe transform 0)."""
     import cv2

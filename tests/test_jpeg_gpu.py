@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from jpeg_corpus import corpus, damaged, large_frames, not_decoded
+from jpeg_corpus import corpus, damaged, large_frames, not_decoded, resize_edge_files
 
 pytestmark = pytest.mark.gpu
 cv2 = pytest.importorskip("cv2")
@@ -120,6 +120,49 @@ def test_run_inference_decodes_jpegs_on_the_gpu(tmp_path, monkeypatch):
     assert len(decoded) == 4  # a caller's imread is used for every file
     assert open(got, "rb").read() == open(ref, "rb").read()
     assert os.path.getsize(got) > 0
+
+
+def test_decoded_frames_at_the_resizer_edges_preprocess_like_cv2(eng):
+    """decode_jpeg -> preprocess on the GPU equals cv2.imdecode -> cv2.resize + letterbox + normalise (cases.cv2_preprocess)
+    on 1x1, 7x5 and 17x9 files (up-scaling from 1-pixel sides), a 1663x1024 file and an EXIF-6 file displayed 1664x1023
+    (exact 1/2 scale with the last column or row cut)."""
+    from cases import cv2_preprocess
+
+    from smap_b200.engine import scale_row
+
+    files = resize_edge_files()
+    shapes = set()
+    for (name, b), g in zip(files, eng.decode_jpeg([b for _, b in files])):
+        ref = cv2_read(b)
+        assert g is not None and np.array_equal(g.cpu().numpy(), ref), name
+        shapes.add(ref.shape[:2])
+        out, scales = eng.preprocess([g])
+        want, sc = cv2_preprocess(ref)
+        got = out[0].cpu().numpy()
+        assert np.array_equal(got, want), (name, "%d values differ" % (got != want).sum())
+        assert np.array_equal(scales[0].numpy(), scale_row(sc)), name
+    assert {(1, 1), (5, 7), (9, 17), (1024, 1663), (1023, 1664)} <= shapes
+
+
+def test_run_inference_takes_frames_at_the_resizer_edges(tmp_path, monkeypatch):
+    """A directory of 1x1, 7x5, 17x9, 1663x1024 and EXIF-6 1664x1023 JPEGs: every file is decoded on the GPU and
+    processed, and the result file equals the one cv2 decoding writes."""
+    from smap_b200 import schema
+    from smap_b200.run_inference import run
+
+    monkeypatch.setenv("SMAPB_NO_AUTOTUNE", "1")  # two handles must choose the same tile shapes for a byte comparison
+    keep = ("1x1_noise_q90_420", "7x5_check_q90_444", "17x9_noise_q50_gray", "1663x1024_noise_q90_420", "exif6_1664x1023_q90_420")
+    data = tmp_path / "imgs"
+    data.mkdir()
+    for name, b in resize_edge_files():
+        if name in keep:
+            (data / (name + ".jpg")).write_bytes(b)
+    assert len(list(data.iterdir())) == len(keep)
+    sd = schema.make_state_dict(0, "identity")
+    got, ref = tmp_path / "gpu.json", tmp_path / "cv2.json"
+    assert run(sd, str(data), str(got), batch_size=3) == len(keep)
+    assert run(sd, str(data), str(ref), batch_size=3, imread=lambda p: cv2.imread(p, cv2.IMREAD_COLOR)) == len(keep)
+    assert open(got, "rb").read() == open(ref, "rb").read()
 
 
 def open_progressive(img):
