@@ -865,6 +865,8 @@ int smapb_comm_create(smapb_handle* h, const void* id128, int rank, int world) {
     if (!h || !id128) return -1;
     NcclApi& a = nccl_api();
     if (!a.lib) return fail(h, -51, a.err.empty() ? "NCCL unavailable" : a.err);
+    // refused here, before NCCL sees them: ncclCommInitRank would otherwise be the one to judge rank and world
+    if (world < 1 || rank < 0 || rank >= world) return fail(h, -1, "communicator: rank / world out of range");
     cudaSetDevice(h->device);
     NcclUid id;
     memcpy(&id, id128, 128);
