@@ -278,13 +278,27 @@ int smapb_set_tile_table(const char* text);
 int smapb_get_tile_table(char* buf, int cap);
 /* conv plan: number of tensor-core conv launches per forward and their algorithmic FLOPs (2*MACs, 1x) */
 int smapb_plan_info(const smapb_handle* h, int B, int* n_conv_launches, double* conv_flops);
-/* Run one standalone convolution through the tensor-core path (test/bench hook).
- * x: fp32 NHWC [B,H,W,Cin]; w: fp32 [Cout,Cin,k,k]; bias fp32 [Cout]; res (optional) fp32 NHWC of the
- * output shape added before the ReLU; post1/post2 (optional) fp32 NHWC added after the ReLU (in that order);
- * y: fp32 NHWC [B,Ho,Wo,Cout].  All device pointers. */
+/* Run one standalone convolution through the tensor-core path (test/bench hook), with every epilogue form the plan uses.
+ * x: fp32 NHWC [B,H,W,Cin]; w: fp32 [Cout,Cin+Cin2,k,k]; bias fp32 [Cout]; padding k/2, Ho = (H + 2 (k/2) - k) / stride + 1
+ * (likewise Wo).  Optional inputs (NULL = absent), converted to the precision's planes as the plan's activations are:
+ *   res        fp32 NHWC [B,Ho,Wo,Cout] added before the ReLU;
+ *   post1/2    fp32 NHWC [B,Ho,Wo,Cout] added after the ReLU, in that order (post2 needs post1);
+ *   in2        fp32 NHWC [B,H2,W2,Cin2], the K-concatenated second input of a fused pair: its 1x1 conv with stride stride2
+ *              (weight columns Cin .. Cin+Cin2-1) joins the same accumulation; needs k = 1, stride = 1, Cin2 % 64 == 0 and
+ *              (H2-1)/stride2 + 1 == Ho, (W2-1)/stride2 + 1 == Wo.  Cin2 = 0 without it;
+ *   up         fp32 NHWC [B,Ho/2,Wo/2,Cout], up-sampled x2 (bilinear, align_corners=True) and added before the ReLU; not
+ *              with res or post1.
+ * res, post1, post2 and up need Cout % 32 == 0.  out_f32 != 0: the conv stores fp32, as the plan's head convs do, instead
+ * of the precision's activation planes.  y: fp32 NHWC [B,Ho,Wo,Cout], the stored output's value.  launch (optional,
+ * int[4]) receives what the result launch ran: BLOCK_N, the patch width tw (128 in the flat mode), 1 for the flat mode
+ * (1x1 stride-1 convs see N*Ho*Wo pixels as one row) or 0 for patch tiles, and the epilogue-input ring (0 none,
+ * 1 residual / skips, 2 up-residual).  All tensors are device pointers.  A combination the plan's conv set-up refuses is
+ * refused here with its error message (smapb_last_error). */
 int smapb_conv_test(smapb_handle* h, const float* x_dev, const float* w_dev, const float* bias_dev,
-                    const float* res_dev, const float* post1_dev, const float* post2_dev, int B, int H, int W, int Cin,
-                    int Cout, int k, int stride, int relu, int precision, float* y_dev, float* ms_out, void* stream);
+                    const float* res_dev, const float* post1_dev, const float* post2_dev, const float* in2_dev,
+                    const float* up_dev, int B, int H, int W, int Cin, int Cout, int k, int stride, int H2, int W2,
+                    int Cin2, int stride2, int relu, int out_f32, int precision, float* y_dev, int* launch, float* ms_out,
+                    void* stream);
 
 #ifdef __cplusplus
 }

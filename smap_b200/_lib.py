@@ -69,8 +69,8 @@ def load():
     lib.smapb_profile_begin.argtypes = [vp]
     lib.smapb_profile_end.argtypes = [vp, c.POINTER(c.c_double), c.POINTER(i32), c.c_char_p]
     lib.smapb_plan_info.argtypes = [vp, i32, c.POINTER(i32), c.POINTER(c.c_double)]
-    lib.smapb_conv_test.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp,
-                                    c.POINTER(c.c_float), vp]
+    lib.smapb_conv_test.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp] + [i32] * 14 + [vp, c.POINTER(i32),
+                                                                                       c.POINTER(c.c_float), vp]
     lib.smapb_refine_load_weight.argtypes = [vp, c.c_char_p, vp, c.POINTER(i64), i32]
     lib.smapb_refine_finalize.argtypes = [vp]
     lib.smapb_refine_mlp.argtypes = [vp, vp, i32, vp, vp]

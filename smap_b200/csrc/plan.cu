@@ -140,11 +140,15 @@ cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t s
     cfg.numAttrs = na;
     return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING, E>, cp);
 }
+// The RING variant a conv runs: 2 = fused bilinear residual, 1 = residual / skip tensors, 0 = no epilogue inputs
+int conv_ring(const ConvParams& cp) { return cp.up_mode ? 2 : (cp.has_res + cp.n_post) ? 1 : 0; }
 template <int BN, int NT, class E = ElemBF16>
 cudaError_t launch_conv_inst(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
-    if (cp.up_mode) return launch_conv_inst2<BN, NT, 2, E>(cp, sm_count, st, pdl);  // fused bilinear residual
-    return (cp.has_res + cp.n_post) ? launch_conv_inst2<BN, NT, 1, E>(cp, sm_count, st, pdl)
-                                    : launch_conv_inst2<BN, NT, 0, E>(cp, sm_count, st, pdl);
+    switch (conv_ring(cp)) {
+        case 2: return launch_conv_inst2<BN, NT, 2, E>(cp, sm_count, st, pdl);
+        case 1: return launch_conv_inst2<BN, NT, 1, E>(cp, sm_count, st, pdl);
+        default: return launch_conv_inst2<BN, NT, 0, E>(cp, sm_count, st, pdl);
+    }
 }
 cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, bool f16, int sm_count, cudaStream_t st, bool pdl) {
 #define SMAPB_CASE(BN)                                                                  \
@@ -223,6 +227,7 @@ int setup_conv(smapb_handle* h, const ConvLayer& L, const ConvIO& io, int block_
     if (L.Cin % 64 != 0) return fail(h, -30, "conv " + L.name + ": Cin must be a multiple of 64");
     memset(cp, 0, sizeof(*cp));
     if ((L.Cin2 != 0) != (in2 != nullptr)) return fail(h, -30, "conv " + L.name + ": second input mismatch");
+    if (L.Cin2 % 64 != 0) return fail(h, -30, "conv " + L.name + ": Cin2 must be a multiple of 64");
     if (in2 && (in2->C != L.Cin2 || L.k != 1 || L.stride != 1)) return fail(h, -30, "conv " + L.name + ": bad fused pair");
     if (up && (res || post1)) return fail(h, -30, "conv " + L.name + ": up-residual excludes other epilogue inputs");
     const bool flat = is_flat(L, io);
@@ -1228,20 +1233,28 @@ __global__ void split_to_f32_kernel(const __nv_bfloat16* __restrict__ in, long l
 }
 
 int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float* bias, const float* res,
-                    const float* post1, const float* post2, int B, int H, int W, int Cin, int Cout, int k, int stride,
-                    int relu, int precision, float* y, float* ms_out, void* stream) {
+                    const float* post1, const float* post2, const float* in2_src, const float* up_src, int B, int H, int W,
+                    int Cin, int Cout, int k, int stride, int H2, int W2, int Cin2, int stride2, int relu, int out_f32,
+                    int precision, float* y, int* launch, float* ms_out, void* stream) {
     if (!h) return -1;
     cudaSetDevice(h->device);
     cudaStream_t st = (cudaStream_t)stream;
     if (!precision_ok(precision)) return fail(h, -1, "smapb_conv_test: unknown precision");
+    if (B < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || k < 1 || stride < 1 || Cin2 < 0)
+        return fail(h, -1, "smapb_conv_test: bad geometry");
+    const int pad = k / 2;
+    const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
+    if (in2_src && (stride2 < 1 || H2 < 1 || W2 < 1 || (H2 - 1) / stride2 + 1 != Ho || (W2 - 1) / stride2 + 1 != Wo))
+        return fail(h, -1, "smapb_conv_test: in2 does not give the output geometry under stride2");
     const int save_terms = h->nterms, save_planes = h->planes;
     const bool save_f16 = h->f16;
     set_precision(h, precision);
     int rc = 0;
     ConvLayer L;
     L.name = "conv_test";
-    L.Cin = Cin, L.Cout = Cout, L.Cout_pad = pad32(Cout), L.k = k, L.stride = stride, L.pad = k / 2;
-    std::vector<float> wh((size_t)Cout * Cin * k * k), bh(Cout);
+    L.Cin = Cin, L.Cout = Cout, L.Cout_pad = pad32(Cout), L.k = k, L.stride = stride, L.pad = pad;
+    L.Cin2 = Cin2, L.stride2 = stride2;
+    std::vector<float> wh((size_t)Cout * (Cin + Cin2) * k * k), bh(Cout);
     std::vector<void*> tmp;
     auto cleanup = [&]() {
         for (void* p : tmp) cudaFree(p);
@@ -1266,35 +1279,54 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         cleanup();
         return rc;
     }
-    const int Ho = (H + 2 * L.pad - k) / stride + 1, Wo = (W + 2 * L.pad - k) / stride + 1;
-    Act in, out;
+    Act in, out, in2, up;
+    ActF32 out32;
     in.N = B, in.H = H, in.W = W, in.C = Cin;
     out.N = B, out.H = Ho, out.W = Wo, out.C = L.Cout_pad;
+    in2.N = B, in2.H = H2, in2.W = W2, in2.C = Cin2;
+    up.N = B, up.H = Ho / 2, up.W = Wo / 2, up.C = Cout;
+    out32.N = B, out32.H = Ho, out32.W = Wo, out32.C = L.Cout_pad;
     ConvIO io{&in, relu};
-    io.out = &out;
     void* p = nullptr;
-    CKT(cudaMalloc(&p, (size_t)in.plane() * 2 * h->planes));
-    tmp.push_back(p);
-    in.ptr = (__nv_bfloat16*)p;
-    CKT(cudaMalloc(&p, (size_t)out.plane() * 2 * h->planes));
-    tmp.push_back(p);
-    out.ptr = (__nv_bfloat16*)p;
-    CKT(cudaMemset(p, 0, (size_t)out.plane() * 2 * h->planes));  // TMA stores are invisible to initcheck
-    CKT(launch_f32_to_split(x, in.ptr, in.plane(), in.plane(), h->planes, st, h->f16));
-    const float* extra_src[3] = {res, post1, post2};
-    Act extra_act[3] = {out, out, out};
-    const Act** extra_role[3] = {&io.res, &io.post1, &io.post2};
-    for (int e = 0; e < 3; e++) {
+    // the operands in the precision's activation planes, converted as the plan converts fp32 tensors (an empty tensor,
+    // an in2 with Cin2 = 0 or an up of a 1-pixel output, is left unallocated: setup_conv refuses it)
+    auto planes_of = [&](const float* src, Act& a) -> cudaError_t {
+        if (a.plane() == 0) return cudaSuccess;
+        cudaError_t e = cudaMalloc(&p, (size_t)a.plane() * 2 * h->planes);
+        if (e != cudaSuccess) return e;
+        tmp.push_back(p);
+        a.ptr = (__nv_bfloat16*)p;
+        return launch_f32_to_split(src, a.ptr, a.plane(), a.plane(), h->planes, st, h->f16);
+    };
+    CKT(planes_of(x, in));
+    if (out_f32) {
+        CKT(cudaMalloc(&p, (size_t)out.plane() * 4));
+        tmp.push_back(p);
+        out32.ptr = (float*)p;
+        CKT(cudaMemset(p, 0, (size_t)out.plane() * 4));
+        io.out_f32 = &out32;
+    } else {
+        CKT(cudaMalloc(&p, (size_t)out.plane() * 2 * h->planes));
+        tmp.push_back(p);
+        out.ptr = (__nv_bfloat16*)p;
+        CKT(cudaMemset(p, 0, (size_t)out.plane() * 2 * h->planes));  // TMA stores are invisible to initcheck
+        io.out = &out;
+    }
+    if (in2_src) {
+        CKT(planes_of(in2_src, in2));
+        io.in2 = &in2;
+    }
+    const float* extra_src[4] = {res, post1, post2, up_src};
+    Act extra_act[4] = {out, out, out, up};
+    const Act** extra_role[4] = {&io.res, &io.post1, &io.post2, &io.up};
+    for (int e = 0; e < 4; e++) {
         if (!extra_src[e]) continue;
         if (L.Cout_pad != Cout) {
             cleanup();
-            return fail(h, -1, "conv_test: residual/post operands require Cout % 32 == 0");
+            return fail(h, -1, "conv_test: residual/post/up operands require Cout % 32 == 0");
         }
-        CKT(cudaMalloc(&p, (size_t)out.plane() * 2 * h->planes));
-        tmp.push_back(p);
-        extra_act[e].ptr = (__nv_bfloat16*)p;
+        CKT(planes_of(extra_src[e], extra_act[e]));
         *extra_role[e] = &extra_act[e];
-        CKT(launch_f32_to_split(extra_src[e], extra_act[e].ptr, out.plane(), out.plane(), h->planes, st, h->f16));
     }
     ConvParams cp;
     int bn = 0;
@@ -1303,6 +1335,12 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     if (rc) {
         cleanup();
         return rc;
+    }
+    if (launch) {
+        launch[0] = bn;
+        launch[1] = 1 << cp.tw_log2;
+        launch[2] = is_flat(L, io) ? 1 : 0;
+        launch[3] = conv_ring(cp);
     }
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
@@ -1353,13 +1391,15 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));
     cudaEventRecord(e1, st);
     h->launches += 1 + reps;
-    // de-pad + convert
-    float* ytmp = nullptr;
-    CKT(cudaMalloc((void**)&ytmp, (size_t)out.plane() * 4));
-    tmp.push_back(ytmp);
-    split_to_f32_kernel<<<(unsigned)((out.plane() + 255) / 256), 256, 0, st>>>(out.ptr, out.plane(), h->planes, ytmp,
-                                                                               out.plane(), h->f16);
-    CKT(cudaGetLastError());
+    // convert (split outputs) + de-pad
+    float* ytmp = out32.ptr;
+    if (!out_f32) {
+        CKT(cudaMalloc((void**)&ytmp, (size_t)out.plane() * 4));
+        tmp.push_back(ytmp);
+        split_to_f32_kernel<<<(unsigned)((out.plane() + 255) / 256), 256, 0, st>>>(out.ptr, out.plane(), h->planes, ytmp,
+                                                                                   out.plane(), h->f16);
+        CKT(cudaGetLastError());
+    }
     CKT(cudaMemcpy2DAsync(y, (size_t)Cout * 4, ytmp, (size_t)L.Cout_pad * 4, (size_t)Cout * 4, (size_t)B * Ho * Wo,
                           cudaMemcpyDeviceToDevice, st));
     CKT(cudaStreamSynchronize(st));

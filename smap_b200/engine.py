@@ -420,20 +420,26 @@ class Engine:
         return n.value, f.value
 
     def conv_test(self, x, w, bias, res=None, stride=1, relu=True, precision="bf16x3", time_it=False, post1=None,
-                  post2=None):
-        """x fp32 NHWC cuda; w [Cout,Cin,k,k]; returns y fp32 NHWC (and ms)."""
+                  post2=None, in2=None, stride2=1, up=None, out_f32=False, launch=None):
+        """One convolution through the tensor-core path (smapb_conv_test).  x fp32 NHWC cuda [B,H,W,Cin]; w
+        [Cout,Cin+Cin2,k,k], Cin2 the channels of in2 (fp32 NHWC, the K-concatenated 1x1 input of a fused pair, with
+        stride2); up fp32 NHWC at half the output size (fused bilinear residual); out_f32: fp32 output as the head convs
+        store it.  launch: a dict that receives block_n, tw, flat and ring of the launch.  Returns y fp32 NHWC (and ms)."""
         B, H, W, Cin = x.shape
         Cout, _, k, _ = w.shape
+        H2, W2, Cin2 = in2.shape[1:] if in2 is not None else (0, 0, 0)
         pad = k // 2
         Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
         y = torch.empty(B, Ho, Wo, Cout, device=x.device)
         ms = ctypes.c_float(0)
-        self._check(self.lib.smapb_conv_test(self._h, _ptr(x.contiguous()), _ptr(w.contiguous()), _ptr(bias.contiguous()),
-                                             _ptr(res.contiguous() if res is not None else None),
-                                             _ptr(post1.contiguous() if post1 is not None else None),
-                                             _ptr(post2.contiguous() if post2 is not None else None), B, H, W, Cin, Cout, k,
-                                             stride, int(relu), PRECISIONS[precision], _ptr(y),
-                                             ctypes.byref(ms) if time_it else None, _stream()), "smapb_conv_test")
+        ran = (ctypes.c_int * 4)()
+        args = [t.contiguous() if t is not None else None for t in (x, w, bias, res, post1, post2, in2, up)]
+        self._check(self.lib.smapb_conv_test(self._h, *[_ptr(t) for t in args], B, H, W, Cin, Cout, k, stride, H2, W2,
+                                             Cin2, stride2, int(relu), int(out_f32),
+                                             PRECISIONS[precision], _ptr(y), ran, ctypes.byref(ms) if time_it else None,
+                                             _stream()), "smapb_conv_test")
+        if launch is not None:
+            launch.update(block_n=ran[0], tw=ran[1], flat=bool(ran[2]), ring=ran[3])
         return (y, ms.value) if time_it else y
 
 

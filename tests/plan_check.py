@@ -1,7 +1,8 @@
 """The per-op checker of the backbone plan, one for every precision (bf16x3, bf16, fp16), and what the GPU tests around
 it share: plan introspection (smapb_debug_checksums, smapb_debug_dump), float64 references of one layer fed the exact
-inputs the op consumed, the op loop check_ops, plan switches that must not change a bit, and the conv cases of
-tests/test_conv_gpu.py and tests/test_fp16_gpu.py.
+inputs the op consumed, the op loop check_ops, plan switches that must not change a bit, and the single-conv checker
+(conv_op, check_conv: a conv_test call described as a plan op and judged by the same judge()) of
+tests/test_conv_gpu.py, tests/test_fp16_gpu.py and tests/test_conv_edges_gpu.py.
 
 The reference r of an op is computed in fp64 from the operands the device holds (folded as the library folds them), so
 what separates the device from it is fp32 arithmetic: every element must lie within its precision's output rounding
@@ -11,7 +12,8 @@ terms (_acc_bound):
     `-s` also prints the per-channel error against it and against the float64 layer of the unfolded state dict;
   * bf16: 1 ulp_bf16(r), bf16 weights;
   * fp16: 1/2 ulp_fp16(y) against clamp(r) to +-65504 (the store's clamp; on in-range data clamp(r) == r), fp16
-    weights, and |y| 2^-24 for the fp32 heads.
+    weights;
+  * fp32 outputs (the heads), in every precision: |y| 2^-24.
 Where an op ends in its ReLU and r's pre-activation is below minus its accumulation bound, the output is exactly 0;
 padded channels are exactly 0; the max-pool and the space-to-depth view match bit for bit; the returned heads
 (head_merge, tapsum) are within 1e-5 of max of their recomputation from the dumped fp32 heads.  The wrong references
@@ -149,23 +151,51 @@ class Weights:
             s = g(".bn.weight") / torch.sqrt(g(".bn.running_var") + smap_torch.BN_EPS)
             W = w * s.view(-1, 1, 1, 1)
             bias = (b - g(".bn.running_mean")) * s + g(".bn.bias")
-            lo = None
-            if self.mode != "x3":
-                wf = W.float()
-                if self.mode == "fp16":
-                    W = wf.half().double()
-                else:
-                    hi = wf.bfloat16()
-                    W = hi.double()
-                    if self.mode == "dev3":
-                        lo = (wf - hi.float()).bfloat16().double()
-                        W = W + lo
-                bias = bias.float()
-            self.cache[name] = (W, bias, lo)
+            self.cache[name] = device_form(W, bias, self.mode)
         return self.cache[name]
 
     def bias_sum(self, b1, b2):
         return b1 + b2 if self.mode == "x3" else (b1 + b2).double()  # an fp32 add on the device
+
+
+def device_form(W, bias, mode):
+    """(W, bias, W_lo) of float64 weights W and bias as the device holds them in `mode` (see Weights); W is rounded to fp32
+    first, as upload_conv_layer receives it.  Mode "x3": unchanged, no W_lo."""
+    if mode == "x3":
+        return W, bias, None
+    wf, lo = W.float(), None
+    if mode == "fp16":
+        W = wf.half().double()
+    else:
+        hi = wf.bfloat16()
+        W = hi.double()
+        if mode == "dev3":
+            lo = (wf - hi.float()).bfloat16().double()
+            W = W + lo
+    return W, bias.float(), lo
+
+
+class ConvWeights:
+    """Weights-like source of one conv_test call: its raw fp32 weights w [Cout, Cin + Cin2, k, k] and bias b, in the
+    device's form (device_form; mode "dev3", "bf16" or "fp16").  A K-concatenated pair (op name ending in
+    fused_conv3_downsample) is served as reference() asks for it: "<base>conv_bn_relu3" the first Cin columns with the bias,
+    "<base>downsample" the other Cin2 columns with a zero bias (b + 0 is b in fp32)."""
+
+    def __init__(self, w, b, cin, mode):
+        self.mode, self.cin = mode, cin
+        self.W, self.bias, self.lo = device_form(w.double(), b.double(), mode)
+
+    def unit(self, name):
+        cols = slice(None)
+        bias = self.bias
+        if name.endswith("conv_bn_relu3"):
+            cols = slice(0, self.cin)
+        elif name.endswith("downsample"):
+            cols, bias = slice(self.cin, None), torch.zeros_like(bias)
+        return self.W[:, cols], bias, None if self.lo is None else self.lo[:, cols]
+
+    def bias_sum(self, b1, b2):
+        return (b1 + b2).double()
 
 
 def _nchw(t):
@@ -181,7 +211,7 @@ def _conv(x, W, stride=1, pad=0):
     return _nhwc(F.conv2d(_nchw(x[..., :W.shape[1]]), W, stride=stride, padding=pad))
 
 
-def _coeff(n_in, n_out):
+def _coeff(n_in, n_out, device):
     """Bilinear align_corners=True indices and weights for one axis, computed in fp32 as ATen (and the kernels) do."""
     scale = torch.tensor(float(n_in - 1), dtype=torch.float32) / torch.tensor(float(n_out - 1), dtype=torch.float32) \
         if n_out > 1 else torch.tensor(0.0)
@@ -190,7 +220,7 @@ def _coeff(n_in, n_out):
     i1 = torch.where(i0 < n_in - 1, i0 + 1, i0)
     l1 = src - i0.float()
     l0 = 1 - l1
-    return i0.cuda(), i1.cuda(), l0.double().cuda(), l1.double().cuda()
+    return i0.to(device), i1.to(device), l0.double().to(device), l1.double().to(device)
 
 
 def _up(t, H, W, align_corners=True):
@@ -198,8 +228,8 @@ def _up(t, H, W, align_corners=True):
     model's F.interpolate(align_corners=True); align_corners=False only serves as a deliberately wrong reference."""
     if not align_corners:
         return _nhwc(F.interpolate(_nchw(t), size=(H, W), mode="bilinear", align_corners=False))
-    y0, y1, hy0, hy1 = _coeff(t.shape[1], H)
-    x0, x1, wx0, wx1 = _coeff(t.shape[2], W)
+    y0, y1, hy0, hy1 = _coeff(t.shape[1], H, t.device)
+    x0, x1, wx0, wx1 = _coeff(t.shape[2], W, t.device)
     a, b = t[:, y0], t[:, y1]
     v = lambda u: u[:, :, x0] * wx0.view(1, 1, -1, 1) + u[:, :, x1] * wx1.view(1, 1, -1, 1)  # noqa: E731
     return v(a) * hy0.view(1, -1, 1, 1) + v(b) * hy1.view(1, -1, 1, 1)
@@ -277,14 +307,26 @@ def reference(op, get, wts, image, mut=None, squares=False, get_lo=None):
         return (pre if squares else F.relu(pre)), pre, True
     assert kind == "conv", "no reference for op kind %r (%s)" % (kind, name)
     stride, pad = int(op["s"]), int(op["pad"].split("x")[0])
+    def last_kb(W, Wlo):  # the weights of the conv's last k-block (tap ky = kh-1, kx = kw-1, last 64 channels) zeroed
+        if mut != "drop_last_kb":
+            return W, Wlo
+        W = W.clone()
+        W[:, -64:, -1, -1] = 0
+        if Wlo is not None:
+            Wlo = Wlo.clone()
+            Wlo[:, -64:, -1, -1] = 0
+        return W, Wlo
+
     if "in2" in op:  # relu(conv3(o2) + downsample(t)) as one K-concatenated GEMM
         base = name[:-len("fused_conv3_downsample")]
         W3, b3, W3lo = unit(base + "conv_bn_relu3")
         Wd, bd, Wdlo = unit(base + "downsample")
+        Wd, Wdlo = last_kb(Wd, Wdlo)  # the second input's k-blocks come last
         shift = (lambda t: torch.roll(t, 1, dims=2)) if mut == "shift_ds" else (lambda t: t)
         pre = cv("in", W3, W3lo) + cv("in2", Wd, Wdlo, xform=shift, stride=int(op["s2"])) + wts.bias_sum(b3, bd)
     else:
         W, b, Wlo = unit(name)
+        W, Wlo = last_kb(W, Wlo)
         pre = cv("in", W, Wlo, stride=stride, pad=pad) + b
     C = pre.shape[-1]
     if "res" in op:
@@ -395,7 +437,7 @@ _MUTATIONS = {  # deliberately wrong reference -> op classes it applies to (larg
     "hi_only": ("largest_k",),      # bf16x3 with the activations' lo plane dropped
     "drop_hi_wlo": ("largest_k",),  # bf16x3 without the a_hi w_lo MMA
     "plain_bf16": ("largest_k",),   # a_hi w_hi only
-}
+}  # and, for single convs only (conv_mutations), "drop_last_kb": without the last k-block (last tap, last 64 channels)
 _X3_ONLY = ("hi_only", "drop_hi_wlo", "plain_bf16")
 
 
@@ -410,6 +452,73 @@ def _changes(rm, r):
     """Whether a wrong reference differs from the right one by more than fp64 rounding (it may not: bilinear
     interpolation from a 1-pixel level is the same with and without align_corners, a bias chunk may equal the next)."""
     return (rm - r).abs().max().item() > 1e-12 * r.abs().max().item()
+
+
+def f32_out(op):
+    """Whether a conv stores fp32 (the heads, or a conv_test call with an fp32 output) rather than activation planes."""
+    return op["kind"] == "conv_f32" or op.get("f32") == "1"
+
+
+def out_rounding(op, precision, yc):
+    """The output-rounding term of an element's bound, as a function of the reference r: fp32 outputs |y| 2^-24 (one
+    fp32 rounding, in every precision); bf16x3 2^-17 |r| (hi + lo carries the fp32 value to 2^-18 relative); bf16 1 ulp
+    of r (<= 1/2 ulp of the fp32 value, <= 1 ulp(r) within a binade of r); fp16 1/2 ulp of the stored y."""
+    if f32_out(op):
+        return lambda r: yc.abs() * 2.0 ** -24
+    if precision == "bf16x3":
+        return lambda r: 2.0 ** -17 * r.abs() * (1 + 2.0 ** -20)
+    if precision == "bf16":
+        return lambda r: _ulp_bf16(r) * (1 + 2.0 ** -20)
+    return lambda r: half_ulp16(yc)
+
+
+def judge(op, y, get, rw, precision, img=None, get_lo=None, muts=()):
+    """One conv-like op's output y (fp64 NHWC, padded channels after the real ones) against the float64 reference of the
+    device's operands (weights rw; inputs get(role, hi_only), lo planes get_lo(role) in bf16x3): every element within
+    out_rounding + _acc_bound, exact zeros where the ReLU must clear, padded channels zero, and in fp16 the store's clamp
+    (clamp_check).  Each wrong reference of muts (keys of _MUTATIONS, or "drop_last_kb") is compared with y by the same
+    bound.
+    -> dict r, pre (the right reference), err (worst |y - r| / bound), share (of the elements outside the bound), bad
+    (violated conditions), over and band (fp16 stores: sure-over and band masks, else None) and tried: wrong reference -> (flagged, share of the elements outside the
+    bound), without those that equal the right reference here (_changes)."""
+    r, pre, relu_last = reference(op, get, rw, img, get_lo=get_lo)
+    q = reference(op, get, rw, img, squares=True)[0].sqrt()
+    yc = y[..., :r.shape[-1]]
+    clamp = precision == "fp16" and not f32_out(op)  # fp16 stores clamp to +-65504; fp32 outputs do not
+    out_round = out_rounding(op, precision, yc)
+
+    def bound(r, pre):
+        return out_round(r) + _acc_bound(op, q, r, pre)
+
+    def dist(r):
+        return (yc - (r.clamp(-FP16_MAX, FP16_MAX) if clamp else r)).abs()
+
+    # exact zeros where the ReLU must clear (pre below minus its own accumulation bound), padded channels
+    bad = x3_error(y, r, pre, relu_last, neg=_acc_bound(op, q, pre))[1]
+    out = {"r": r, "pre": pre, "over": None, "band": None, "tried": {}}
+    if clamp:
+        if not torch.isfinite(y).all():
+            bad.append("non-finite activations")
+        over, in_band, err, more = clamp_check(yc, r, _acc_bound(op, q, r, pre))
+        bad += more
+        out.update(over=over, band=in_band)
+    else:
+        err = (dist(r) / bound(r, pre).clamp(min=1e-30)).max().item()
+        if err > 1.0:
+            bad.append("error %.3g x the bound" % err)
+    out["share"] = (dist(r) > bound(r, pre)).double().mean().item()
+    # the wrong references (host-side only: the same device output)
+    for mut in muts:
+        hi = mut in ("hi_only", "plain_bf16")
+        rm, pm, _ = reference(op, lambda role: get(role, hi), rw, img, mut=mut,
+                              get_lo=None if hi or precision != "bf16x3" else get_lo)
+        if not _changes(rm, r):
+            continue
+        over = dist(rm) > bound(rm, pm)
+        zeros = bool(x3_error(y, rm, pm, relu_last, neg=_acc_bound(op, q, pm))[1])
+        out["tried"][mut] = (bool(over.any()) or zeros, over.double().mean().item())
+    out.update(err=err, bad=bad)
+    return out
 
 
 def check_ops(eng, B, sd, img, outs, precision):
@@ -459,63 +568,29 @@ def check_ops(eng, B, sd, img, outs, precision):
                 bad.append("max-pool not bit-exact")
         else:
             y = value(y_raw)
-            r, pre, relu_last = reference(op, get, wts, img)
+            # the checker must flag deliberately wrong references: those not yet flagged that apply to this op
+            muts = [m for m, mcls in _MUTATIONS.items()
+                    if m not in flagged and not (m in _X3_ONLY and precision != "bf16x3")
+                    and (cls in mcls or (i == largest_k and "largest_k" in mcls))]
+            j = judge(op, y, get, rw, precision, img, get_lo=get_lo, muts=muts)
+            err, r, pre = j["err"], j["r"], j["pre"]
+            bad += j["bad"]
             if precision == "bf16x3":
-                spec = x3_error(y, r, pre, relu_last)[0]
-                r, pre, _ = reference(op, get, rw, img, get_lo=get_lo)
-                dev = x3_error(y, r, pre, relu_last)[0]
+                rs, ps, relu_last = reference(op, get, wts, img)
                 d0, s0 = per_channel.get(cls, (0.0, 0.0))
-                per_channel[cls] = (max(d0, dev), max(s0, spec))
-            q = reference(op, get, rw, img, squares=True)[0].sqrt()
-            yc = y[..., :r.shape[-1]]
-            clamp = fp16 and op["kind"] != "conv_f32"  # fp16 stores clamp to +-65504; the fp32 heads do not
-            if precision == "bf16x3":  # hi + lo carries the fp32 value to 2^-18 relative (2^-17 used)
-                out_round = lambda r: 2.0 ** -17 * r.abs() * (1 + 2.0 ** -20)  # noqa: E731
-            elif precision == "bf16":  # <= 1/2 ulp of the fp32 value, <= 1 ulp(r) within a binade of r
-                out_round = lambda r: _ulp_bf16(r) * (1 + 2.0 ** -20)  # noqa: E731
-            elif clamp:
-                out_round = lambda r: half_ulp16(yc)  # noqa: E731
-            else:
-                out_round = lambda r: yc.abs() * 2.0 ** -24  # noqa: E731
-
-            def bound(r, pre):
-                return out_round(r) + _acc_bound(op, q, r, pre)
-
-            def dist(r):
-                return (yc - (r.clamp(-FP16_MAX, FP16_MAX) if clamp else r)).abs()
-
-            # exact zeros where the ReLU must clear (pre below minus its own accumulation bound), padded channels
-            bad += x3_error(y, r, pre, relu_last, neg=_acc_bound(op, q, pre))[1]
-            if clamp:
-                if not torch.isfinite(y).all():
-                    bad.append("non-finite activations")
-                over, in_band, err, more = clamp_check(yc, r, _acc_bound(op, q, r, pre))
-                bad += more
-                n_over = int(over.sum().item())
-                neg += int((over & (r < 0)).sum().item())
-                band += int(in_band.sum().item())
-            else:
-                err = (dist(r) / bound(r, pre).clamp(min=1e-30)).max().item()
-                if err > 1.0:
-                    bad.append("error %.3g x the bound" % err)
-            # the checker must flag deliberately wrong references (host-side only: the same dumps)
-            for mut, mcls in _MUTATIONS.items():
-                if mut in flagged or (mut in _X3_ONLY and precision != "bf16x3"):
-                    continue
-                if cls not in mcls and not (i == largest_k and "largest_k" in mcls):
-                    continue
-                hi = mut in ("hi_only", "plain_bf16")
-                rm, pm, _ = reference(op, lambda role: get(role, hi), rw, img, mut=mut,
-                                      get_lo=None if hi or precision != "bf16x3" else get_lo)
-                if not _changes(rm, r):
+                per_channel[cls] = (max(d0, x3_error(y, r, pre, relu_last)[0]), max(s0, x3_error(y, rs, ps, relu_last)[0]))
+            if j["over"] is not None:
+                n_over = int(j["over"].sum().item())
+                neg += int((j["over"] & (r < 0)).sum().item())
+                band += int(j["band"].sum().item())
+            for mut in muts:
+                if mut not in j["tried"]:
                     print("  wrong reference %-12s on op %d %s: equals the right one here, tried on a later op"
                           % (mut, i, op["name"]))
                     continue
-                over = dist(rm) > bound(rm, pm)
-                zeros = bool(x3_error(y, rm, pm, relu_last, neg=_acc_bound(op, q, pm))[1])
-                flagged[mut] = bool(over.any()) or zeros
+                flagged[mut], share = j["tried"][mut]
                 print("  wrong reference %-12s on op %d %s (K %d): %.3g of its elements outside the bound"
-                      % (mut, i, op["name"], _K(op), over.double().mean().item()))
+                      % (mut, i, op["name"], _K(op), share))
         if op["kind"] == "conv_f32":
             heads[op["name"]] = y_raw
         if n_over:
@@ -722,15 +797,84 @@ CASES = [
 _TILE_CASES = [(8, 32, 52, 256, 256, 3, 1, False), (8, 32, 52, 1024, 256, 1, 1, False), (2, 16, 26, 512, 512, 3, 2, False),
                (4, 64, 104, 128, 512, 1, 1, True), (2, 128, 208, 256, 64, 1, 1, False)]
 
+CONV_MODES = {"bf16x3": "dev3", "bf16": "bf16", "fp16": "fp16"}  # precision -> the device's weight form (ConvWeights)
 
-def _case_tensors(case, seed=None):
-    """-> (x, w, b, res or None) on the device, for a case of CASES or _TILE_CASES (the first seven fields and, last,
-    whether there is a residual); seeded from the case unless seed is given."""
-    B, H, W, Cin, Cout, k, stride = case[:7]
-    g = torch.Generator(device="cpu").manual_seed(hash(case) % (2 ** 31) if seed is None else seed)
-    x = torch.randn(B, H, W, Cin, generator=g).cuda()
-    w = (torch.randn(Cout, Cin, k, k, generator=g) / (Cin * k * k) ** 0.5).cuda()
-    b = torch.randn(Cout, generator=g).cuda()
-    Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
-    res = torch.randn(B, Ho, Wo, Cout, generator=g).cuda() if case[-1] else None
-    return x, w, b, res
+
+def conv_op(B, H, W, cin, cout, k=1, s=1, relu=True, res=False, posts=0, cin2=0, s2=1, up=False, f32=False):
+    """A conv_test call described as a plan op (kind conv, the fields and roles check_ops reads), so that reference(),
+    _acc_bound and judge() check it as they check the plan's ops.  The input x is [B, H, W, cin], padding k // 2; res,
+    posts (1: p1, 2: p1 and p2) and up add epilogue inputs; cin2 > 0 adds a K-concatenated second input of
+    ((Ho - 1) s2 + 1) x ((Wo - 1) s2 + 1) pixels (the smallest, so odd for s2 = 2) and needs k = s = 1; f32: fp32 output."""
+    p = k // 2
+    Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
+    op = {"name": "conv_test.fused_conv3_downsample" if cin2 else "conv_test", "kind": "conv", "k": "%dx%d" % (k, k),
+          "cin": str(cin), "cin2": str(cin2), "s": str(s), "s2": str(s2), "pad": "%dx%d" % (p, p), "relu": str(int(relu)),
+          "cout": str(cout), "in": "in", "geom": "%dx%dx%d" % (B, H, W), "out": "%dx%dx%dx%d" % (B, Ho, Wo, cout)}
+    for role, on in (("res", res), ("p1", posts >= 1), ("p2", posts >= 2), ("in2", cin2 > 0), ("up", up)):
+        if on:
+            op[role] = role
+    if f32:
+        op["f32"] = "1"
+    return op
+
+
+def legacy_op(case):
+    """conv_op of a case of CASES (B, H, W, Cin, Cout, k, stride, relu, res) or _TILE_CASES (..., stride, res; ReLU)."""
+    B, H, W, cin, cout, k, s = case[:7]
+    return conv_op(B, H, W, cin, cout, k, s, relu=case[7] if len(case) == 9 else True, res=case[-1])
+
+
+def conv_inputs(op, seed, device="cuda"):
+    """fp32 tensors of a conv_op: role -> NHWC tensor (in, and res, p1, p2, in2, up as the op names them), "w" [Cout,
+    Cin + Cin2, k, k] scaled by 1 / sqrt(K) and "b" [Cout]; standard normal otherwise, so every value is in fp16's range."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    B, H, W = (int(v) for v in op["geom"].split("x"))
+    _, Ho, Wo, cout = _dims(op)
+    cin, cin2, k, s2 = int(op["cin"]), int(op["cin2"]), int(op["k"].split("x")[0]), int(op["s2"])
+    shapes = {"in": (B, H, W, cin), "res": (B, Ho, Wo, cout), "p1": (B, Ho, Wo, cout), "p2": (B, Ho, Wo, cout),
+              "in2": (B, (Ho - 1) * s2 + 1, (Wo - 1) * s2 + 1, cin2), "up": (B, Ho // 2, Wo // 2, cout)}
+    t = {r: torch.randn(*shape, generator=g) for r, shape in shapes.items() if r in op}
+    t["w"] = torch.randn(cout, cin + cin2, k, k, generator=g) / _K(op) ** 0.5
+    t["b"] = torch.randn(cout, generator=g)
+    return {r: v.to(device) for r, v in t.items()}
+
+
+def run_conv(eng, op, t, precision, launch=None):
+    """The device output of a conv_op on inputs t (conv_inputs): fp32 NHWC [B, Ho, Wo, Cout]."""
+    return eng.conv_test(t["in"], t["w"], t["b"], res=t.get("res"), stride=int(op["s"]), relu=op["relu"] == "1",
+                         precision=precision, post1=t.get("p1"), post2=t.get("p2"), in2=t.get("in2"), stride2=int(op["s2"]),
+                         up=t.get("up"), out_f32=f32_out(op), launch=launch)
+
+
+def device_planes(t, precision):
+    """[planes, ...] of fp32 tensor t as launch_f32_to_split stores it: bf16 hi (and lo = bf16(t - hi) in bf16x3), or one
+    fp16 plane."""
+    if precision == "fp16":
+        return t.half()[None]
+    hi = t.bfloat16()
+    return torch.stack([hi, (t - hi.float()).bfloat16()]) if precision == "bf16x3" else hi[None]
+
+
+def conv_operands(op, t, precision):
+    """-> (get, get_lo, weights) for reference() and judge(): the fp64 values of t's tensors in the planes
+    launch_f32_to_split makes (device_planes), their lo planes (bf16x3), and the weights in the device's form."""
+    planes = {r: device_planes(v, precision) for r, v in t.items() if r in ROLES}
+    return (lambda role, hi_only=False: value(planes[role], hi_only), lambda role: planes[role][1].double(),
+            ConvWeights(t["w"], t["b"], int(op["cin"]), CONV_MODES[precision]))
+
+
+def check_conv(op, y, t, precision, muts=(), operands=None):
+    """judge() of a conv_test output y (fp32 NHWC, real channels) against the float64 reference of the operands the device
+    held (conv_operands).  operands: the precision whose operand rounding the reference assumes (default `precision`;
+    another one makes a deliberately wrong reference).  -> judge's dict."""
+    get, get_lo, rw = conv_operands(op, t, operands or precision)
+    return judge(op, y.double(), get, rw, precision, get_lo=get_lo, muts=muts)
+
+
+def conv_mutations(op, precision):
+    """The wrong references that apply to a conv_op: the reference without its last k-block, a shifted bias
+    chunk (Cout >= 64), hi-only activations, no a_hi w_lo MMA and plain bf16 products (bf16x3), and the one of its
+    epilogue form (align_false: up; shift_ds: in2; drop_post2: p2)."""
+    muts = ["drop_last_kb"] + (["bias_shift"] if int(op["cout"]) >= 64 else [])
+    muts += list(_X3_ONLY) if precision == "bf16x3" else []
+    return muts + [m for m, role in (("align_false", "up"), ("shift_ds", "in2"), ("drop_post2", "p2")) if role in op]

@@ -1,14 +1,15 @@
-"""GPU: the wgmma implicit-GEMM convolution against a plain PyTorch fp32 reference of the same op
-(TF32 disabled).  Tolerance for the bf16x3 (split-bf16, fp32-faithful) mode: 2e-5 of the output max."""
+"""GPU: the wgmma implicit-GEMM convolution at the network's layer shapes, persistent regime included, against the float64
+reference of the operands the device holds, element by element: check_conv in tests/plan_check.py, the bound the plan's
+ops meet (2^-17 |r| in bf16x3, one bf16 ulp in bf16, plus the accumulation bound; exact zeros where the ReLU clears).
+The edges of the tiling, every kernel instance and every epilogue form are swept in tests/test_conv_edges_gpu.py."""
 import os
 import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from plan_check import CASES, _TILE_CASES, _case_tensors, no_tf32  # noqa: E402
+from plan_check import CASES, _TILE_CASES, check_conv, conv_inputs, conv_op, legacy_op, no_tf32, run_conv  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -23,47 +24,41 @@ def eng():
     e.close()
 
 
+def _assert_checked(op, y, t, precision):
+    j = check_conv(op, y, t, precision)
+    assert not j["bad"], "\n".join(j["bad"])
+    return j["err"]
+
+
 @pytest.mark.parametrize("case", CASES)
 def test_conv_bf16x3_matches_fp32(eng, case):
-    B, H, W, Cin, Cout, k, stride, relu, use_res = case
-    x, w, b, res = _case_tensors(case)
-    ref = F.conv2d(x.permute(0, 3, 1, 2), w, b, stride=stride, padding=k // 2)
-    if use_res:
-        ref = ref + res.permute(0, 3, 1, 2)
-    if relu:
-        ref = F.relu(ref)
-    y = eng.conv_test(x, w, b, res=res, stride=stride, relu=relu)
+    op = legacy_op(case)
+    t = conv_inputs(op, hash(case) % (2 ** 31))
+    y = run_conv(eng, op, t, "bf16x3")
     torch.cuda.synchronize()
-    ref = ref.permute(0, 2, 3, 1)
-    err = (y - ref).abs().max().item() / ref.abs().max().item()
-    assert err < 2e-5, "relative error %g" % err
+    _assert_checked(op, y, t, "bf16x3")
 
 
 def test_conv_bf16_fast_mode_is_coarser_but_sane(eng):
-    g = torch.Generator(device="cpu").manual_seed(0)
-    x = torch.randn(1, 16, 24, 128, generator=g).cuda()
-    w = (torch.randn(128, 128, 3, 3, generator=g) / (128 * 9) ** 0.5).cuda()
-    b = torch.zeros(128).cuda()
-    ref = F.conv2d(x.permute(0, 3, 1, 2), w, b, padding=1).permute(0, 2, 3, 1)
-    y = eng.conv_test(x, w, b, relu=False, precision="bf16")
-    err = (y - ref).abs().max().item() / ref.abs().max().item()
-    assert err < 2e-2
+    op = conv_op(1, 16, 24, 128, 128, k=3, relu=False)
+    t = conv_inputs(op, 0)
+    t["b"].zero_()
+    y = run_conv(eng, op, t, "bf16")
+    torch.cuda.synchronize()
+    _assert_checked(op, y, t, "bf16")
+    assert not torch.equal(y, run_conv(eng, op, t, "bf16x3")), "bf16 gave the bits of bf16x3"
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 128, 208, 64, 256), (8, 64, 104, 128, 512), (1, 16, 26, 512, 2048)])
 def test_conv_residual_and_post_adds_deterministic(eng, B, H, W, Cin, Cout):
     """Last bottleneck of a layer in stages 1-2: relu(conv3 + x) + skip1 + skip2 (model/smap.py:74-75,143)."""
-    g = torch.Generator(device="cpu").manual_seed(7)
-    x = torch.randn(B, H, W, Cin, generator=g).cuda()
-    w = (torch.randn(Cout, Cin, 1, 1, generator=g) / Cin ** 0.5).cuda()
-    b = torch.randn(Cout, generator=g).cuda()
-    res, p1, p2 = (torch.randn(B, H, W, Cout, generator=g).cuda() for _ in range(3))
-    ref = F.relu(F.conv2d(x.permute(0, 3, 1, 2), w, b).permute(0, 2, 3, 1) + res) + p1 + p2
-    ys = [eng.conv_test(x, w, b, res=res, relu=True, post1=p1, post2=p2) for _ in range(4)]
+    op = conv_op(B, H, W, Cin, Cout, res=True, posts=2)
+    t = conv_inputs(op, 7)
+    ys = [run_conv(eng, op, t, "bf16x3") for _ in range(4)]
     torch.cuda.synchronize()
     for y in ys:
         assert torch.equal(y, ys[0]), "non-deterministic output"
-        assert (y - ref).abs().max().item() / ref.abs().max().item() < 2e-5
+    _assert_checked(op, ys[0], t, "bf16x3")
 
 
 _TILES = ("128", "64", "32")
@@ -74,22 +69,20 @@ def test_every_tile_shape_gives_the_same_bits(eng, monkeypatch, case):
     """The tile table / autotuner may pick any of these BLOCK_N shapes: each must be correct AND all must
     produce the same bits (every output element accumulates its K products in the same order whatever the tile), so that
     results do not depend on which shape a handle, a process or a rank happens to use."""
-    B, H, W, Cin, Cout, k, stride, use_res = case
-    x, w, b, res = _case_tensors(case, seed=11)
-    ref = F.conv2d(x.permute(0, 3, 1, 2), w, b, stride=stride, padding=k // 2).permute(0, 2, 3, 1)
-    ref = F.relu(ref + res if use_res else ref)
+    op = legacy_op(case)
+    t = conv_inputs(op, 11)
     first, n = None, 0
     for tile in _TILES:
-        bn = int(tile)
-        if Cout % bn:
+        if int(op["cout"]) % int(tile):
             continue
         monkeypatch.setenv("SMAPB_FORCE_TILE", tile)
-        y = eng.conv_test(x, w, b, res=res, stride=stride, relu=True)
+        launch = {}
+        y = run_conv(eng, op, t, "bf16x3", launch)
         torch.cuda.synchronize()
-        err = (y - ref).abs().max().item() / ref.abs().max().item()
-        assert err < 2e-5, "tile %s: relative error %g" % (tile, err)
+        assert launch["block_n"] == int(tile), launch
         if first is None:
             first = y
+            _assert_checked(op, y, t, "bf16x3")
         assert torch.equal(y, first), "tile %s differs from tile %s in %d elements" % (tile, _TILES[0], (y != first).sum().item())
         n += 1
     assert n >= 2

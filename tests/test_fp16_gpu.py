@@ -1,8 +1,9 @@
 """GPU: the fp16 precision (SMAPB_PREC_FP16): fp16 operands and activations, fp32 accumulation, stores clamped to +-65504.
 
   * single convolutions (the CASES of tests/plan_check.py) against a float64 reference built from the fp16-rounded
-    operands the device holds: |y - r| <= 1/2 ulp_fp16(y) + _acc_bound (tests/plan_check.py), and the same checker
-    flags a reference built from bf16-rounded operands;
+    operands the device holds, by the conv-level checker check_conv (tests/plan_check.py): |y - r| <= 1/2 ulp_fp16(y) +
+    _acc_bound, and the same checker flags a reference built from bf16-rounded operands (every kernel instance and
+    epilogue form at the edges of the tiling: tests/test_conv_edges_gpu.py);
   * saturation: outputs beyond +-65504 are exactly +-65504, never inf / NaN, and counted; folded weights beyond the range
     are rejected by finalize;
   * every op of the real plan against a float64 reference of its own layer, by the checker of tests/plan_check.py that
@@ -38,8 +39,8 @@ import torch.nn.functional as F
 from oracle import smap_torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from plan_check import (CASES, FP16_MAX, _TILE_CASES, _K, _acc_bound, _case_tensors, _gid, _nchw, _nhwc,  # noqa: E402
-                        assert_checked, check_switches, half_ulp16, no_tf32, op_class, plan_summary)
+from plan_check import (CASES, FP16_MAX, _TILE_CASES, _K, _gid, _nchw, _nhwc, assert_checked, check_conv,  # noqa: E402
+                        check_switches, conv_inputs, legacy_op, no_tf32, op_class, plan_summary, run_conv)
 
 pytestmark = pytest.mark.gpu
 
@@ -56,37 +57,16 @@ def eng():
     e.close()
 
 
-def _conv_reference(case, x, w, b, res, rnd):
-    """fp64 (r, pre, q) of one conv_test case with x, w, res rounded by rnd (the device's storage format)."""
-    B, H, W, Cin, Cout, k, stride, relu, use_res = case
-    d = lambda t: rnd(t).double()  # noqa: E731
-    conv = lambda xx, ww: F.conv2d(_nchw(xx), ww, stride=stride, padding=k // 2)  # noqa: E731
-    pre = _nhwc(conv(d(x), d(w))) + b.double()
-    sq = _nhwc(conv(d(x) ** 2, d(w) ** 2)) + b.double() ** 2
-    if use_res:
-        pre = pre + d(res)
-        sq = sq + d(res) ** 2
-    r = F.relu(pre) if relu else pre
-    return r, pre, sq.sqrt()
-
-
-def _conv_op(case):
-    return {"kind": "conv", "k": "%dx%d" % (case[5], case[5]), "cin": str(case[3])}
-
-
 @pytest.mark.parametrize("case", CASES)
 def test_conv_fp16_matches_fp64_of_device_operands(eng, case):
-    x, w, b, res = _case_tensors(case)
-    relu = case[7]
-    y = eng.conv_test(x, w, b, res=res, stride=case[6], relu=relu, precision="fp16").double()
+    op = legacy_op(case)
+    t = conv_inputs(op, hash(case) % (2 ** 31))
+    y = run_conv(eng, op, t, "fp16")
     torch.cuda.synchronize()
-    assert torch.equal(y, y.half().double()), "outputs are not fp16 values"
-    r, pre, q = _conv_reference(case, x, w, b, res, lambda t: t.half())
-    bound = half_ulp16(y) + _acc_bound(_conv_op(case), q, r, pre)
-    err = ((y - r).abs() / bound).max().item()
-    assert err <= 1.0, "error %.3g x the bound" % err
-    if relu:  # the ReLU clears exactly
-        assert (y[pre < -_acc_bound(_conv_op(case), q, pre)] == 0).all()
+    assert torch.equal(y, y.half().float()), "outputs are not fp16 values"
+    j = check_conv(op, y, t, "fp16")
+    assert not j["bad"], "\n".join(j["bad"])
+    assert not j["over"].any() and not j["band"].any()
     assert eng.saturation_count(reset=True) == 0
 
 
@@ -94,32 +74,33 @@ def test_checker_flags_a_bf16_operand_reference(eng):
     """On the largest-K case the checker that passes fp16 rejects a reference built from bf16-rounded operands: the bound
     resolves fp16's 4x finer operand rounding."""
     case = max(CASES, key=lambda c: c[3] * c[5] * c[5])
-    x, w, b, res = _case_tensors(case)
-    y = eng.conv_test(x, w, b, res=res, stride=case[6], relu=case[7], precision="fp16").double()
-    r16, pre16, q = _conv_reference(case, x, w, b, res, lambda t: t.half())
-    r, pre, _ = _conv_reference(case, x, w, b, res, lambda t: t.bfloat16())
-    over16 = (y - r16).abs() > half_ulp16(y) + _acc_bound(_conv_op(case), q, r16, pre16)
-    over = (y - r).abs() > half_ulp16(y) + _acc_bound(_conv_op(case), q, r, pre)
+    op = legacy_op(case)
+    t = conv_inputs(op, hash(case) % (2 ** 31))
+    y = run_conv(eng, op, t, "fp16")
+    torch.cuda.synchronize()
+    right, wrong = check_conv(op, y, t, "fp16"), check_conv(op, y, t, "fp16", operands="bf16")
     print("\n[fp16 checker] K=%d: fp16-operand reference %.3g, bf16-operand reference %.3g of the elements outside the"
-          " bound" % (_K(_conv_op(case)), over16.double().mean().item(), over.double().mean().item()))
-    assert not over16.any()
-    assert over.double().mean().item() > 0.05
+          " bound" % (_K(op), right["share"], wrong["share"]))
+    assert not right["bad"], right["bad"]
+    assert wrong["share"] > 0.05
 
 
 @pytest.mark.parametrize("case", _TILE_CASES)
 def test_fp16_every_tile_width_and_every_run_gives_the_same_bits(eng, monkeypatch, case):
-    B, H, W, Cin, Cout, k, stride, use_res = case
-    x, w, b, res = _case_tensors(case, seed=11)
+    op = legacy_op(case)
+    t = conv_inputs(op, 11)
     first, n = None, 0
     for tile in ("128", "64", "32"):
-        if Cout % int(tile):
+        if int(op["cout"]) % int(tile):
             continue
         monkeypatch.setenv("SMAPB_FORCE_TILE", tile)
         for _ in range(2):
-            y = eng.conv_test(x, w, b, res=res, stride=stride, relu=True, precision="fp16")
+            y = run_conv(eng, op, t, "fp16")
             torch.cuda.synchronize()
             if first is None:
                 first = y
+                j = check_conv(op, y, t, "fp16")
+                assert not j["bad"], "\n".join(j["bad"])
             assert torch.equal(y, first), "tile %s: %d elements differ" % (tile, (y != first).sum().item())
         n += 1
     assert n >= 2

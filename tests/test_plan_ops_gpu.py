@@ -8,7 +8,7 @@ per-channel max|y - r| / max|r_channel| (floored at 1e-3 max|r|) against the dev
 float64 layer computed from the unfolded state dict.  It is not asserted: channels that the ReLU or cancellation leave
 small carry the error of their inputs' magnitude (up to a few 1e-3 at 832x512).
 The checker is shown to flag deliberately wrong references, and plan switches (reverse tile order, PDL, one stream,
-forced tile widths) are shown not to change a single bit of any op."""
+forced tile widths) are shown not to change a single bit of any op, in bf16x3 and in bf16."""
 import os
 import re
 import sys
@@ -21,7 +21,7 @@ from plan_check import _MUTATIONS, _X3_ONLY, _gid, check_switches, op_class, pla
 pytestmark = pytest.mark.gpu
 
 BF16X3_GEOMS = [(64, 96, 2), (96, 160, 3), (512, 832, 8), (1024, 1024, 1)]
-BF16_GEOMS = [(64, 96, 2), (512, 832, 2)]
+BF16_GEOMS = [(64, 96, 2), (96, 160, 3), (512, 832, 2)]
 SWITCH_GEOMS = [(96, 160, 3), (512, 832, 8)]
 
 
@@ -75,7 +75,8 @@ def test_plan_op_coverage():
 
 
 @pytest.mark.parametrize("geom", SWITCH_GEOMS, ids=_gid)
-def test_plan_switches_keep_the_bits(geom, monkeypatch):
+@pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
+def test_plan_switches_keep_the_bits(precision, geom, monkeypatch):
     """Reverse tile order, PDL, one stream and every forced tile width give every op the same bits as the default plan.
     (Switches held in function-local statics, SMAPB_NO_GRAPH / SMAPB_DEBUG_STOP, cannot be toggled in one process.)"""
-    check_switches(geom, monkeypatch, "bf16x3")
+    check_switches(geom, monkeypatch, precision)
