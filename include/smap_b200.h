@@ -106,6 +106,31 @@ int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, i
 int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
                          int flags, int* status_host, void* stream);
 
+/* ---- PNG decoding (the step in front of pre-processing) -------------------------------------------------------------- */
+/* Replaces: cv2.imread(path, IMREAD_COLOR) (dataset/custom_dataset.py:27) for the PNGs it can decode, byte for byte: every
+ * legal bit depth / colour type pair (grey 1/2/4/8/16, RGB 8/16, palette 1/2/4/8, grey+alpha and RGBA 8/16), interlace 0
+ * and Adam7, any zlib stream (stored, fixed and dynamic blocks, any level, strategy, window and flush) in IDATs of any
+ * size, eXIf orientation 1..8 applied as cv2 applies it, up to SMAPB_JPEG_MAX_PIXELS.  As cv2 does, it keeps the high byte
+ * of 16-bit samples, drops alpha without compositing, replicates grey, scales 1/2/4-bit grey to 8 bits, reads a palette
+ * index past PLTE's entries as black and ignores tRNS, gAMA, sBIT, bKGD and colour management.  Everything else (APNG, an
+ * unknown critical chunk, a PLTE in a grey image, a CRC error in any chunk, a bad zlib header, preset dictionaries, a
+ * stream that does not inflate to exactly the scanlines' bytes, data after its Adler-32, non-PNG data) gets a status
+ * != SMAPB_JPEG_OK and is meant for cv2.imread; every file cv2 refuses is among them.  The statuses are SMAPB_JPEG_*. */
+/* Host only (no GPU work): chunk walk of one file.  *status = SMAPB_JPEG_*; when it is SMAPB_JPEG_OK, *h x *w is the shape
+ * cv2.imread returns (after the EXIF orientation) and *orientation the EXIF value (1 without one); zeros otherwise.
+ * Returns 0, or -1 for a NULL status. */
+int smapb_png_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* orientation, int* status);
+/* Decodes n files (host memory) into bgr_dev[i]: uint8 [h, w, 3] BGR as smapb_png_info reports the shape, which
+ * smapb_preprocess consumes.  bgr_dev[i] may be NULL only for files smapb_png_info does not accept.  status_host[i]
+ * (SMAPB_JPEG_*) says whether bgr_dev[i] holds the image; the header status can turn into SMAPB_JPEG_CORRUPT (an IDAT CRC,
+ * the Adler-32, a code or distance zlib refuses, too little data) or SMAPB_JPEG_UNSUPPORTED once the data is inflated.
+ * The zlib streams are inflated block-parallel: a block finder lists candidate dynamic-block headers, which are decoded
+ * side by side, and a walk from each stream's first block keeps the real ones and decodes the rest itself.  Each phase is
+ * one launch for the whole batch.  The workspace is owned by the handle and grows on demand; the call synchronises
+ * `stream` and returns once status_host is known, so it cannot be captured into a CUDA graph. */
+int smapb_decode_png(smapb_handle* h, int n, const uint8_t* const* png_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                     int* status_host, void* stream);
+
 /* ---- backbone -------------------------------------------------------------------------------- */
 /* Replaces: SMAP.forward inference branch (model/smap.py:403-419).
  * imgs_nchw_dev: fp32 [B,3,in_h,in_w] (normalised BGR).  Outputs fp32 NCHW:

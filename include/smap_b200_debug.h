@@ -34,6 +34,12 @@ long long smapb_debug_dump(smapb_handle* h, int B, int idx, void* host, long lon
 int smapb_debug_resize_plan(int src_w, int src_h, int net_w, int net_h, int* dims6, double* scale, int* xofs, short* xcoef,
                             int* yofs, short* ycoef);
 
+/* Inflate counters of the handle's last smapb_decode_png call: counts4 = {candidates the block finder listed, false
+ * positives (candidates no chained block starts at), chained blocks confirmed through the finder, chained blocks the
+ * serial walk handled itself (stored, fixed-Huffman, and dynamic blocks the finder missed or could not confirm)}.
+ * Zeros before the first call. */
+int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4);
+
 /* Environment switches read when a handle / plan is built (never on the per-call path):
  *   SMAPB_DEBUG_STOP=n        run only the first n ops of the plan
  *   SMAPB_DEBUG_SYNC=1        synchronise the stream after every launch

@@ -21,7 +21,7 @@ EXPORTS = [
     "smapb_comm_unique_id", "smapb_comm_create", "smapb_comm_attach", "smapb_allgather_records",
     "smapb_infer_device_gather", "smapb_submit_host_gather", "smapb_set_tile_table", "smapb_get_tile_table",
     "smapb_lift3d_gt", "smapb_infer_device_gather_async", "smapb_gather_sync", "smapb_saturation_count",
-    "smapb_jpeg_info", "smapb_decode_jpeg", "smapb_jpeg_info_ex", "smapb_decode_jpeg_ex",
+    "smapb_jpeg_info", "smapb_decode_jpeg", "smapb_jpeg_info_ex", "smapb_decode_jpeg_ex", "smapb_png_info", "smapb_decode_png",
 ]
 
 _lib = None
@@ -90,6 +90,9 @@ def load():
     lib.smapb_decode_jpeg.argtypes = [vp, i32, c.POINTER(c.c_char_p), c.POINTER(i64), c.POINTER(vp), c.POINTER(i32), vp]
     lib.smapb_jpeg_info_ex.argtypes = [c.c_char_p, i64, i32, c.POINTER(i32), c.POINTER(i32), c.POINTER(i32), c.POINTER(i32)]
     lib.smapb_decode_jpeg_ex.argtypes = [vp, i32, c.POINTER(c.c_char_p), c.POINTER(i64), c.POINTER(vp), i32, c.POINTER(i32), vp]
+    lib.smapb_png_info.argtypes = [c.c_char_p, i64, c.POINTER(i32), c.POINTER(i32), c.POINTER(i32), c.POINTER(i32)]
+    lib.smapb_decode_png.argtypes = [vp, i32, c.POINTER(c.c_char_p), c.POINTER(i64), c.POINTER(vp), c.POINTER(i32), vp]
+    lib.smapb_png_inflate_stats.argtypes = [vp, c.POINTER(i64)]  # include/smap_b200_debug.h
     lib.smapb_set_tile_table.argtypes = [c.c_char_p]
     lib.smapb_get_tile_table.argtypes = [c.c_char_p, i32]
     lib.smapb_json_open.argtypes = [c.POINTER(vp), c.c_char_p, c.c_char_p]

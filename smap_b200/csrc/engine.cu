@@ -211,6 +211,7 @@ void smapb_destroy(smapb_handle* h) {
     if (h->pre_stage) cudaFree(h->pre_stage);
     for (auto& e : h->pre_cache) cudaFree(e.second.buf);
     smapb::jpeg_workspace_destroy(h->jpeg);
+    smapb::png_workspace_destroy(h->png);
     delete h;
 }
 
@@ -415,6 +416,20 @@ int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host
 int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
                       int* status_host, void* stream) {
     return smapb_decode_jpeg_ex(h, n, jpeg_host, nbytes, bgr_dev, 0, status_host, stream);
+}
+
+int smapb_decode_png(smapb_handle* h, int n, const uint8_t* const* png_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
+                     int* status_host, void* stream) {
+    if (!h) return -1;
+    cudaSetDevice(h->device);
+    if (!h->png) h->png = smapb::png_workspace_create();
+    return smapb::png_decode(h->png, n, png_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4) {
+    if (!h || !counts4) return -1;
+    smapb::png_last_stats(h->png, counts4);
+    return 0;
 }
 
 // host-only introspection of the resampling plan (tests compare it with the oracle over many geometries without a GPU)

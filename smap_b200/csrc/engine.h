@@ -14,6 +14,7 @@
 #include "../../include/smap_b200.h"
 #include "conv_tc.cuh"
 #include "jpeg.h"
+#include "png.h"
 #include "preprocess.h"
 #include "refine.h"
 
@@ -166,6 +167,7 @@ struct smapb_handle {
     uint8_t* pre_stage = nullptr;
     size_t pre_stage_bytes = 0;
     smapb::JpegWorkspace* jpeg = nullptr;  // JPEG decoding (smapb_decode_jpeg), created on first use
+    smapb::PngWorkspace* png = nullptr;    // PNG decoding (smapb_decode_png), created on first use
     // RefineNet (optional post-processing step, SURVEY 8(f) f2)
     std::map<std::string, std::vector<float>> refine_raw;
     float* refine_buf = nullptr;  // folded, transposed weights + biases of the five layers

@@ -34,6 +34,7 @@
 
 #include "../../include/smap_b200.h"
 #include "jpeg.h"
+#include "orient.h"
 
 namespace smapb {
 namespace {
@@ -123,37 +124,7 @@ inline int u16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
 // EXIF orientation from an APP1 payload: 0 = not an EXIF block, 1..8, -1 = an orientation cv2 might read otherwise
 int exif_orientation(const uint8_t* s, int64_t len) {
     if (len < 6 || memcmp(s, "Exif\0\0", 6) != 0) return 0;
-    const uint8_t* t = s + 6;
-    const int64_t n = len - 6;
-    if (n < 8) return -1;
-    bool le;
-    if (memcmp(t, "II*\0", 4) == 0) le = true;
-    else if (memcmp(t, "MM\0*", 4) == 0) le = false;
-    else return -1;
-    auto rd = [&](int64_t i, int k, bool* ok) -> uint32_t {
-        if (i < 0 || i + k > n) {
-            *ok = false;
-            return 0;
-        }
-        uint32_t v = 0;
-        for (int j = 0; j < k; j++) v |= (uint32_t)t[i + j] << (8 * (le ? j : k - 1 - j));
-        return v;
-    };
-    bool ok = true;
-    const int64_t ifd = rd(4, 4, &ok);
-    const int cnt = (int)rd(ifd, 2, &ok);
-    if (!ok) return -1;
-    for (int e = 0; e < cnt; e++) {
-        const int64_t p = ifd + 2 + 12 * (int64_t)e;
-        const uint32_t tag = rd(p, 2, &ok);
-        if (!ok) return -1;
-        if (tag == 0x0112) {
-            const uint32_t typ = rd(p + 2, 2, &ok), c = rd(p + 4, 4, &ok), v = rd(p + 8, 2, &ok);
-            if (!ok || typ != 3 || c != 1 || v < 1 || v > 8) return -1;
-            return (int)v;
-        }
-    }
-    return 1;
+    return exif_tiff_orientation(s + 6, len - 6);
 }
 
 // Validates a Huffman table (canonical codes must fit their lengths) and fills the device form.
@@ -1070,18 +1041,8 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict_
         b = Y + ((116130 * cb + 32768) >> 16);
         r = min(max(r, 0), 255), g = min(max(g, 0), 255), b = min(max(b, 0), 255);
     }
-    // EXIF orientation as cv2 applies it (2 flip x, 3 rotate 180, 4 flip y, 5 transpose, 6 rotate 90 cw, 7 transverse, 8 ccw)
-    int oy = y, ox = x;
-    switch (I.orientation) {
-        case 2: ox = I.w - 1 - x; break;
-        case 3: oy = I.h - 1 - y, ox = I.w - 1 - x; break;
-        case 4: oy = I.h - 1 - y; break;
-        case 5: oy = x, ox = y; break;
-        case 6: oy = x, ox = I.h - 1 - y; break;
-        case 7: oy = I.w - 1 - x, ox = I.h - 1 - y; break;
-        case 8: oy = I.w - 1 - x, ox = y; break;
-        default: break;
-    }
+    int oy, ox;
+    orient_store_pos(I.orientation, I.h, I.w, y, x, &oy, &ox);
     uint8_t* o = I.out + ((int64_t)oy * I.out_w + ox) * 3;
     o[0] = (uint8_t)b, o[1] = (uint8_t)g, o[2] = (uint8_t)r;
 }

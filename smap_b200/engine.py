@@ -78,6 +78,16 @@ def jpeg_info(data, scans=False):
     return st.value, h.value, w.value, o.value
 
 
+def png_info(data):
+    """Chunk walk of one PNG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
+    handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h)."""
+    h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    rc = _lib.load().smapb_png_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
+    if rc != 0:
+        raise SmapB200Error("smapb_png_info failed (%d)" % rc)
+    return st.value, h.value, w.value, o.value
+
+
 class Engine:
     """One handle per (process, device).  in_h/in_w: network input size (multiples of 32)."""
 
@@ -245,6 +255,33 @@ class Engine:
         self._check(self.lib.smapb_decode_jpeg_ex(self._h, n, data, sizes, ptrs, flags, status, self._st()),
                     "smapb_decode_jpeg_ex")
         return [o if status[i] == 0 else None for i, o in enumerate(out)]
+
+    # ---- PNG decoding --------------------------------------------------------------------------
+    def decode_png(self, files):
+        """files: list of bytes (whole PNG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
+        cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
+        n = len(files)
+        out = [None] * n
+        if n == 0:
+            return out
+        ptrs = (ctypes.c_void_p * n)()
+        for i, f in enumerate(files):
+            st, h, w = png_info(f)[:3]
+            if st == 0:
+                out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
+                ptrs[i] = out[i].data_ptr()
+        data = (ctypes.c_char_p * n)(*files)
+        sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
+        status = (ctypes.c_int * n)()
+        self._check(self.lib.smapb_decode_png(self._h, n, data, sizes, ptrs, status, self._st()), "smapb_decode_png")
+        return [o if status[i] == 0 else None for i, o in enumerate(out)]
+
+    def png_stats(self):
+        """Inflate counters of the last decode_png call (smapb_png_inflate_stats): dict with candidates, false_positives,
+        confirmed (chained blocks found by the block finder) and serial (chained blocks the serial walk handled)."""
+        v = (ctypes.c_int64 * 4)()
+        self._check(self.lib.smapb_png_inflate_stats(self._h, v), "smapb_png_inflate_stats")
+        return dict(zip(("candidates", "false_positives", "confirmed", "serial"), list(v)))
 
     # ---- pre-processing ------------------------------------------------------------------------
     def preprocess(self, images, out=None):

@@ -7,8 +7,8 @@ path: images on disk -> result JSON.
 Same flags and the same output file name / schema as the reference ('{OUT}/stage3_root2_run_inference_{data_mode}_{suffix}.json',
 test.py:147-152).  Differences, both deliberate: images are visited in sorted path order unless --glob_order 1 (the
 reference uses glob order, dataset/custom_dataset.py:16-18).  Decoding, resize, letterbox, normalisation, backbone,
-association, lift, RefineNet and the JSON text are produced by libsmap_b200.so: .jpg/.jpeg files the GPU decoder supports
-are decoded on the GPU (byte-identical to cv2.imread), every other file by cv2.imread as in the reference.
+association, lift, RefineNet and the JSON text are produced by libsmap_b200.so: .jpg/.jpeg and .png files the GPU decoders
+support are decoded on the GPU (byte-identical to cv2.imread), every other file by cv2.imread as in the reference.
 """
 import argparse
 import glob
@@ -38,28 +38,30 @@ def image_name(path, dataset_path):
 
 
 def read_frames(eng, paths, imread):
-    """.jpg/.jpeg files through the GPU decoder, in one batch; the rest, and the JPEGs it leaves to cv2, through imread."""
+    """.jpg/.jpeg files through the GPU JPEG decoder and .png files through the GPU PNG decoder, one batch each; the rest,
+    and the files a decoder leaves to cv2, through imread."""
     frames = [None] * len(paths)
-    jpg = [i for i, p in enumerate(paths) if p.lower().endswith((".jpg", ".jpeg"))]
-    if jpg:
-        files = []
-        for i in jpg:
-            with open(paths[i], "rb") as f:
-                files.append(f.read())
-        for i, im in zip(jpg, eng.decode_jpeg(files)):
-            frames[i] = im
+    for exts, decode in (((".jpg", ".jpeg"), eng.decode_jpeg), ((".png",), eng.decode_png)):
+        sel = [i for i, p in enumerate(paths) if p.lower().endswith(exts)]
+        if sel:
+            files = []
+            for i in sel:
+                with open(paths[i], "rb") as f:
+                    files.append(f.read())
+            for i, im in zip(sel, decode(files)):
+                frames[i] = im
     return [imread(p) if im is None else im for p, im in zip(paths, frames)]
 
 
 def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False, dataset_name="CMU",
         device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None):
     """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3], used for every file; by default .jpg/.jpeg
-    files are decoded on the GPU (Engine.decode_jpeg, byte-identical to cv2.imread) and the files it does not handle, as
-    every other file, go through cv2.imread(path, IMREAD_COLOR).  precision: one of engine.PRECISIONS.  stats (a dict,
+    and .png files are decoded on the GPU (Engine.decode_jpeg / Engine.decode_png, byte-identical to cv2.imread) and the
+    files they do not handle, as every other file, go through cv2.imread(path, IMREAD_COLOR).  precision: one of engine.PRECISIONS.  stats (a dict,
     optional) receives "saturation": the fp16 clamp count."""
     if precision not in PRECISIONS:
         raise ValueError("unknown precision %r (choose from %s)" % (precision, ", ".join(PRECISIONS)))
-    gpu_jpeg = imread is None
+    gpu_decode = imread is None
     if imread is None:
         import cv2
 
@@ -80,7 +82,7 @@ def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batc
         with ResultWriter(output_file, dataset_name) as w:
             for lo in range(0, len(paths), batch_size):
                 chunk = paths[lo:lo + batch_size]
-                frames = read_frames(eng, chunk, imread) if gpu_jpeg else [imread(p) for p in chunk]
+                frames = read_frames(eng, chunk, imread) if gpu_decode else [imread(p) for p in chunk]
                 frames = [f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f)) for f in frames]
                 imgs, scales = eng.preprocess(frames)
                 rec = eng.infer_device(imgs, scales.to(imgs.device), do_flip=bool(do_flip))
