@@ -115,7 +115,9 @@ int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host
  * index past PLTE's entries as black and ignores tRNS, gAMA, sBIT, bKGD and colour management.  Everything else (APNG, an
  * unknown critical chunk, a PLTE in a grey image, a CRC error in any chunk, a bad zlib header, preset dictionaries, a
  * stream that does not inflate to exactly the scanlines' bytes, data after its Adler-32, non-PNG data) gets a status
- * != SMAPB_JPEG_OK and is meant for cv2.imread; every file cv2 refuses is among them.  The statuses are SMAPB_JPEG_*. */
+ * != SMAPB_JPEG_OK and is meant for cv2.imread; every file cv2 refuses is among them.  Two kinds of valid stream that
+ * cv2 reads are among them too: more DEFLATE blocks than (zlib stream bytes) / 8 + 64, and a match reaching past the
+ * window the zlib header declares.  The statuses are SMAPB_JPEG_*. */
 /* Host only (no GPU work): chunk walk of one file.  *status = SMAPB_JPEG_*; when it is SMAPB_JPEG_OK, *h x *w is the shape
  * cv2.imread returns (after the EXIF orientation) and *orientation the EXIF value (1 without one); zeros otherwise.
  * Returns 0, or -1 for a NULL status. */

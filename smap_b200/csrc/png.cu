@@ -28,6 +28,11 @@
 //                       resolved, computes the Adler-32 and checks it
 //   7. unfilter_kernel  one CTA per (image, Adam7 pass): a wavefront in which row r runs one unit behind row r - 1
 //   8. colour_kernel    bit unpacking, palette, grey replication, high bytes, RGB -> BGR, Adam7 scatter, EXIF orientation
+// Two valid streams that cv2 reads are refused on the device (SMAPB_JPEG_UNSUPPORTED and SMAPB_JPEG_CORRUPT) and left to
+// cv2: one with more DEFLATE blocks than blk_cap = zlen / 8 + 64, the block records reserved per image (an exact bound, one
+// block per 10 bits, would take 6.4 times the memory; a run of empty fixed blocks such as Z_PARTIAL_FLUSH writes reaches
+// it), and one with a match that reaches past the window its zlib header's CINFO declares (zlib only refuses a distance
+// past the bytes it holds, so whether cv2 reads it depends on the output buffers libpng hands to inflate).
 // oracle/png_numpy.py restates the walk and the pixel rules, oracle/inflate_numpy.py the block structure and the finder.
 #include <stdlib.h>
 #include <string.h>

@@ -95,8 +95,9 @@ def compress(raw, level=6, wbits=15, mem=8, strategy=zlib.Z_DEFAULT_STRATEGY, fl
 
 
 def write_png(s, ctype, depth, interlace=0, filters=lambda r: r % 5, z=None, zopts=None, split=None, pre=b"", post=b"",
-              palette=None):
-    """A PNG of the samples: IHDR, `pre` chunks, PLTE, IDAT(s) cut into pieces of the sizes split(i) gives, `post`, IEND."""
+              palette=None, empty_after=0):
+    """A PNG of the samples: IHDR, `pre` chunks, PLTE, IDAT(s) cut into pieces of the sizes split(i) gives (0 = an empty
+    IDAT), `empty_after` empty IDATs, `post`, IEND."""
     h, w = s.shape[:2]
     if z is None:
         z = compress(scanlines(s, ctype, depth, interlace, filters), **(zopts or {}))
@@ -112,6 +113,7 @@ def write_png(s, ctype, depth, interlace=0, filters=lambda r: r % 5, z=None, zop
             n = split(k)
             b += chunk(b"IDAT", z[i:i + n])
             i, k = i + n, k + 1
+    b += chunk(b"IDAT", b"") * empty_after
     return b + post + chunk(b"IEND", b"")
 
 

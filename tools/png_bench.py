@@ -9,7 +9,12 @@ candidates and false positives and the blocks per image.  Then the run_inference
 (decode, preprocess, infer_device, records to the host) is timed in bf16x3 and fp16 with each decoder (cv2 on one thread
 is what the CLI did before).  The GPU's name, power limit and SM clock are read in the same call.
 
+--single-block instead times one 1920x1080 frame stored as a single dynamic block of literals (as fpnge-style writers
+store a frame): a block of millions of symbols is past the count pass's symbol cap, so the chain walk and the write pass
+each decode it on one thread.  The same frame written by cv2.imencode (hundreds of blocks) is timed beside it.
+
     python tools/png_bench.py [--batch 8] [--rounds 5] [--json out/png_bench.json]
+    python tools/png_bench.py --single-block [--rounds 5] [--json out/png_single_block.json]
 """
 import argparse
 import json
@@ -25,7 +30,8 @@ from decode_bench import cv2_decode, gpu_info, sm_clock, timed  # noqa: E402
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from png_corpus import large_frames  # noqa: E402
+from deflate_writer import one_block_zlib  # noqa: E402
+from png_corpus import large_frames, scanlines, write_png  # noqa: E402
 from smap_b200 import schema  # noqa: E402
 from smap_b200.engine import RECORD_BYTES, Engine  # noqa: E402
 
@@ -49,12 +55,44 @@ def phase_shares(eng, files):
     return {"kernel_ms": round(tot / 1e3, 3), **{p: round(v / tot, 3) for p, v in by.items()}} if tot else None
 
 
+def single_block(a):
+    from jpeg_corpus import content
+    from png_corpus import cv2_png
+
+    name, power = gpu_info()
+    im = content("smooth", 1080, 1920, np.random.default_rng(1))
+    s = np.ascontiguousarray(im[..., ::-1])
+    one = write_png(s, 2, 8, z=one_block_zlib(scanlines(s, 2, 8, 0, lambda r: 4)))
+    out = {"gpu": name, "power_limit": power, "frame": "1920x1080", "rounds": a.rounds}
+    eng = Engine(0, max_batch=1)
+    for key, f in (("one_dynamic_block", one), ("cv2_imencode", cv2_png(im))):
+        (g,) = eng.decode_png([f])
+        assert g is not None and np.array_equal(g.cpu().numpy(), cv2_decode(f)), key
+        row = {"mbytes": round(len(f) / 1e6, 3), "finder": eng.png_stats()}
+        for arm, fn in (("gpu_ms", lambda: eng.decode_png([f])), ("cv2_1_thread_ms", lambda: cv2_decode(f))):
+            row[arm] = round(1e3 * timed(fn, a.rounds), 2)
+        row["sm_clock_mhz"] = sm_clock()
+        row["phase_share_of_kernel_time"] = phase_shares(eng, [f])
+        out[key] = row
+    eng.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--json", default="")
+    ap.add_argument("--single-block", action="store_true")
     a = ap.parse_args()
+    if a.single_block:
+        out = single_block(a)
+        print(json.dumps(out))
+        if a.json:
+            os.makedirs(os.path.dirname(os.path.abspath(a.json)), exist_ok=True)
+            with open(a.json, "w") as f:
+                f.write(json.dumps(out) + "\n")
+        return
     B = a.batch
     cores = os.cpu_count() or 1
     pool = ThreadPoolExecutor(cores)
