@@ -45,13 +45,13 @@ def _u16(d, i):
 
 def _huff_table(counts, symbols):
     """Canonical code assignment (T.81 Annex C) -> list of 65536 entries (len << 8 | symbol) indexed by the next 16 bits;
-    0 = no code.  Over-subscribed tables are rejected."""
+    0 = no code.  Tables that are over-subscribed or use a code of all ones are rejected (_check_canonical)."""
     lut = [0] * 65536
     code, k = 0, 0
     for length in range(1, 17):
         for _ in range(counts[length - 1]):
-            if code >= (1 << length):
-                raise NotDecoded(MALFORMED, "over-subscribed Huffman table")
+            if code >= (1 << length) - 1:
+                raise NotDecoded(MALFORMED, "over-subscribed Huffman table or a code of all ones")
             lo = code << (16 - length)
             e = (length << 8) | symbols[k]
             for j in range(lo, lo + (1 << (16 - length))):
@@ -63,11 +63,13 @@ def _huff_table(counts, symbols):
 
 
 def _check_canonical(counts):
+    """libjpeg's rule (jpeg_make_d_derived_tbl): the codes of each length must fit it, and none may be all ones, so a
+    complete code is refused too."""
     code = 0
     for length in range(1, 17):
         code += counts[length - 1]
-        if code > (1 << length):
-            raise NotDecoded(MALFORMED, "over-subscribed Huffman table")
+        if code >= (1 << length):
+            raise NotDecoded(MALFORMED, "over-subscribed Huffman table or a code of all ones")
         code <<= 1
 
 

@@ -127,14 +127,15 @@ int exif_orientation(const uint8_t* s, int64_t len) {
     return exif_tiff_orientation(s + 6, len - 6);
 }
 
-// Validates a Huffman table (canonical codes must fit their lengths) and fills the device form.
+// Validates a Huffman table and fills the device form.  As in libjpeg (jpeg_make_d_derived_tbl), the canonical codes
+// must fit their lengths and none may be all ones, so a complete code is refused (cv2 fails on such a file).
 bool build_huff(const HuffSpec& s, DevHuff* d) {
     memset(d, 0, sizeof(*d));
     int code = 0, k = 0;
     for (int l = 1; l <= 16; l++) {
         d->valoff[l] = k - code;
         for (int i = 0; i < s.counts[l - 1]; i++) {
-            if (code >= (1 << l)) return false;
+            if (code >= (1 << l) - 1) return false;
             if (l <= 9)
                 for (int j = 0; j < (1 << (9 - l)); j++) d->fast[(code << (9 - l)) + j] = (uint16_t)((l << 8) | s.vals[k]);
             code++, k++;
