@@ -100,7 +100,9 @@ int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, c
  * progressive Huffman files (SOF2) whose progression libjpeg accepts without a warning and whose coefficients 1..9 are
  * fully refined in every component (otherwise libjpeg-turbo smooths the output, and the file is left to cv2), with at
  * most 64 scans and no DQT redefining a table a scan already used.  One call decodes a mixed batch (single-scan,
- * multi-scan and refused files); the status codes, the shape rule and the synchronisation are those of the plain forms. */
+ * multi-scan and refused files); the status codes, the shape rule and the synchronisation are those of the plain forms.
+ * AC refinement scans decode sequentially within a restart segment (a block's bits depend on its coefficients' history),
+ * one warp per segment against per-block history masks; the segments, and the images of a batch, run side by side. */
 #define SMAPB_JPEG_SCANS 1
 int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status);
 int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,

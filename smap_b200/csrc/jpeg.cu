@@ -22,7 +22,13 @@
 //      scan_write_kernel  the final pass: coefficients into their blocks (DC as differences)
 //      scan_dc_kernel     DC prediction: a scan per component, reset at every restart
 //      dc_refine_kernel   one raw bit per block at a position known from the block's index in its restart segment
-//      ac_refine_kernel   one thread per restart segment: the bits a block takes depend on its nonzero history
+//      AC refinement: the bits a block takes depend on which of its coefficients are already nonzero (its history), so
+//      no speculative decoder can start mid-segment; the history is fixed before the scan, so the serial part walks
+//      registers only:
+//      acr_mask_kernel    the history of every block as a 64-bit mask, one thread per block
+//      acr_decode_kernel  one warp per restart segment: one lane decodes the symbols against the masks and stores per
+//                         block its correction bits and new coefficients; the warp takes long EOB runs 32 blocks a step
+//      acr_apply_kernel   corrections and new coefficients into the blocks, one thread per block
 //   c. idct_kernel        dequantisation + accurate-integer IDCT (LL&M, 13-bit constants, 2 pass-1 bits), saturated
 //   d. colour_kernel      fancy upsampling, fixed-point YCbCr -> BGR, EXIF orientation, uint8 HWC BGR
 // oracle/jpeg_numpy.py restates every stage on the CPU, oracle/jpeg_scans_numpy.py the multi-scan entropy decoding.
@@ -89,6 +95,7 @@ struct DevScan {
     int blk_comp[6], blk_map[6];  // block of the scan's MCU -> scan component, -> block of the frame's MCU (interleaved)
     int blk_dc[6], blk_ac[6];     // -> its tables (indices into the batch's table array)
     int seg0, nseg, sub0, nsub;
+    int acr_off;                  // AC refinement: the scan's first block in the round's masks and records
     int64_t raw_off, raw_len, unst_off;
 };
 
@@ -836,92 +843,261 @@ __global__ void __launch_bounds__(256) dc_refine_kernel(const DevImage* __restri
     }
 }
 
-// AC refinement (libjpeg's decode_mcu_AC_refine): the bits a block takes depend on which of its coefficients are already
-// nonzero, so no speculative decoder can start mid-segment; one thread decodes one restart segment.  It reads and writes
-// only the current block's coefficients, at or after its zig-zag position.
-__global__ void __launch_bounds__(128) ac_refine_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
-                                                        const DevHuff* __restrict__ huffs, const int* __restrict__ list, int n,
-                                                        const DevSeg* __restrict__ segs, const uint8_t* __restrict__ unst,
-                                                        int* __restrict__ status, int16_t* __restrict__ coef) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    const DevSeg& G = segs[list[t]];
-    const DevScan& S = scans[G.scan];
-    const DevImage& I = imgs[S.img];
-    if (status[S.img] != SMAPB_JPEG_OK) return;
-    const DevHuff& T = huffs[S.blk_ac[0]];
-    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
-    int16_t* cf = coef + I.coef_off * 64;
-    const int p1 = 1 << S.al, m1 = -(1 << S.al);
-    uint32_t pos = G.bit_begin;
-    const uint32_t end = G.bit_end;
-    bool bad = false;
-    int eobrun = 0;
-    auto bit = [&]() -> int {
-        if (pos >= end) {
-            bad = true;
-            return 0;
+// AC refinement (libjpeg's decode_mcu_AC_refine), in three phases.  The bits a block takes depend only on which of its
+// coefficients in [Ss, Se] are nonzero before the scan (its history): one correction bit for every history coefficient the
+// decoder passes, and the zero ones count towards a symbol's run.  A coefficient the scan makes nonzero lies behind the
+// decoder, so the history stays fixed while the scan is decoded.
+//   acr_mask_kernel    one thread per block: its history as a mask, bit k = zig-zag coefficient k, in the scan's order
+//   acr_decode_kernel  one warp per restart segment: one lane decodes the symbols against the masks alone, in registers,
+//                      and stores per block its correction bits and its new coefficients (AcrRecord); the blocks of an EOB
+//                      run past the lane's window of 32 blocks are taken by the whole warp, 32 per step
+//   acr_apply_kernel   one thread per block: the corrections and the new +-2^Al coefficients into the coefficient buffer
+// A segment's masks and records lie at the scan's acr_off + the segment's first block (these scans are not interleaved).
+struct AcrRecord {
+    unsigned long long corr;  // bit i: correction bit of the i-th history coefficient (in zig-zag order)
+    unsigned long long pos;   // bit k: zig-zag coefficient k becomes +-2^Al
+    unsigned long long neg;   // bit k: ... and it is -2^Al
+};
+
+constexpr int ACR_WARPS = 4;  // segments per CTA of acr_decode_kernel
+
+__device__ __forceinline__ uint32_t word_be(const uint32_t* words, uint32_t w) { return __byte_perm(words[w], 0, 0x0123); }
+
+// The 64 bits from `pos`, MSB first.
+__device__ __forceinline__ unsigned long long peek64(const uint32_t* words, uint32_t pos) {
+    const uint32_t w = pos >> 5, sh = pos & 31;
+    const uint32_t a = word_be(words, w), b = word_be(words, w + 1), c = word_be(words, w + 2);
+    return (unsigned long long)__funnelshift_l(b, a, sh) << 32 | __funnelshift_l(c, b, sh);
+}
+
+// The top n bits of v (MSB first) as a word whose bit i is the i-th of them.
+__device__ __forceinline__ unsigned long long first_bits_lsb(unsigned long long v, int n) {
+    return n ? __brevll(v & ~(~0ull >> n)) : 0ull;
+}
+
+// MSB-first bit reader over the unstuffed words: `buf` holds the next `nb` bits (33..64 between calls).
+struct BitBuf {
+    const uint32_t* words;
+    unsigned long long buf;
+    int nb;
+    uint32_t w, pos;  // next word to load, bit position of buf's first bit
+    __device__ __forceinline__ void init(const uint32_t* wd, uint32_t p) {
+        words = wd, pos = p, w = p >> 5;
+        buf = (unsigned long long)word_be(words, w++) << (32 + (p & 31));
+        nb = 32 - (int)(p & 31);
+        fill();
+    }
+    __device__ __forceinline__ void fill() {
+        if (nb <= 32) {
+            buf |= (unsigned long long)word_be(words, w++) << (32 - nb);
+            nb += 32;
         }
-        return (int)(peek32(words, pos++) >> 31);
-    };
-    for (int q = 0; q < G.nmcu && !bad; q++) {
-        int16_t* blk = cf + scan_block(S, I, G.first_mcu + q) * 64;
-        int k = S.ss;
-        if (eobrun == 0) {
-            for (; k <= S.se && !bad; k++) {
-                int sym = 0;
-                const int len = huff_lookup(T, peek32(words, pos), &sym);
-                if (!len || pos + len > end) {
-                    bad = true;
-                    break;
-                }
-                pos += len;
-                int r = sym >> 4, s = sym & 15, sv = 0;
-                if (s) {
-                    if (s != 1) {
+    }
+    // the next n <= 32 bits, left-aligned
+    __device__ __forceinline__ unsigned long long take(int n) {
+        const unsigned long long v = buf & ~(~0ull >> n);
+        buf <<= n;
+        nb -= n, pos += n;
+        fill();
+        return v;
+    }
+    // the next n <= 63 bits, left-aligned
+    __device__ __forceinline__ unsigned long long take_long(int n) {
+        const int a = min(n, 32);
+        const unsigned long long hi = take(a);
+        return hi | (take(n - a) >> a);
+    }
+};
+
+__global__ void __launch_bounds__(256) acr_mask_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                       const int* __restrict__ list, const int* __restrict__ status,
+                                                       const int16_t* __restrict__ coef, unsigned long long* __restrict__ masks) {
+    const DevScan& S = scans[list[blockIdx.y]];
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= S.nmcu * S.bpm || status[S.img] != SMAPB_JPEG_OK) return;
+    const DevImage& I = imgs[S.img];
+    const int4* c = (const int4*)(coef + (I.coef_off + scan_block(S, I, t)) * 64);
+    unsigned long long nz = 0;  // natural order
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+        const int4 v = c[q];
+        const int x[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; e++)
+            nz |= (unsigned long long)((x[e] & 0xFFFF) != 0) << (8 * q + 2 * e) |
+                  (unsigned long long)((x[e] >> 16) != 0) << (8 * q + 2 * e + 1);
+    }
+    unsigned long long m = 0;
+    for (int k = S.ss; k <= S.se; k++) m |= (nz >> c_zigzag[k] & 1ull) << k;
+    masks[S.acr_off + t] = m;
+}
+
+__global__ void __launch_bounds__(32 * ACR_WARPS, 1) acr_decode_kernel(const DevScan* __restrict__ scans,
+                                                                    const DevHuff* __restrict__ huffs,
+                                                                    const int* __restrict__ list, int n,
+                                                                    const DevSeg* __restrict__ segs,
+                                                                    const uint8_t* __restrict__ unst, int* __restrict__ status,
+                                                                    const unsigned long long* __restrict__ masks,
+                                                                    AcrRecord* __restrict__ recs) {
+    __shared__ DevHuff s_huff[ACR_WARPS];
+    __shared__ unsigned long long s_mask[ACR_WARPS][32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int g = blockIdx.x * ACR_WARPS + wid;
+    if (g >= n) return;
+    const DevSeg& G = segs[list[g]];
+    const DevScan& S = scans[G.scan];
+    if (status[S.img] != SMAPB_JPEG_OK) return;
+    {
+        const uint32_t* src = (const uint32_t*)&huffs[S.blk_ac[0]];
+        uint32_t* dst = (uint32_t*)&s_huff[wid];
+        for (int i = lane; i < (int)(sizeof(DevHuff) / 4); i += 32) dst[i] = src[i];
+    }
+    __syncwarp();
+    const DevHuff& T = s_huff[wid];
+    const uint32_t* words = (const uint32_t*)(unst + S.unst_off);
+    const unsigned long long* M = masks + S.acr_off + (int64_t)G.first_mcu * S.bpm;
+    AcrRecord* rec = recs + S.acr_off + (int64_t)G.first_mcu * S.bpm;
+    const int nblk = G.nmcu * S.bpm;
+    const unsigned long long band = (~0ull << S.ss) & (~0ull >> (63 - S.se));  // bits Ss..Se
+    const uint32_t end = G.bit_end;
+    uint32_t pos = G.bit_begin;
+    int run = 0;  // blocks of an open EOB run still to take
+    bool bad = false;
+    unsigned long long ahead = lane < nblk ? M[lane] : 0ull;  // the next window's masks, one per lane
+    for (int q = 0; q < nblk; q += 32) {
+        const unsigned long long mine = ahead;
+        ahead = q + 32 + lane < nblk ? M[q + 32 + lane] : 0ull;
+        const int cnt = min(32, nblk - q);
+        int j = 0;
+        if (run > 0) {
+            // the warp takes the run's blocks of this window: each lane one block, its bits at a warp prefix sum
+            j = min(run, cnt);
+            const int nb = lane < j ? __popcll(mine) : 0;
+            int incl = nb;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += y;
+            }
+            const int total = __shfl_sync(0xffffffffu, incl, 31);
+            if ((uint64_t)pos + total > end) {
+                bad = true;
+                break;
+            }
+            if (lane < j) rec[q + lane] = {first_bits_lsb(peek64(words, pos + incl - nb), nb), 0ull, 0ull};
+            pos += total;
+            run -= j;
+        }
+        if (j == cnt) continue;
+        s_mask[wid][lane] = mine;
+        __syncwarp();
+        if (lane == 0) {
+            BitBuf B;
+            B.init(words, pos);
+            for (; j < cnt && !bad; j++) {
+                const unsigned long long m = s_mask[wid][j];
+                if (run > 0) {  // a block of the run: one correction bit per history coefficient
+                    const int nc = __popcll(m);
+                    if (B.pos + nc > end) {
                         bad = true;
                         break;
                     }
-                    sv = bit() ? p1 : m1;
-                } else if (r != 15) {
-                    eobrun = 1 << r;
-                    if (r) {
-                        if (pos + r > end) {
+                    rec[q + j] = {first_bits_lsb(B.take_long(nc), nc), 0ull, 0ull};
+                    run--;
+                    continue;
+                }
+                // hist / zeros: the history and the zero coefficients of [Ss, Se] the decoder has not passed yet; the
+                // correction bits are gathered from bit 63 down and reversed once
+                unsigned long long hist = m, zeros = ~m & band, acc = 0, newp = 0, newn = 0;
+                int nc = 0;
+                for (;;) {
+                    int sym = 0;
+                    const int len = huff_lookup(T, (uint32_t)(B.buf >> 32), &sym);
+                    const int r = sym >> 4, s = sym & 15;
+                    // a new coefficient's sign bit follows its code: both are taken at once
+                    if (!len || B.pos + len + (s != 0) > end || s > 1) {
+                        bad = true;
+                        break;
+                    }
+                    const bool neg = s && (B.buf >> (63 - len) & 1) == 0;
+                    B.take(len + s);
+                    unsigned long long passed, at = 0;  // the history coefficients the symbol passes, its new coefficient
+                    if (!s && r != 15) {  // EOBn: this block's remaining history, then 2^r + extra - 1 more blocks
+                        if (B.pos + r > end) {
                             bad = true;
                             break;
                         }
-                        eobrun += (int)(peek32(words, pos) >> (32 - r));
-                        pos += r;
+                        run = (1 << r) + (r ? (int)(B.take(r) >> (64 - r)) : 0) - 1;
+                        passed = hist;
+                    } else {
+                        // the (r + 1)-th zero coefficient; a ZRL that finds none passes the rest and ends the block
+                        unsigned long long z = zeros;
+                        for (int i = 0; i < r && z; i++) z &= z - 1;  // r is 0 for most symbols
+                        at = z & (0ull - z);
+                        if (s && !at) {
+                            bad = true;  // a new coefficient past Se
+                            break;
+                        }
+                        passed = at ? hist & (at - 1) : hist;
+                        zeros = z ^ at;
                     }
-                    break;
-                }
-                do {
-                    int16_t* c = blk + c_zigzag[k];
-                    if (*c != 0) {
-                        if (bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
-                    } else if (--r < 0) {
-                        break;
-                    }
-                    k++;
-                } while (k <= S.se);
-                if (sv) {
-                    if (k > S.se) {
+                    const int nb = __popcll(passed);
+                    if (B.pos + nb > end) {
                         bad = true;
                         break;
                     }
-                    blk[c_zigzag[k]] = (int16_t)sv;
+                    if (nb) {
+                        acc |= (nb <= 32 ? B.take(nb) : B.take_long(nb)) >> nc;
+                        nc += nb;
+                    }
+                    hist ^= passed;
+                    if (s) {
+                        newp |= at;
+                        if (neg) newn |= at;
+                    }
+                    if (!at || !(zeros | hist)) break;  // EOB, a ZRL that ran out, or Se passed
                 }
+                const unsigned long long corr = __brevll(acc);
+                if (bad) break;
+                rec[q + j] = {corr, newp, newn};
             }
+            pos = B.pos;
         }
-        if (eobrun > 0) {
-            for (; k <= S.se; k++) {
-                int16_t* c = blk + c_zigzag[k];
-                if (*c != 0 && bit() && (*c & p1) == 0) *c = (int16_t)(*c >= 0 ? *c + p1 : *c + m1);
-            }
-            eobrun--;
+        __syncwarp();
+        pos = __shfl_sync(0xffffffffu, pos, 0);
+        run = __shfl_sync(0xffffffffu, run, 0);
+        if (__shfl_sync(0xffffffffu, (int)bad, 0)) {
+            bad = true;
+            break;
         }
     }
-    if (bad) status[S.img] = SMAPB_JPEG_CORRUPT;
+    if (bad && lane == 0) status[S.img] = SMAPB_JPEG_CORRUPT;
+}
+
+__global__ void __launch_bounds__(256) acr_apply_kernel(const DevImage* __restrict__ imgs, const DevScan* __restrict__ scans,
+                                                        const int* __restrict__ list, const int* __restrict__ status,
+                                                        const unsigned long long* __restrict__ masks,
+                                                        const AcrRecord* __restrict__ recs, int16_t* __restrict__ coef) {
+    const DevScan& S = scans[list[blockIdx.y]];
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= S.nmcu * S.bpm || status[S.img] != SMAPB_JPEG_OK) return;
+    const AcrRecord R = recs[S.acr_off + t];
+    if (!(R.corr | R.pos)) return;
+    const DevImage& I = imgs[S.img];
+    int16_t* c = coef + (I.coef_off + scan_block(S, I, t)) * 64;
+    const int p1 = 1 << S.al;
+    // the i-th correction bit goes with the i-th set bit of the history mask
+    unsigned long long m = masks[S.acr_off + t];
+    for (unsigned long long corr = R.corr; corr; corr >>= 1, m &= m - 1) {
+        if (corr & 1) {
+            int16_t* v = c + c_zigzag[__ffsll((long long)m) - 1];
+            if ((*v & p1) == 0) *v = (int16_t)(*v >= 0 ? *v + p1 : *v - p1);
+        }
+    }
+    for (unsigned long long p = R.pos; p; p &= p - 1) {
+        const int k = __ffsll((long long)p) - 1;
+        c[c_zigzag[k]] = (int16_t)(R.neg >> k & 1 ? -p1 : p1);
+    }
 }
 
 // ---- c. dequantisation + IDCT ----------------------------------------------------------------------------------------
@@ -1074,6 +1250,10 @@ struct JpegWorkspace {
     size_t base_cap = 0;
     int16_t* coef = nullptr;
     size_t coef_cap = 0;
+    unsigned long long* acr_mask = nullptr;  // AC refinement: history masks and records of a round's blocks
+    size_t acr_mask_cap = 0;
+    AcrRecord* acr_rec = nullptr;
+    size_t acr_rec_cap = 0;
     uint8_t* planes = nullptr;
     size_t planes_cap = 0;
     int* small = nullptr;  // status[n] then changed[passes]
@@ -1096,7 +1276,7 @@ void jpeg_workspace_destroy(JpegWorkspace* ws) {
     if (!ws) return;
     if (ws->host) cudaFreeHost(ws->host);
     if (ws->small_host) cudaFreeHost(ws->small_host);
-    void* d[] = {ws->dev_in, ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->planes, ws->small};
+    void* d[] = {ws->dev_in, ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->acr_mask, ws->acr_rec, ws->planes, ws->small};
     for (void* p : d)
         if (p) cudaFree(p);
     delete ws;
@@ -1106,10 +1286,12 @@ static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 namespace {
 // What one round (the r-th scan of every image that has one) launches: subsequences [sub_lo, sub_lo + nsub) of its
-// Huffman scans, and ranges of the batch's index list (scans, or segments for AC refinement).
+// Huffman scans, and ranges of the batch's index list (scans, and segments for AC refinement).  AC refinement scans
+// take acr_total blocks of the masks and records, the largest acr_blocks.
 struct Round {
     int sub_lo = 0, nsub = 0, max_nsub_seg = 1;
     int huff_off = 0, nhuff = 0, dc_off = 0, ndc = 0, dcr_off = 0, ndcr = 0, dcr_blocks = 0, acr_off = 0, nacr = 0;
+    int acrs_off = 0, nacrs = 0, acr_blocks = 0, acr_total = 0;
 };
 }  // namespace
 
@@ -1184,11 +1366,12 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
     }
     // scans round by round, so that every round's subsequences are contiguous
     std::vector<Round> rounds(nrounds);
-    std::vector<int> huff_l, dc_l, dcr_l, acr_l;
+    std::vector<int> huff_l, dc_l, dcr_l, acr_l, acrs_l;
+    int acr_cap = 0;  // blocks of the masks and records: the most any round needs
     for (int r = 0; r < nrounds; r++) {
         Round& R = rounds[r];
         R.sub_lo = (int)subs.size();
-        huff_l.clear(), dc_l.clear(), dcr_l.clear(), acr_l.clear();
+        huff_l.clear(), dc_l.clear(), dcr_l.clear(), acr_l.clear(), acrs_l.clear();
         for (int k = 0; k < m; k++) {
             const ScanHeader& M = H[idx[k]];
             if ((int)M.scans.size() <= r) continue;
@@ -1267,6 +1450,11 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             } else if (D.kind == SCAN_DC_REFINE) {
                 dcr_l.push_back(si);
                 R.dcr_blocks = std::max(R.dcr_blocks, D.nmcu * D.bpm);
+            } else {
+                acrs_l.push_back(si);
+                D.acr_off = R.acr_total;
+                R.acr_total += D.nmcu * D.bpm;
+                R.acr_blocks = std::max(R.acr_blocks, D.nmcu * D.bpm);
             }
             scans.push_back(D);
         }
@@ -1279,6 +1467,8 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
         put(dc_l, &R.dc_off, &R.ndc);
         put(dcr_l, &R.dcr_off, &R.ndcr);
         put(acr_l, &R.acr_off, &R.nacr);
+        put(acrs_l, &R.acrs_off, &R.nacrs);
+        acr_cap = std::max(acr_cap, R.acr_total);
     }
     const int nscan = (int)scans.size();
     int max_passes = 1;
@@ -1323,6 +1513,10 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
     JCK(grow(&ws->base, &ws->base_cap, nsub));
     JCK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
     JCK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
+    if (acr_cap) {
+        JCK(grow(&ws->acr_mask, &ws->acr_mask_cap, (size_t)acr_cap));
+        JCK(grow(&ws->acr_rec, &ws->acr_rec_cap, (size_t)acr_cap));
+    }
     JCK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
     if ((size_t)m + PASS_GROUP > ws->small_host_cap) {
         if (ws->small_host) cudaFreeHost(ws->small_host);
@@ -1393,10 +1587,14 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             ++*launches;
         }
         if (R.nacr) {
-            ac_refine_kernel<<<(R.nacr + 127) / 128, 128, 0, st>>>(d_img, d_scan, d_huff, d_list + R.acr_off, R.nacr, d_seg, ws->unst,
-                                                                 d_status, ws->coef);
+            const dim3 grid((R.acr_blocks + 255) / 256, R.nacrs);
+            acr_mask_kernel<<<grid, 256, 0, st>>>(d_img, d_scan, d_list + R.acrs_off, d_status, ws->coef, ws->acr_mask);
+            acr_decode_kernel<<<(R.nacr + ACR_WARPS - 1) / ACR_WARPS, 32 * ACR_WARPS, 0, st>>>(
+                d_scan, d_huff, d_list + R.acr_off, R.nacr, d_seg, ws->unst, d_status, ws->acr_mask, ws->acr_rec);
+            acr_apply_kernel<<<grid, 256, 0, st>>>(d_img, d_scan, d_list + R.acrs_off, d_status, ws->acr_mask, ws->acr_rec,
+                                                   ws->coef);
             JCK(cudaGetLastError());
-            ++*launches;
+            *launches += 3;
         }
     }
     idct_kernel<<<dim3((max_blocks + 127) / 128, m), 128, 0, st>>>(d_img, ws->coef, ws->planes, d_status);

@@ -237,7 +237,9 @@ class Engine:
     def decode_jpeg_ex(self, files, scans=True):
         """decode_jpeg for a batch that may also hold progressive Huffman files and sequential files with several scans
         (smapb_decode_jpeg_ex with SMAPB_JPEG_SCANS; scans=False is decode_jpeg).  -> per file a CUDA uint8 BGR [H,W,3]
-        tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None (cv2 must read it)."""
+        tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None (cv2 must read it).  Progressive files decode their AC
+        refinement scans sequentially within each restart segment (one warp per segment, the batch's images side by side),
+        so a batch takes about as long as its slowest image; run_inference sends the JPEGs decode_jpeg refuses here."""
         n = len(files)
         out = [None] * n
         if n == 0:

@@ -8,7 +8,8 @@ Same flags and the same output file name / schema as the reference ('{OUT}/stage
 test.py:147-152).  Differences, both deliberate: images are visited in sorted path order unless --glob_order 1 (the
 reference uses glob order, dataset/custom_dataset.py:16-18).  Decoding, resize, letterbox, normalisation, backbone,
 association, lift, RefineNet and the JSON text are produced by libsmap_b200.so: .jpg/.jpeg and .png files the GPU decoders
-support are decoded on the GPU (byte-identical to cv2.imread), every other file by cv2.imread as in the reference.
+support are decoded on the GPU (byte-identical to cv2.imread), every other file by cv2.imread as in the reference.  Baseline
+JPEGs go through Engine.decode_jpeg; progressive and multi-scan JPEGs through Engine.decode_jpeg_ex, in a batch of their own.
 """
 import argparse
 import glob
@@ -18,7 +19,7 @@ import os.path as osp
 import numpy as np
 import torch
 
-from .engine import PRECISIONS, RECORD_BYTES, Engine
+from .engine import PRECISIONS, RECORD_BYTES, Engine, jpeg_info
 from .results import ResultWriter, result_file_name
 
 
@@ -38,25 +39,35 @@ def image_name(path, dataset_path):
 
 
 def read_frames(eng, paths, imread):
-    """.jpg/.jpeg files through the GPU JPEG decoder and .png files through the GPU PNG decoder, one batch each; the rest,
-    and the files a decoder leaves to cv2, through imread."""
+    """.jpg/.jpeg files through the GPU JPEG decoder and .png files through the GPU PNG decoder, one batch each; the JPEGs
+    decode_jpeg leaves to cv2 that the multi-scan header walk accepts (progressive and multi-scan sequential files) through
+    decode_jpeg_ex, as one more batch, so baseline files never wait behind its rounds; the rest, and the files a decoder
+    leaves to cv2, through imread."""
     frames = [None] * len(paths)
-    for exts, decode in (((".jpg", ".jpeg"), eng.decode_jpeg), ((".png",), eng.decode_png)):
+    jpegs = {}
+    for exts, decode, jpeg in (((".jpg", ".jpeg"), eng.decode_jpeg, True), ((".png",), eng.decode_png, False)):
         sel = [i for i, p in enumerate(paths) if p.lower().endswith(exts)]
         if sel:
             files = []
             for i in sel:
                 with open(paths[i], "rb") as f:
                     files.append(f.read())
-            for i, im in zip(sel, decode(files)):
+            for i, b, im in zip(sel, files, decode(files)):
                 frames[i] = im
+                if jpeg:
+                    jpegs[i] = b
+    multi = [i for i, b in jpegs.items() if frames[i] is None and jpeg_info(b, scans=True)[0] == 0]
+    if multi:
+        for i, im in zip(multi, eng.decode_jpeg_ex([jpegs[i] for i in multi])):
+            frames[i] = im
     return [imread(p) if im is None else im for p, im in zip(paths, frames)]
 
 
 def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False, dataset_name="CMU",
         device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None):
     """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3], used for every file; by default .jpg/.jpeg
-    and .png files are decoded on the GPU (Engine.decode_jpeg / Engine.decode_png, byte-identical to cv2.imread) and the
+    and .png files are decoded on the GPU (Engine.decode_jpeg, then Engine.decode_jpeg_ex for the progressive and
+    multi-scan JPEGs decode_jpeg leaves, and Engine.decode_png; byte-identical to cv2.imread) and the
     files they do not handle, as every other file, go through cv2.imread(path, IMREAD_COLOR).  precision: one of engine.PRECISIONS.  stats (a dict,
     optional) receives "saturation": the fp16 clamp count."""
     if precision not in PRECISIONS:

@@ -5,10 +5,12 @@ photo-like entropy of roughly 1-2 bits per pixel) is decoded
   1. by Engine.decode_jpeg in batches of --batch (host parse, upload, every phase, status read-back: the whole call),
   2. by cv2.imdecode on one thread, and on a pool of all host cores,
 in images/s and Mpixel/s.  The same q90 4:2:0 frames written progressive by cv2 (libjpeg's default 10-scan script) are
-decoded by Engine.decode_jpeg_ex against cv2, with the share of kernel time that goes to the AC refinement scans (one
-thread per restart segment; these files have no restart markers) from torch.profiler.  Then the run_inference loop from file bytes to skeleton records (decode, preprocess, infer_device,
-records to the host) is timed in bf16x3 and fp16 with each decoder (cv2 on one thread is what the CLI did before).  The
-GPU's name and power limit are read in the same call.
+decoded by Engine.decode_jpeg_ex against cv2, with the share of kernel time that goes to the AC refinement scans (the
+history masks, one warp per restart segment decoding against them, and the apply pass; these files have no restart
+markers) from torch.profiler.  Then the run_inference loop from files on disk to skeleton records (decode, preprocess,
+infer_device, records to the host) is timed in bf16x3 and fp16, its GPU arm through run_inference.read_frames (the CLI's
+own routing: decode_jpeg, then decode_jpeg_ex for the progressive files) and its cv2 arm through cv2.imread on one thread
+(what the CLI did before).  The GPU's name, power limit and SM clock are read in the same call.
 
     python tools/decode_bench.py [--batch 8] [--rounds 5] [--json out/decode_bench.json]
 """
@@ -18,6 +20,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 from concurrent.futures import ThreadPoolExecutor
 
@@ -33,6 +36,7 @@ from jpeg_corpus import content, cv2_jpeg  # noqa: E402
 from jpeg_scans import cv2_progressive  # noqa: E402
 from smap_b200 import schema  # noqa: E402
 from smap_b200.engine import RECORD_BYTES, Engine  # noqa: E402
+from smap_b200.run_inference import read_frames  # noqa: E402
 
 
 def gpu_info():
@@ -56,7 +60,7 @@ def make_corpus(h, w, n, seed, progressive=False):
 
 
 def refine_share(eng, files):
-    """Share of the decode call's kernel time spent in ac_refine_kernel (torch.profiler, one call)."""
+    """Share of the decode call's kernel time spent in the AC refinement kernels (acr_*, torch.profiler, one call)."""
     from torch.profiler import ProfilerActivity, profile
 
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -67,7 +71,7 @@ def refine_share(eng, files):
         t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
         if "kernel" in e.key and "Memcpy" not in e.key and "Memset" not in e.key:
             tot += t
-            if "ac_refine_kernel" in e.key:
+            if "acr_mask_kernel" in e.key or "acr_decode_kernel" in e.key or "acr_apply_kernel" in e.key:
                 ref += t
     return round(ref / tot, 3) if tot else None
 
@@ -126,34 +130,42 @@ def main():
         row["sm_clock_mhz_after_gpu_arm"] = sm_clock()
         row["ac_refine_share_of_kernel_time"] = refine_share(eng, files)
         out["decode"][key] = row
-    # the CLI loop: bytes -> records, 4 batches of 1920x1080 frames per round
-    files = corpora["1920x1080"] * 4
-    prog = make_corpus(1080, 1920, B, 3, progressive=True) * 4
+    # the CLI loop: files -> records, 4 batches of 1920x1080 frames per round
+    tmp = tempfile.TemporaryDirectory()
+    paths = {}
+    for kind, fs in (("baseline", corpora["1920x1080"]), ("progressive", make_corpus(1080, 1920, B, 3, progressive=True))):
+        paths[kind] = []
+        for k, b in enumerate(fs * 4):
+            p = os.path.join(tmp.name, "%s_%02d.jpg" % (kind, k))
+            with open(p, "wb") as f:
+                f.write(b)
+            paths[kind].append(p)
     host = torch.empty(B, RECORD_BYTES, dtype=torch.uint8).pin_memory()
     sd = schema.make_state_dict(0, "identity")
+
+    def imread(p):
+        return cv2.imread(p, cv2.IMREAD_COLOR)
+
     for prec in ("bf16x3", "fp16"):
         eng.load_state_dict(sd, prec)
 
-        def loop(gpu_decode, files=files, decode=eng.decode_jpeg):
-            for lo in range(0, len(files), B):
-                chunk = files[lo:lo + B]
-                if gpu_decode:
-                    frames = decode(chunk)
-                else:
-                    frames = [torch.from_numpy(cv2_decode(f)) for f in chunk]
+        def loop(gpu_decode, ps):
+            for lo in range(0, len(ps), B):
+                chunk = ps[lo:lo + B]
+                frames = read_frames(eng, chunk, imread) if gpu_decode else [imread(p) for p in chunk]
+                frames = [f if torch.is_tensor(f) else torch.from_numpy(f) for f in frames]
                 imgs, scales = eng.preprocess(frames)
                 rec = eng.infer_device(imgs, scales.to(imgs.device))
                 host[:len(chunk)].copy_(rec)
                 torch.cuda.current_stream().synchronize()
 
         row = {}
-        for arm, flag in (("gpu_decode", True), ("cv2_1_thread", False)):
-            t = timed(lambda: loop(flag), a.rounds)
-            row[arm] = {"frames_per_s": round(len(files) / t, 1)}
-        for arm, flag in (("progressive_gpu_decode", True), ("progressive_cv2_1_thread", False)):
-            t = timed(lambda: loop(flag, prog, eng.decode_jpeg_ex), a.rounds)
-            row[arm] = {"frames_per_s": round(len(prog) / t, 1)}
+        for kind, prefix in (("baseline", ""), ("progressive", "progressive_")):
+            for arm, flag in (("gpu_decode", True), ("cv2_1_thread", False)):
+                t = timed(lambda: loop(flag, paths[kind]), a.rounds)
+                row[prefix + arm] = {"frames_per_s": round(len(paths[kind]) / t, 1)}
         out["cli"][prec] = row
+    tmp.cleanup()
     eng.close()
     pool.shutdown()
     line = json.dumps(out)
