@@ -22,7 +22,9 @@
  * Parity pin: the reference ships no golden vectors for this path.  This file
  * is pinned on the GPU box against oracle/_ref/dapalib (the UNMODIFIED
  * reference extension compiled from /root/reference/extensions by
- * oracle/build_ref.py) in tests/test_assoc_gpu.py.
+ * oracle/build_ref.py): through recorded digests in tests/test_assoc_gpu.py, and
+ * run live on the adversarial frames of tests/golden/assoc_adversary.py in
+ * tests/test_assoc_reference_gpu.py.
  */
 #include <math.h>
 #include <stdint.h>
@@ -46,6 +48,16 @@ static const float kBoneLength[NL] = {26.42178982f, 48.36980909f, 14.88291009f, 
                                       23.915707f,   14.97674918f, 31.28002549f, 23.91570732f,
                                       12.4644364f,  48.26604433f, 39.03553194f, 12.4644364f,
                                       48.19076948f, 39.03553252f};
+
+/* The NaN a GPU operation returns is always 0x7fffffff; x86 returns 0xffc00000 for an invalid operation.  Applied
+ * where the reference can compute a NaN that reaches its output: the centroid of a window holding +inf (inf / inf). */
+static float gpu_nan(float v) {
+    if (v != v) {
+        const uint32_t q = 0x7fffffffu;
+        memcpy(&v, &q, sizeof v);
+    }
+    return v;
+}
 
 /* ---------------------------------------------------------------- NMS ---- */
 /* peaks: [NJ][MAXP+1][3]; slot 0 = (count, -, -), slots 1..count = (x, y, score)
@@ -99,8 +111,8 @@ void oracle_nms(const float* hms, int h, int w, float threshold, float* peaks) {
                             }
                     }
                     float* o = out + (peakIndex + 1) * 3;
-                    o[0] = xAcc / sAcc + 0.5f; /* nmsBase.cu:124 */
-                    o[1] = yAcc / sAcc + 0.5f;
+                    o[0] = gpu_nan(xAcc / sAcc + 0.5f); /* nmsBase.cu:124 */
+                    o[1] = gpu_nan(yAcc / sAcc + 0.5f);
                     o[2] = src[py * w + px];
                 }
             }
@@ -111,6 +123,17 @@ void oracle_nms(const float* hms, int h, int w, float threshold, float* peaks) {
 }
 
 /* ---------------------------------------------------------------- PAF ---- */
+/* int(float) as the reference's device code converts it (cvt.rzi.s32.f32): truncation, saturated to the int range,
+ * NaN -> 0.  A plain C cast is undefined there (x86 gives INT_MIN), and it is reached: a 7x7 window holding +inf or
+ * values whose x * score overflows gives a peak at +inf or NaN, and the sample count and sample pixels of every pair
+ * involving it come from such conversions. */
+static int f2i_rz(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return INT32_MAX;
+    if (v <= -2147483648.0f) return INT32_MIN;
+    return (int)v;
+}
+
 /* bodyPartConnectorBase.cu:11-63 with T=float */
 static float paf_process(const float* a, const float* b, const float* mapX, const float* mapY, int w,
                          int h) {
@@ -118,7 +141,7 @@ static float paf_process(const float* a, const float* b, const float* mapX, cons
     const float dx = b[0] - a[0];
     const float dy = b[1] - a[1];
     const float dmax = fmaxf(fabsf(dx), fabsf(dy));
-    int n = (int)(sqrtf(5 * dmax) + 0.5f);
+    int n = f2i_rz(sqrtf(5 * dmax) + 0.5f);
     n = n < 25 ? n : 25;
     n = n > 5 ? n : 5;
     const float norm = sqrtf(fmaf(dx, dx, dy * dy));
@@ -129,8 +152,8 @@ static float paf_process(const float* a, const float* b, const float* mapX, cons
         int count = 0;
         const float stepX = dx / (float)n, stepY = dy / (float)n;
         for (int lm = 0; lm < n; lm++) {
-            int mX = (int)(fmaf((float)lm, stepX, sX) + 0.5f);
-            int mY = (int)(fmaf((float)lm, stepY, sY) + 0.5f);
+            int mX = f2i_rz(fmaf((float)lm, stepX, sX) + 0.5f);
+            int mY = f2i_rz(fmaf((float)lm, stepY, sY) + 0.5f);
             mX = mX < w - 1 ? mX : w - 1;
             mY = mY < h - 1 ? mY : h - 1;
             const int idx = mY * w + mX;
