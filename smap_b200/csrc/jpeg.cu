@@ -39,6 +39,7 @@
 #include <vector>
 
 #include "../../include/smap_b200.h"
+#include "decode_host.h"
 #include "jpeg.h"
 #include "orient.h"
 
@@ -1224,24 +1225,10 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict_
     o[0] = (uint8_t)b, o[1] = (uint8_t)g, o[2] = (uint8_t)r;
 }
 
-template <typename T>
-cudaError_t grow(T** p, size_t* cap, size_t n) {
-    if (n <= *cap) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    cudaError_t e = cudaMalloc((void**)p, n * sizeof(T));
-    if (e == cudaSuccess) *cap = n;
-    return e;
-}
-
 }  // namespace
 
-struct JpegWorkspace {
-    uint8_t* host = nullptr;  // pinned staging: descriptors + scan bytes, one upload per batch
-    size_t host_cap = 0;
-    uint8_t* dev_in = nullptr;  // device copy of the staging area
-    size_t dev_in_cap = 0;
+// staging: descriptors and scan bytes; small: status[m] then changed[passes]
+struct JpegWorkspace : DecodeBuffers {
     uint8_t* unst = nullptr;
     size_t unst_cap = 0;
     SubState* st[2] = {nullptr, nullptr};
@@ -1256,10 +1243,6 @@ struct JpegWorkspace {
     size_t acr_rec_cap = 0;
     uint8_t* planes = nullptr;
     size_t planes_cap = 0;
-    int* small = nullptr;  // status[n] then changed[passes]
-    size_t small_cap = 0;
-    int* small_host = nullptr;  // pinned
-    size_t small_host_cap = 0;
     int sub_bits = SUB_BITS;  // subsequence length of the Huffman passes (SMAPB_JPEG_SUB_BITS)
 };
 
@@ -1274,15 +1257,12 @@ JpegWorkspace* jpeg_workspace_create() {
 
 void jpeg_workspace_destroy(JpegWorkspace* ws) {
     if (!ws) return;
-    if (ws->host) cudaFreeHost(ws->host);
-    if (ws->small_host) cudaFreeHost(ws->small_host);
-    void* d[] = {ws->dev_in, ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->acr_mask, ws->acr_rec, ws->planes, ws->small};
+    free_decode_buffers(ws);
+    void* d[] = {ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->acr_mask, ws->acr_rec, ws->planes};
     for (void* p : d)
         if (p) cudaFree(p);
     delete ws;
 }
-
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 namespace {
 // What one round (the r-th scan of every image that has one) launches: subsequences [sub_lo, sub_lo + nsub) of its
@@ -1297,39 +1277,12 @@ struct Round {
 
 int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int64_t* nbytes, uint8_t* const* bgr, int flags,
                 int* status, cudaStream_t st, int64_t* launches, std::string* err) {
-#define JCK(call)                                                                                             \
-    do {                                                                                                      \
-        cudaError_t e_ = (call);                                                                              \
-        if (e_ != cudaSuccess) {                                                                              \
-            *err = std::string(#call) + ": " + cudaGetErrorString(e_) + " @jpeg.cu:" + std::to_string(__LINE__); \
-            return -10;                                                                                       \
-        }                                                                                                     \
-    } while (0)
-    if (n < 0 || (n > 0 && (!jpeg || !nbytes || !bgr || !status))) {
-        *err = "smapb_decode_jpeg_ex: null argument";
-        return -1;
-    }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    JCK(cudaStreamIsCapturing(st, &cap));
-    if (cap != cudaStreamCaptureStatusNone) {
-        *err = "smapb_decode_jpeg_ex: not capturable (it synchronises and may grow its workspace)";
-        return -1;
-    }
     // host: parse, then lay out descriptors and scan bytes
-    std::vector<ScanHeader> H(n);
+    std::vector<ScanHeader> H;
     std::vector<int> idx;  // images that go to the device
-    for (int i = 0; i < n; i++) {
-        status[i] = jpeg ? jpeg_parse(jpeg[i], nbytes[i], flags, &H[i]) : SMAPB_JPEG_MALFORMED;
-        if (status[i] == SMAPB_JPEG_OK) {
-            if (!bgr[i]) {
-                *err = "smapb_decode_jpeg_ex: no output buffer for decodable image " + std::to_string(i);
-                return -1;
-            }
-            idx.push_back(i);
-        }
-    }
-    const int m = (int)idx.size();
-    if (m == 0) return 0;
+    const auto walk = [flags](const uint8_t* d, int64_t nb, ScanHeader* M) { return jpeg_parse(d, nb, flags, M); };
+    const int m = decode_preamble("smapb_decode_jpeg_ex", n, jpeg, nbytes, bgr, status, st, walk, &H, &idx, err);
+    if (m <= 0) return m;
     std::vector<DevImage> imgs(m);
     std::vector<DevScan> scans;
     std::vector<DevHuff> huffs;
@@ -1480,14 +1433,8 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
                  o_sub = align_up(o_seg + sizeof(DevSeg) * segs.size(), 256),
                  o_list = align_up(o_sub + sizeof(DevSub) * subs.size(), 256),
                  o_raw = align_up(o_list + sizeof(int) * lists.size(), 256), total = o_raw + raw_total;
-    if (total > ws->host_cap) {
-        if (ws->host) cudaFreeHost(ws->host);
-        ws->host = nullptr;
-        ws->host_cap = 0;
-        JCK(cudaMallocHost((void**)&ws->host, total));
-        ws->host_cap = total;
-    }
-    JCK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
+    DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total));
+    DECODE_CK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
     memcpy(ws->host + o_img, imgs.data(), sizeof(DevImage) * m);
     memcpy(ws->host + o_scan, scans.data(), sizeof(DevScan) * nscan);
     memcpy(ws->host + o_huff, huffs.data(), sizeof(DevHuff) * huffs.size());
@@ -1506,25 +1453,19 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             }
     }
     const size_t nsub = std::max<size_t>(1, subs.size());
-    JCK(grow(&ws->dev_in, &ws->dev_in_cap, total));
-    JCK(grow(&ws->unst, &ws->unst_cap, (size_t)unst_total));
-    JCK(grow(&ws->st[0], &ws->st_cap[0], nsub));
-    JCK(grow(&ws->st[1], &ws->st_cap[1], nsub));
-    JCK(grow(&ws->base, &ws->base_cap, nsub));
-    JCK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
-    JCK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
+    DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total));
+    DECODE_CK(grow(&ws->unst, &ws->unst_cap, (size_t)unst_total));
+    DECODE_CK(grow(&ws->st[0], &ws->st_cap[0], nsub));
+    DECODE_CK(grow(&ws->st[1], &ws->st_cap[1], nsub));
+    DECODE_CK(grow(&ws->base, &ws->base_cap, nsub));
+    DECODE_CK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
+    DECODE_CK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
     if (acr_cap) {
-        JCK(grow(&ws->acr_mask, &ws->acr_mask_cap, (size_t)acr_cap));
-        JCK(grow(&ws->acr_rec, &ws->acr_rec_cap, (size_t)acr_cap));
+        DECODE_CK(grow(&ws->acr_mask, &ws->acr_mask_cap, (size_t)acr_cap));
+        DECODE_CK(grow(&ws->acr_rec, &ws->acr_rec_cap, (size_t)acr_cap));
     }
-    JCK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
-    if ((size_t)m + PASS_GROUP > ws->small_host_cap) {
-        if (ws->small_host) cudaFreeHost(ws->small_host);
-        ws->small_host = nullptr;
-        ws->small_host_cap = 0;
-        JCK(cudaMallocHost((void**)&ws->small_host, sizeof(int) * (m + PASS_GROUP)));
-        ws->small_host_cap = m + PASS_GROUP;
-    }
+    DECODE_CK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
+    DECODE_CK(grow_pinned(&ws->small_host, &ws->small_host_cap, (size_t)m + PASS_GROUP));
     const DevImage* d_img = (const DevImage*)(ws->dev_in + o_img);
     const DevScan* d_scan = (const DevScan*)(ws->dev_in + o_scan);
     const DevHuff* d_huff = (const DevHuff*)(ws->dev_in + o_huff);
@@ -1535,15 +1476,15 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
     int* d_status = ws->small;
     int* d_changed = ws->small + m;
     for (int k = 0; k < m; k++) ws->small_host[k] = status[idx[k]];
-    JCK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
-    JCK(cudaMemcpyAsync(d_status, ws->small_host, sizeof(int) * m, cudaMemcpyHostToDevice, st));
-    JCK(cudaMemsetAsync(ws->coef, 0, (size_t)coef_blocks * 64 * sizeof(int16_t), st));
+    DECODE_CK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
+    DECODE_CK(cudaMemcpyAsync(d_status, ws->small_host, sizeof(int) * m, cudaMemcpyHostToDevice, st));
+    DECODE_CK(cudaMemsetAsync(ws->coef, 0, (size_t)coef_blocks * 64 * sizeof(int16_t), st));
     unstuff_kernel<<<nscan, 1024, 0, st>>>(d_scan, d_raw, ws->unst);
-    JCK(cudaGetLastError());
+    DECODE_CK(cudaGetLastError());
     ++*launches;
     for (const Round& R : rounds) {
         if (R.nsub) {
-            JCK(cudaMemsetAsync(d_changed, 0, sizeof(int) * (max_passes + PASS_GROUP), st));
+            DECODE_CK(cudaMemsetAsync(d_changed, 0, sizeof(int) * (max_passes + PASS_GROUP), st));
             const int round_passes = R.max_nsub_seg + 1;
             const int sgrid = (R.nsub + 255) / 256;
             int pass = 0, final_pass = -1;
@@ -1553,11 +1494,12 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
                 for (; pass < stop; pass++) {
                     scan_sync_kernel<<<sgrid, 256, 0, st>>>(d_img, d_scan, d_huff, d_seg, d_sub, R.sub_lo, R.nsub, ws->unst,
                                                             ws->st[(pass + 1) & 1], ws->st[pass & 1], d_changed, pass);
-                    JCK(cudaGetLastError());
+                    DECODE_CK(cudaGetLastError());
                     ++*launches;
                 }
-                JCK(cudaMemcpyAsync(ws->small_host, d_changed + first, sizeof(int) * (stop - first), cudaMemcpyDeviceToHost, st));
-                JCK(cudaStreamSynchronize(st));
+                DECODE_CK(cudaMemcpyAsync(ws->small_host, d_changed + first, sizeof(int) * (stop - first), cudaMemcpyDeviceToHost,
+                                          st));
+                DECODE_CK(cudaStreamSynchronize(st));
                 for (int p = first; p < stop; p++)
                     if (p > 0 && ws->small_host[p - first] == 0) {
                         final_pass = p;
@@ -1572,18 +1514,18 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             scan_prefix_kernel<<<R.nhuff, 1024, 0, st>>>(d_scan, d_list + R.huff_off, d_seg, d_sub, fin, ws->base, d_status);
             scan_write_kernel<<<sgrid, 256, 0, st>>>(d_img, d_scan, d_huff, d_seg, d_sub, R.sub_lo, R.nsub, ws->unst, fin, ws->base,
                                                      d_status, ws->coef);
-            JCK(cudaGetLastError());
+            DECODE_CK(cudaGetLastError());
             *launches += 2;
         }
         if (R.ndc) {
             scan_dc_kernel<<<dim3(R.ndc, 3), 1024, 0, st>>>(d_img, d_scan, d_list + R.dc_off, d_status, ws->coef);
-            JCK(cudaGetLastError());
+            DECODE_CK(cudaGetLastError());
             ++*launches;
         }
         if (R.ndcr) {
             dc_refine_kernel<<<dim3((R.dcr_blocks + 255) / 256, R.ndcr), 256, 0, st>>>(d_img, d_scan, d_list + R.dcr_off, d_seg,
                                                                                        ws->unst, d_status, ws->coef);
-            JCK(cudaGetLastError());
+            DECODE_CK(cudaGetLastError());
             ++*launches;
         }
         if (R.nacr) {
@@ -1593,20 +1535,19 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
                 d_scan, d_huff, d_list + R.acr_off, R.nacr, d_seg, ws->unst, d_status, ws->acr_mask, ws->acr_rec);
             acr_apply_kernel<<<grid, 256, 0, st>>>(d_img, d_scan, d_list + R.acrs_off, d_status, ws->acr_mask, ws->acr_rec,
                                                    ws->coef);
-            JCK(cudaGetLastError());
+            DECODE_CK(cudaGetLastError());
             *launches += 3;
         }
     }
     idct_kernel<<<dim3((max_blocks + 127) / 128, m), 128, 0, st>>>(d_img, ws->coef, ws->planes, d_status);
     colour_kernel<<<dim3((unsigned)((max_px + 255) / 256), m), 256, 0, st>>>(d_img, ws->planes, d_status);
-    JCK(cudaGetLastError());
+    DECODE_CK(cudaGetLastError());
     *launches += 2;
-    JCK(cudaMemcpyAsync(ws->small_host, d_status, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
-    JCK(cudaStreamSynchronize(st));
+    DECODE_CK(cudaMemcpyAsync(ws->small_host, d_status, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
+    DECODE_CK(cudaStreamSynchronize(st));
     for (int k = 0; k < m; k++)
         if (status[idx[k]] == SMAPB_JPEG_OK) status[idx[k]] = ws->small_host[k];
     return 0;
-#undef JCK
 }
 
 }  // namespace smapb
@@ -1616,13 +1557,7 @@ extern "C" {
 int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status) {
     if (!status || (flags & ~SMAPB_JPEG_SCANS)) return -1;
     smapb::ScanHeader M;
-    *status = smapb::jpeg_parse(data, nbytes, flags, &M);
-    const smapb::Header& H = M.f;
-    const bool ok = *status == SMAPB_JPEG_OK;
-    if (h) *h = ok ? H.out_h : 0;
-    if (w) *w = ok ? H.out_w : 0;
-    if (orientation) *orientation = ok ? H.orientation : 0;
-    return 0;
+    return smapb::report_info(smapb::jpeg_parse(data, nbytes, flags, &M), M.f, status, h, w, orientation);
 }
 
 int smapb_jpeg_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* orientation, int* status) {

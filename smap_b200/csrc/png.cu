@@ -41,6 +41,7 @@
 #include <vector>
 
 #include "../../include/smap_b200.h"
+#include "decode_host.h"
 #include "orient.h"
 #include "png.h"
 
@@ -842,26 +843,10 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevPng* __restrict__ 
     o[0] = (uint8_t)b, o[1] = (uint8_t)g, o[2] = (uint8_t)r;
 }
 
-template <typename T>
-cudaError_t grow(T** p, size_t* cap, size_t n) {
-    if (n <= *cap) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    cudaError_t e = cudaMalloc((void**)p, n * sizeof(T));
-    if (e == cudaSuccess) *cap = n;
-    return e;
-}
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 }  // namespace
 
-struct PngWorkspace {
-    uint8_t* host = nullptr;  // pinned staging: descriptors + IDAT regions, one upload per batch
-    size_t host_cap = 0;
-    uint8_t* dev_in = nullptr;
-    size_t dev_in_cap = 0;
+// staging: descriptors and IDAT regions; small: stats[4] | status[m] | nblk[m] | adler[m]
+struct PngWorkspace : DecodeBuffers {
     uint8_t* stream = nullptr;
     size_t stream_cap = 0;
     unsigned long long* cand = nullptr;
@@ -878,10 +863,6 @@ struct PngWorkspace {
     size_t marks_cap = 0;
     uint8_t* raw = nullptr;
     size_t raw_cap = 0;
-    int* small = nullptr;  // stats[4] | status[m] | nblk[m] | adler[m]
-    size_t small_cap = 0;
-    int* small_host = nullptr;  // pinned
-    size_t small_host_cap = 0;
     int64_t stats[4] = {0, 0, 0, 0};
 };
 
@@ -889,9 +870,8 @@ PngWorkspace* png_workspace_create() { return new PngWorkspace(); }
 
 void png_workspace_destroy(PngWorkspace* ws) {
     if (!ws) return;
-    if (ws->host) cudaFreeHost(ws->host);
-    if (ws->small_host) cudaFreeHost(ws->small_host);
-    void* d[] = {ws->dev_in, ws->stream, ws->cand, ws->res, ws->hkey, ws->hval, ws->blocks, ws->marks, ws->raw, ws->small};
+    free_decode_buffers(ws);
+    void* d[] = {ws->stream, ws->cand, ws->res, ws->hkey, ws->hval, ws->blocks, ws->marks, ws->raw};
     for (void* p : d)
         if (p) cudaFree(p);
     delete ws;
@@ -903,39 +883,11 @@ void png_last_stats(const PngWorkspace* ws, int64_t out[4]) {
 
 int png_decode(PngWorkspace* ws, int n, const uint8_t* const* png, const int64_t* nbytes, uint8_t* const* bgr, int* status,
                cudaStream_t st, int64_t* launches, std::string* err) {
-#define PCK(call)                                                                                            \
-    do {                                                                                                     \
-        cudaError_t e_ = (call);                                                                             \
-        if (e_ != cudaSuccess) {                                                                             \
-            *err = std::string(#call) + ": " + cudaGetErrorString(e_) + " @png.cu:" + std::to_string(__LINE__); \
-            return -10;                                                                                      \
-        }                                                                                                    \
-    } while (0)
-    if (n < 0 || (n > 0 && (!png || !nbytes || !bgr || !status))) {
-        *err = "smapb_decode_png: null argument";
-        return -1;
-    }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    PCK(cudaStreamIsCapturing(st, &cap));
-    if (cap != cudaStreamCaptureStatusNone) {
-        *err = "smapb_decode_png: not capturable (it synchronises and may grow its workspace)";
-        return -1;
-    }
     for (int i = 0; i < 4; i++) ws->stats[i] = 0;
-    std::vector<PngHeader> H(n);
+    std::vector<PngHeader> H;
     std::vector<int> idx;
-    for (int i = 0; i < n; i++) {
-        status[i] = png_parse(png[i], nbytes[i], &H[i]);
-        if (status[i] == SMAPB_JPEG_OK) {
-            if (!bgr[i]) {
-                *err = "smapb_decode_png: no output buffer for decodable image " + std::to_string(i);
-                return -1;
-            }
-            idx.push_back(i);
-        }
-    }
-    const int m = (int)idx.size();
-    if (m == 0) return 0;
+    const int m = decode_preamble("smapb_decode_png", n, png, nbytes, bgr, status, st, png_parse, &H, &idx, err);
+    if (m <= 0) return m;
     std::vector<DevPng> imgs(m);
     std::vector<DevChunk> chunks;
     int64_t in_total = 0, z_total = 0, raw_total = 0, blk_total = 0, max_px = 0;
@@ -994,35 +946,23 @@ int png_decode(PngWorkspace* ws, int n, const uint8_t* const* png, const int64_t
     // staging layout: images | chunks | IDAT regions
     const size_t o_img = 0, o_chunk = align_up(sizeof(DevPng) * m, 256), o_in = align_up(o_chunk + sizeof(DevChunk) * chunks.size(), 256),
                  total = o_in + in_total;
-    if (total > ws->host_cap) {
-        if (ws->host) cudaFreeHost(ws->host);
-        ws->host = nullptr;
-        ws->host_cap = 0;
-        PCK(cudaMallocHost((void**)&ws->host, total));
-        ws->host_cap = total;
-    }
-    PCK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
+    DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total));
+    DECODE_CK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
     memcpy(ws->host + o_img, imgs.data(), sizeof(DevPng) * m);
     memcpy(ws->host + o_chunk, chunks.data(), sizeof(DevChunk) * chunks.size());
     for (int k = 0; k < m; k++) memcpy(ws->host + o_in + in_off[k], png[idx[k]] + H[idx[k]].idat.front(), in_len[k]);
     const size_t nsmall = 4 + 3 * (size_t)m;
-    PCK(grow(&ws->dev_in, &ws->dev_in_cap, total));
-    PCK(grow(&ws->stream, &ws->stream_cap, (size_t)z_total));
-    PCK(grow(&ws->cand, &ws->cand_cap, (size_t)cand_cap));
-    PCK(grow(&ws->res, &ws->res_cap, (size_t)cand_cap));
-    PCK(grow(&ws->hkey, &ws->hkey_cap, (size_t)hsize));
-    PCK(grow(&ws->hval, &ws->hval_cap, (size_t)hsize));
-    PCK(grow(&ws->blocks, &ws->blocks_cap, (size_t)blk_total));
-    PCK(grow(&ws->marks, &ws->marks_cap, (size_t)raw_total));
-    PCK(grow(&ws->raw, &ws->raw_cap, (size_t)raw_total));
-    PCK(grow(&ws->small, &ws->small_cap, nsmall));
-    if (nsmall > ws->small_host_cap) {
-        if (ws->small_host) cudaFreeHost(ws->small_host);
-        ws->small_host = nullptr;
-        ws->small_host_cap = 0;
-        PCK(cudaMallocHost((void**)&ws->small_host, sizeof(int) * nsmall));
-        ws->small_host_cap = nsmall;
-    }
+    DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total));
+    DECODE_CK(grow(&ws->stream, &ws->stream_cap, (size_t)z_total));
+    DECODE_CK(grow(&ws->cand, &ws->cand_cap, (size_t)cand_cap));
+    DECODE_CK(grow(&ws->res, &ws->res_cap, (size_t)cand_cap));
+    DECODE_CK(grow(&ws->hkey, &ws->hkey_cap, (size_t)hsize));
+    DECODE_CK(grow(&ws->hval, &ws->hval_cap, (size_t)hsize));
+    DECODE_CK(grow(&ws->blocks, &ws->blocks_cap, (size_t)blk_total));
+    DECODE_CK(grow(&ws->marks, &ws->marks_cap, (size_t)raw_total));
+    DECODE_CK(grow(&ws->raw, &ws->raw_cap, (size_t)raw_total));
+    DECODE_CK(grow(&ws->small, &ws->small_cap, nsmall));
+    DECODE_CK(grow_pinned(&ws->small_host, &ws->small_host_cap, nsmall));
     const DevPng* d_img = (const DevPng*)(ws->dev_in + o_img);
     const DevChunk* d_chunk = (const DevChunk*)(ws->dev_in + o_chunk);
     const uint8_t* d_in = ws->dev_in + o_in;
@@ -1033,19 +973,19 @@ int png_decode(PngWorkspace* ws, int n, const uint8_t* const* png, const int64_t
     int* hs = ws->small_host;
     for (int i = 0; i < 4; i++) hs[i] = 0;
     for (int k = 0; k < m; k++) hs[4 + k] = SMAPB_JPEG_OK;
-    PCK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(ws->small, hs, sizeof(int) * (4 + m), cudaMemcpyHostToDevice, st));
-    PCK(cudaMemsetAsync(ws->hkey, 0, sizeof(unsigned long long) * hsize, st));
+    DECODE_CK(cudaMemcpyAsync(ws->dev_in, ws->host, total, cudaMemcpyHostToDevice, st));
+    DECODE_CK(cudaMemcpyAsync(ws->small, hs, sizeof(int) * (4 + m), cudaMemcpyHostToDevice, st));
+    DECODE_CK(cudaMemsetAsync(ws->hkey, 0, sizeof(unsigned long long) * hsize, st));
     gather_kernel<<<m, GATHER_THREADS, 0, st>>>(d_img, d_chunk, d_in, ws->stream, d_status);
     find_kernel<<<dim3((max_zbits + 255) / 256, m), 256, 0, st>>>(d_img, ws->stream, d_status, ws->cand, cand_cap, ws->hkey, ws->hval,
                                                                   hsize - 1, d_stats);
     count_kernel<<<(cand_cap + 63) / 64, 64, 0, st>>>(d_img, ws->stream, ws->cand, d_stats, cand_cap, ws->res);
     chain_kernel<<<(m + 31) / 32, 32, 0, st>>>(d_img, m, ws->stream, ws->hkey, ws->hval, hsize - 1, ws->res, ws->blocks, d_nblk,
                                                d_adler, d_status, d_stats);
-    PCK(cudaGetLastError());
+    DECODE_CK(cudaGetLastError());
     *launches += 4;
-    PCK(cudaMemcpyAsync(hs + 4 + m, d_nblk, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
-    PCK(cudaStreamSynchronize(st));
+    DECODE_CK(cudaMemcpyAsync(hs + 4 + m, d_nblk, sizeof(int) * m, cudaMemcpyDeviceToHost, st));
+    DECODE_CK(cudaStreamSynchronize(st));
     int max_blk = 0;
     for (int k = 0; k < m; k++) max_blk = std::max(max_blk, hs[4 + m + k]);
     if (max_blk > 0) {
@@ -1053,18 +993,17 @@ int png_decode(PngWorkspace* ws, int n, const uint8_t* const* png, const int64_t
         resolve_kernel<<<m, RESOLVE_THREADS, 0, st>>>(d_img, ws->blocks, d_nblk, ws->marks, ws->raw, d_adler, d_status);
         unfilter_kernel<<<dim3(7, m), UNFILTER_THREADS, 0, st>>>(d_img, ws->raw, d_status);
         colour_kernel<<<dim3((unsigned)((max_px + 255) / 256), m), 256, 0, st>>>(d_img, ws->raw, d_status);
-        PCK(cudaGetLastError());
+        DECODE_CK(cudaGetLastError());
         *launches += 4;
     }
-    PCK(cudaMemcpyAsync(hs, ws->small, sizeof(int) * (4 + m), cudaMemcpyDeviceToHost, st));
-    PCK(cudaStreamSynchronize(st));
+    DECODE_CK(cudaMemcpyAsync(hs, ws->small, sizeof(int) * (4 + m), cudaMemcpyDeviceToHost, st));
+    DECODE_CK(cudaStreamSynchronize(st));
     ws->stats[0] = hs[ST_CAND];
     ws->stats[1] = hs[ST_CAND] - hs[ST_ONCHAIN];
     ws->stats[2] = hs[ST_CONFIRMED];
     ws->stats[3] = hs[ST_SERIAL];
     for (int k = 0; k < m; k++) status[idx[k]] = hs[4 + k];
     return 0;
-#undef PCK
 }
 
 }  // namespace smapb
@@ -1074,12 +1013,7 @@ extern "C" {
 int smapb_png_info(const uint8_t* data, int64_t nbytes, int* h, int* w, int* orientation, int* status) {
     if (!status) return -1;
     smapb::PngHeader H;
-    *status = smapb::png_parse(data, nbytes, &H);
-    const bool ok = *status == SMAPB_JPEG_OK;
-    if (h) *h = ok ? H.out_h : 0;
-    if (w) *w = ok ? H.out_w : 0;
-    if (orientation) *orientation = ok ? H.orientation : 0;
-    return 0;
+    return smapb::report_info(smapb::png_parse(data, nbytes, &H), H, status, h, w, orientation);
 }
 #pragma GCC visibility pop
 }

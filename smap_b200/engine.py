@@ -62,30 +62,27 @@ def get_tile_table():
 JPEG_SCANS = 1  # SMAPB_JPEG_SCANS
 
 
+def _header_info(fn, data, *flags):
+    """fn(data, nbytes, *flags, &h, &w, &orientation, &status), a header-only info entry point -> (status, h, w,
+    orientation)."""
+    h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    rc = fn(bytes(data), len(data), *flags, ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
+    if rc != 0:
+        raise SmapB200Error("%s failed (%d)" % (fn.__name__, rc))
+    return st.value, h.value, w.value, o.value
+
+
 def jpeg_info(data, scans=False):
     """Header walk of one JPEG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
     handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h).
     scans=True: the walk of Engine.decode_jpeg_ex, which also takes multi-scan sequential and progressive files."""
-    h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    lib = _lib.load()
-    if scans:
-        rc = lib.smapb_jpeg_info_ex(bytes(data), len(data), JPEG_SCANS, ctypes.byref(h), ctypes.byref(w), ctypes.byref(o),
-                                    ctypes.byref(st))
-    else:
-        rc = lib.smapb_jpeg_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
-    if rc != 0:
-        raise SmapB200Error("%s failed (%d)" % ("smapb_jpeg_info_ex" if scans else "smapb_jpeg_info", rc))
-    return st.value, h.value, w.value, o.value
+    return _header_info(_lib.load().smapb_jpeg_info_ex, data, JPEG_SCANS if scans else 0)
 
 
 def png_info(data):
     """Chunk walk of one PNG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
     handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h)."""
-    h, w, o, st = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    rc = _lib.load().smapb_png_info(bytes(data), len(data), ctypes.byref(h), ctypes.byref(w), ctypes.byref(o), ctypes.byref(st))
-    if rc != 0:
-        raise SmapB200Error("smapb_png_info failed (%d)" % rc)
-    return st.value, h.value, w.value, o.value
+    return _header_info(_lib.load().smapb_png_info, data)
 
 
 class Engine:
@@ -214,25 +211,30 @@ class Engine:
                                              _ptr(rdp), _ptr(co), self._st()), "smapb_lift3d_gt")
         return p2, p3, rdp, co
 
-    # ---- JPEG decoding -------------------------------------------------------------------------
-    def decode_jpeg(self, files):
-        """files: list of bytes (whole JPEG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
-        cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
+    # ---- image decoding ------------------------------------------------------------------------
+    def _decode(self, files, info, fn, *flags):
+        """Output tensors sized by info(file) -> (status, h, w, orientation), then one batch call fn(handle, n, files,
+        sizes, outputs, *flags, status, stream) -> per file the tensor, or None where the status is not 0."""
         n = len(files)
         out = [None] * n
         if n == 0:
             return out
         ptrs = (ctypes.c_void_p * n)()
         for i, f in enumerate(files):
-            st, h, w = jpeg_info(f)[:3]
+            st, h, w = info(f)[:3]
             if st == 0:
                 out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
                 ptrs[i] = out[i].data_ptr()
         data = (ctypes.c_char_p * n)(*files)
         sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
         status = (ctypes.c_int * n)()
-        self._check(self.lib.smapb_decode_jpeg(self._h, n, data, sizes, ptrs, status, self._st()), "smapb_decode_jpeg")
+        self._check(fn(self._h, n, data, sizes, ptrs, *flags, status, self._st()), fn.__name__)
         return [o if status[i] == 0 else None for i, o in enumerate(out)]
+
+    def decode_jpeg(self, files):
+        """files: list of bytes (whole JPEG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
+        cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
+        return self._decode(files, jpeg_info, self.lib.smapb_decode_jpeg)
 
     def decode_jpeg_ex(self, files, scans=True):
         """decode_jpeg for a batch that may also hold progressive Huffman files and sequential files with several scans
@@ -240,43 +242,12 @@ class Engine:
         tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None (cv2 must read it).  Progressive files decode their AC
         refinement scans sequentially within each restart segment (one warp per segment, the batch's images side by side),
         so a batch takes about as long as its slowest image; run_inference sends the JPEGs decode_jpeg refuses here."""
-        n = len(files)
-        out = [None] * n
-        if n == 0:
-            return out
-        ptrs = (ctypes.c_void_p * n)()
-        for i, f in enumerate(files):
-            st, h, w = jpeg_info(f, scans)[:3]
-            if st == 0:
-                out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
-                ptrs[i] = out[i].data_ptr()
-        data = (ctypes.c_char_p * n)(*files)
-        sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
-        status = (ctypes.c_int * n)()
-        flags = JPEG_SCANS if scans else 0
-        self._check(self.lib.smapb_decode_jpeg_ex(self._h, n, data, sizes, ptrs, flags, status, self._st()),
-                    "smapb_decode_jpeg_ex")
-        return [o if status[i] == 0 else None for i, o in enumerate(out)]
+        return self._decode(files, lambda f: jpeg_info(f, scans), self.lib.smapb_decode_jpeg_ex, JPEG_SCANS if scans else 0)
 
-    # ---- PNG decoding --------------------------------------------------------------------------
     def decode_png(self, files):
         """files: list of bytes (whole PNG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
         cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
-        n = len(files)
-        out = [None] * n
-        if n == 0:
-            return out
-        ptrs = (ctypes.c_void_p * n)()
-        for i, f in enumerate(files):
-            st, h, w = png_info(f)[:3]
-            if st == 0:
-                out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=self.device)
-                ptrs[i] = out[i].data_ptr()
-        data = (ctypes.c_char_p * n)(*files)
-        sizes = (ctypes.c_int64 * n)(*[len(f) for f in files])
-        status = (ctypes.c_int * n)()
-        self._check(self.lib.smapb_decode_png(self._h, n, data, sizes, ptrs, status, self._st()), "smapb_decode_png")
-        return [o if status[i] == 0 else None for i, o in enumerate(out)]
+        return self._decode(files, png_info, self.lib.smapb_decode_png)
 
     def png_stats(self):
         """Inflate counters of the last decode_png call (smapb_png_inflate_stats): dict with candidates, false_positives,
