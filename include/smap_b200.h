@@ -104,6 +104,16 @@ int smapb_decode_jpeg(smapb_handle* h, int n, const uint8_t* const* jpeg_host, c
  * AC refinement scans decode sequentially within a restart segment (a block's bits depend on its coefficients' history),
  * one warp per segment against per-block history masks; the segments, and the images of a batch, run side by side. */
 #define SMAPB_JPEG_SCANS 1
+/* SMAPB_JPEG_COLOUR (alone or with SMAPB_JPEG_SCANS) also accepts the frames libjpeg reads that the plain forms leave to
+ * cv2 for their colour space or sampling: 4 components (CMYK, or YCCK when an Adobe APP14 says transform 2; other Adobe
+ * transforms are left to cv2), 3 components libjpeg treats as RGB (an Adobe transform of 0 without JFIF, or ids 'R','G','B'
+ * without either marker), and every sampling with factors H, V in 1..4 whose ratios to the frame's largest factors are
+ * integral (4:1:1, 4:1:0, factors of 3, chroma finer than luma, Pillow's CMYK with the factors on C) and at most 10 blocks
+ * per MCU.  Each component is upsampled as libjpeg-turbo 3.x does it (fancy h2v1 / h1v2 / h2v2 where a factor is halved,
+ * replication for other ratios); RGB is reordered to BGR, and CMYK (YCCK first converted to CMYK with the YCbCr tables)
+ * goes through cv2's CMYK -> BGR, out = K - ((255 - ink) * K >> 8).  Still left to cv2: fractional sampling ratios, frames
+ * over 10 blocks per MCU, 2-component frames, arithmetic coding, 12-bit and lossless files. */
+#define SMAPB_JPEG_COLOUR 2
 int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status);
 int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
                          int flags, int* status_host, void* stream);

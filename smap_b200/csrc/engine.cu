@@ -403,7 +403,7 @@ int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, i
 int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host, const int64_t* nbytes, uint8_t* const* bgr_dev,
                          int flags, int* status_host, void* stream) {
     if (!h) return -1;
-    if (flags & ~SMAPB_JPEG_SCANS) {
+    if (flags & ~(SMAPB_JPEG_SCANS | SMAPB_JPEG_COLOUR)) {
         h->err = "smapb_decode_jpeg_ex: unknown flags";
         return -1;
     }

@@ -30,8 +30,10 @@
 //                         block its correction bits and new coefficients; the warp takes long EOB runs 32 blocks a step
 //      acr_apply_kernel   corrections and new coefficients into the blocks, one thread per block
 //   c. idct_kernel        dequantisation + accurate-integer IDCT (LL&M, 13-bit constants, 2 pass-1 bits), saturated
-//   d. colour_kernel      fancy upsampling, fixed-point YCbCr -> BGR, EXIF orientation, uint8 HWC BGR
-// oracle/jpeg_numpy.py restates every stage on the CPU, oracle/jpeg_scans_numpy.py the multi-scan entropy decoding.
+//   d. colour_kernel      per-component upsampling (libjpeg-turbo's choice of method), the colour conversion of the
+//                         frame's colour space (grayscale, YCbCr, RGB, CMYK, YCCK) to BGR, EXIF orientation, uint8 HWC BGR
+// oracle/jpeg_numpy.py restates every stage on the CPU, oracle/jpeg_scans_numpy.py the multi-scan entropy decoding,
+// oracle/jpeg_colour_numpy.py the frames SMAPB_JPEG_COLOUR adds.
 #include <stdlib.h>
 #include <string.h>
 
@@ -66,14 +68,21 @@ struct DevHuff {
     uint8_t vals[256];
 };
 
+constexpr int MAX_COMPS = 4;   // components of a frame
+constexpr int MAX_BLOCKS = 10;  // blocks of a frame's MCU (libjpeg's D_MAX_BLOCKS_IN_MCU)
+
+// Colour space of the component planes (libjpeg's jpeg_color_space for the frame)
+enum ColourSpace { CS_GRAY = 0, CS_YCC = 1, CS_RGB = 2, CS_CMYK = 3, CS_YCCK = 4 };
+
 struct DevImage {
-    int h, w, out_h, out_w, orientation, ncomp, hmax, vmax, mcux, mcuy, nmcu, bpm;
-    int blk_comp[6], blk_dx[6], blk_dy[6];
-    int comp_h[3], comp_v[3];
-    int plane_w[3], plane_h[3];
-    int64_t coef_off, plane_off[3];
+    int h, w, out_h, out_w, orientation, ncomp, colour, hmax, vmax, mcux, mcuy, nmcu, bpm;
+    int blk_comp[MAX_BLOCKS], blk_dx[MAX_BLOCKS], blk_dy[MAX_BLOCKS];
+    int comp_h[MAX_COMPS], comp_v[MAX_COMPS];
+    int down_w[MAX_COMPS], down_h[MAX_COMPS];  // the component's real (downsampled) size
+    int plane_w[MAX_COMPS], plane_h[MAX_COMPS];
+    int64_t coef_off, plane_off[MAX_COMPS];
     uint8_t* out;
-    int16_t qt[3][64];  // natural order (values > 32767 are rejected on the host)
+    int16_t qt[MAX_COMPS][64];  // natural order (values > 32767 are rejected on the host)
 };
 
 // A restart segment of a scan; first_mcu / nmcu count the scan's MCUs (single blocks when it is not interleaved).
@@ -91,10 +100,11 @@ enum ScanKind { SCAN_HUFF = 0, SCAN_DC_REFINE = 1, SCAN_AC_REFINE = 2 };
 
 struct DevScan {
     int img, kind, ncomp, bpm, mcux, nmcu, per, inter;
+    int tbl_bpm;  // blocks after which the tables repeat: 1 when every block of the MCU uses the same ones
     int ss, se, al;
     int h, v, j0;                 // not interleaved: the component's sampling factors and first block within the frame's MCU
-    int blk_comp[6], blk_map[6];  // block of the scan's MCU -> scan component, -> block of the frame's MCU (interleaved)
-    int blk_dc[6], blk_ac[6];     // -> its tables (indices into the batch's table array)
+    int blk_comp[MAX_BLOCKS], blk_map[MAX_BLOCKS];  // block of the scan's MCU -> scan component, -> block of the frame's MCU
+    int blk_dc[MAX_BLOCKS], blk_ac[MAX_BLOCKS];     // -> its tables (indices into the batch's table array)
     int seg0, nseg, sub0, nsub;
     int acr_off;                  // AC refinement: the scan's first block in the round's masks and records
     int64_t raw_off, raw_len, unst_off;
@@ -121,9 +131,9 @@ struct HuffSpec {
 
 struct Header {
     int h = 0, w = 0, out_h = 0, out_w = 0, orientation = 1, ncomp = 0, hmax = 1, vmax = 1, mcux = 0, mcuy = 0, nmcu = 0;
-    int dri = 0;
-    int comp_h[3] = {1, 1, 1}, comp_v[3] = {1, 1, 1};
-    uint16_t qt[3][64];
+    int dri = 0, colour = CS_GRAY;
+    int comp_h[MAX_COMPS] = {1, 1, 1, 1}, comp_v[MAX_COMPS] = {1, 1, 1, 1};
+    uint16_t qt[MAX_COMPS][64];
     HuffSpec dht[2][4];  // the tables defined so far
 };
 
@@ -158,10 +168,11 @@ bool build_huff(const HuffSpec& s, DevHuff* d) {
 constexpr int MAX_SCANS = 64;
 
 struct ScanSpec {
-    int ncomp = 0, comp[3] = {0, 0, 0};  // frame component of each scan component
+    int ncomp = 0, comp[MAX_COMPS] = {0, 0, 0, 0};  // frame component of each scan component
     int ss = 0, se = 63, ah = 0, al = 0, dri = 0;
     int mcux = 0, nmcu = 0, bpm = 0;     // the scan's MCU grid: the frame's when interleaved, the component's block grid if not
-    HuffSpec dc[3], ac[3];               // the tables in force at this SOS (optimised progressive files redefine them per scan)
+    bool one_table = true;               // every scan component names the same DC and AC tables (libjpeg's CMYK)
+    HuffSpec dc[MAX_COMPS], ac[MAX_COMPS];  // the tables in force at this SOS (optimised progressive files redefine them per scan)
     std::vector<int64_t> seg_begin, seg_end;  // raw byte ranges of the restart segments
     std::vector<int64_t> seg_stuffed;         // FF00 pairs inside each segment
 };
@@ -181,26 +192,37 @@ bool huff_ok(const HuffSpec& s) {
 // component in exactly one scan) and progressive Huffman files (SOF2) whose progression libjpeg accepts without a warning
 // and whose output libjpeg-turbo does not smooth.  Everything else gets a status and goes to cv2.  The two modes report
 // some defects at different points (the `!multi` checks), so a file with two defects keeps the status each mode always
-// gave it.
+// gave it.  SMAPB_JPEG_COLOUR widens the frames either mode accepts: 4 components, 3 components libjpeg treats as RGB,
+// and every integral sampling (factors 1..4, at most MAX_BLOCKS blocks per MCU); without it a frame is grayscale or
+// YCbCr with luma H, V in {1, 2} and chroma 1x1.
 int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
-    const bool multi = flags & SMAPB_JPEG_SCANS;
+    const bool multi = flags & SMAPB_JPEG_SCANS, colour = flags & SMAPB_JPEG_COLOUR;
     Header* H = &M->f;
     if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return SMAPB_JPEG_MALFORMED;
     int64_t p = 2;
     const uint8_t* qt[4] = {nullptr, nullptr, nullptr, nullptr};
     int qprec[4] = {0, 0, 0, 0};
     bool sof = false, progressive = false, jfif = false, adobe = false, have_orient = false, qt_used[4] = {false, false, false, false};
-    bool latched[3] = {false, false, false};
-    int adobe_transform = 0, ids[3] = {0, 0, 0}, tq[3] = {0, 0, 0};
-    int coef_bits[3][64];  // libjpeg's progression record: -1 = never coded, else the Al of the last scan that coded it
-    int nscanned[3] = {0, 0, 0};
+    bool latched[MAX_COMPS] = {false, false, false, false};
+    int adobe_transform = 0, ids[MAX_COMPS] = {0, 0, 0, 0}, tq[MAX_COMPS] = {0, 0, 0, 0};
+    int coef_bits[MAX_COMPS][64];  // libjpeg's progression record: -1 = never coded, else the Al of the last scan that coded it
+    int nscanned[MAX_COMPS] = {0, 0, 0, 0};
     memset(coef_bits, 0xFF, sizeof(coef_bits));
-    // libjpeg's colour-space rule for 3 components: a JFIF APP0 means YCbCr; else an Adobe APP14 means RGB when its
-    // transform flag is 0 and YCbCr otherwise; else component ids 'R','G','B' mean RGB, anything else YCbCr
-    auto ycc = [&]() {
-        if (H->ncomp != 3 || jfif) return true;
-        if (adobe) return adobe_transform != 0;
-        return !(ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B');
+    // libjpeg's colour-space rule (default_decompress_parms).  3 components: a JFIF APP0 means YCbCr; else an Adobe APP14
+    // means RGB when its transform flag is 0 and YCbCr otherwise; else component ids 'R','G','B' mean RGB, anything else
+    // YCbCr.  4 components: an Adobe transform of 2 means YCCK, 0 or no Adobe marker CMYK; libjpeg warns about any other
+    // transform and such files are left to cv2.  Without SMAPB_JPEG_COLOUR only grayscale and YCbCr are decoded.
+    // -> the colour space, or -1 for a frame left to cv2.
+    auto colour_space = [&]() -> int {
+        int cs = CS_GRAY;
+        if (H->ncomp == 3) {
+            if (jfif) cs = CS_YCC;
+            else if (adobe) cs = adobe_transform != 0 ? CS_YCC : CS_RGB;
+            else cs = ids[0] == 'R' && ids[1] == 'G' && ids[2] == 'B' ? CS_RGB : CS_YCC;
+        } else if (H->ncomp == 4) {
+            cs = !adobe || adobe_transform == 0 ? CS_CMYK : adobe_transform == 2 ? CS_YCCK : -1;
+        }
+        return colour || cs <= CS_YCC ? cs : -1;
     };
     auto too_large = [&]() { return (int64_t)H->h * H->w > SMAPB_JPEG_MAX_PIXELS; };
     for (;;) {
@@ -255,7 +277,8 @@ int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
             const int prec = s[0], nf = s[5];
             H->h = u16(s + 1), H->w = u16(s + 3);
             if (L != 6 + 3 * nf) return SMAPB_JPEG_MALFORMED;
-            if (prec != 8 || H->h == 0 || H->w == 0 || (nf != 1 && nf != 3)) return SMAPB_JPEG_UNSUPPORTED;
+            if (prec != 8 || H->h == 0 || H->w == 0 || (nf != 1 && nf != 3 && !(colour && nf == 4)))
+                return SMAPB_JPEG_UNSUPPORTED;
             H->ncomp = nf;
             for (int c = 0; c < nf; c++) {
                 ids[c] = s[6 + 3 * c];
@@ -266,15 +289,33 @@ int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
                 for (int e = 0; e < c; e++)
                     if (ids[e] == ids[c]) return SMAPB_JPEG_MALFORMED;
             }
+            if (colour) {
+                // libjpeg: factors 1..4 (initial_setup); every ratio to the maxima integral (libjpeg-turbo's upsampler
+                // has no fractional one); at most D_MAX_BLOCKS_IN_MCU blocks in an interleaved scan's MCU - frames
+                // over it are refused whatever their scans, as the coefficient buffer keeps the frame's MCU
+                int hmax = 1, vmax = 1, blocks = 0;
+                for (int c = 0; c < nf; c++) {
+                    if (H->comp_h[c] < 1 || H->comp_h[c] > 4 || H->comp_v[c] < 1 || H->comp_v[c] > 4)
+                        return SMAPB_JPEG_UNSUPPORTED;
+                    hmax = std::max(hmax, H->comp_h[c]), vmax = std::max(vmax, H->comp_v[c]);
+                    blocks += H->comp_h[c] * H->comp_v[c];
+                }
+                if (nf > 1) {
+                    for (int c = 0; c < nf; c++)
+                        if (hmax % H->comp_h[c] || vmax % H->comp_v[c]) return SMAPB_JPEG_UNSUPPORTED;
+                    if (blocks > MAX_BLOCKS) return SMAPB_JPEG_UNSUPPORTED;
+                }
+            }
             if (nf == 1) {
                 H->comp_h[0] = H->comp_v[0] = 1;  // one component: one block per MCU whatever its factors say
-            } else {
+            } else if (!colour) {
                 const bool ok = (H->comp_h[0] == 1 || H->comp_h[0] == 2) && (H->comp_v[0] == 1 || H->comp_v[0] == 2) &&
                                 H->comp_h[1] == 1 && H->comp_v[1] == 1 && H->comp_h[2] == 1 && H->comp_v[2] == 1;
                 if (!ok) return SMAPB_JPEG_UNSUPPORTED;
             }
             if (multi && too_large()) return SMAPB_JPEG_TOO_LARGE;  // without SMAPB_JPEG_SCANS: at the SOS
-            H->hmax = H->comp_h[0], H->vmax = H->comp_v[0];
+            H->hmax = H->vmax = 1;
+            for (int c = 0; c < nf; c++) H->hmax = std::max(H->hmax, H->comp_h[c]), H->vmax = std::max(H->vmax, H->comp_v[c]);
             H->mcux = (H->w + 8 * H->hmax - 1) / (8 * H->hmax);
             H->mcuy = (H->h + 8 * H->vmax - 1) / (8 * H->vmax);
             H->nmcu = H->mcux * H->mcuy;
@@ -345,6 +386,7 @@ int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
                 }
                 const int c = S.comp[k];
                 const int td = s[2 + 2 * k] >> 4, ta = s[2 + 2 * k] & 15;
+                if (s[2 + 2 * k] != s[2]) S.one_table = false;
                 if (!multi && (ta > 3 || !H->dht[1][ta].defined || !qt[tq[c]])) return SMAPB_JPEG_UNSUPPORTED;
                 if (dc_first) {
                     if (td > 3 || !H->dht[0][td].defined) return SMAPB_JPEG_UNSUPPORTED;
@@ -370,7 +412,7 @@ int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
             }
             if (!multi) {
                 if (S.ss != 0 || S.se != 63 || S.ah != 0 || S.al != 0) return SMAPB_JPEG_UNSUPPORTED;
-                if (!ycc()) return SMAPB_JPEG_UNSUPPORTED;
+                if (colour_space() < 0) return SMAPB_JPEG_UNSUPPORTED;
                 if (too_large()) return SMAPB_JPEG_TOO_LARGE;
             }
             if (ns == 1) {  // non-interleaved: the component's own block grid
@@ -429,13 +471,14 @@ int jpeg_parse(const uint8_t* d, int64_t n, int flags, ScanHeader* M) {
             for (int i = 1; i <= 9; i++)
                 if (coef_bits[c][i] != 0) return SMAPB_JPEG_UNSUPPORTED;
         }
-        if (!ycc()) return SMAPB_JPEG_UNSUPPORTED;
+        if (colour_space() < 0) return SMAPB_JPEG_UNSUPPORTED;
     } else {
         // the one scan covers every component and its colour space was checked at its SOS; its tables are checked last
         const ScanSpec& S = M->scans[0];
         for (int k = 0; k < S.ncomp; k++)
             if (!huff_ok(S.dc[k]) || !huff_ok(S.ac[k])) return SMAPB_JPEG_MALFORMED;
     }
+    H->colour = colour_space();
     H->out_h = H->orientation >= 5 ? H->w : H->h;
     H->out_w = H->orientation >= 5 ? H->h : H->w;
     return SMAPB_JPEG_OK;
@@ -682,7 +725,7 @@ __device__ RunResult scan_run(const DevScan& S, const DevImage& I, const DevHuff
         if (done) {
             zz = S.ss;
             nblk = min(nblk + done, BLOCK_SAT);
-            if (++blk == S.bpm) blk = 0;
+            if (++blk == S.tbl_bpm) blk = 0;
         }
     }
     return {pos, blk, zz, nblk, err};
@@ -1184,40 +1227,68 @@ __global__ void __launch_bounds__(128) idct_kernel(const DevImage* __restrict__ 
 // ---- d. upsampling, colour, orientation ------------------------------------------------------------------------------
 __device__ __forceinline__ int px(const uint8_t* p, int pw, int y, int x) { return p[(int64_t)y * pw + x]; }
 
-// libjpeg's fancy upsampling of a chroma plane (factors 1x1) to the luma grid at (y, x); cw x ch = the plane's real size
-__device__ int chroma_at(const uint8_t* C, int pw, int cw, int ch, int hmax, int vmax, int y, int x) {
-    if (hmax == 1 && vmax == 1) return px(C, pw, y, x);
-    const int i = x >> (hmax - 1);
-    if (hmax == 2 && cw <= 2) return px(C, pw, y >> (vmax - 1), i);  // fancy h2 filters need 3 columns: replication
-    if (vmax == 1) {  // h2v1
-        const int n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);
+// Component c at the frame's pixel (y, x), upsampled by the method libjpeg-turbo 3.x picks for it (jinit_upsampler), from
+// its factors (h, v) and the frame's maxima: equal factors as is; twice as wide (same height) fancy h2v1, twice as tall
+// (same width) fancy h1v2, both fancy h2v2 - the h2 filters only when the component is more than 2 samples wide, else
+// replication; any other integral ratio replication (int_upsample).  Fancy filters clamp at the component's real size.
+__device__ int sample_at(const DevImage& I, const uint8_t* __restrict__ planes, int c, int y, int x) {
+    const uint8_t* C = planes + I.plane_off[c];
+    const int pw = I.plane_w[c], h = I.comp_h[c], v = I.comp_v[c], cw = I.down_w[c], ch = I.down_h[c];
+    if (h == I.hmax && v == I.vmax) return px(C, pw, y, x);
+    const bool h2 = 2 * h == I.hmax && cw > 2, v2 = 2 * v == I.vmax;
+    if (h2 && v == I.vmax) {  // h2v1
+        const int i = x >> 1, n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);
         return (3 * px(C, pw, y, i) + px(C, pw, y, n) + ((x & 1) ? 2 : 1)) >> 2;
     }
-    const int r0 = y >> 1, r1 = (y & 1) ? min(r0 + 1, ch - 1) : max(r0 - 1, 0);
-    if (hmax == 1)  // h1v2
+    if (v2 && h == I.hmax) {  // h1v2
+        const int r0 = y >> 1, r1 = (y & 1) ? min(r0 + 1, ch - 1) : max(r0 - 1, 0);
         return (3 * px(C, pw, r0, x) + px(C, pw, r1, x) + ((y & 1) ? 2 : 1)) >> 2;
-    const int n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);  // h2v2: column sums of the nearer and the further row
-    const int s0 = 3 * px(C, pw, r0, i) + px(C, pw, r1, i), s1 = 3 * px(C, pw, r0, n) + px(C, pw, r1, n);
-    return (3 * s0 + s1 + ((x & 1) ? 7 : 8)) >> 4;
+    }
+    if (h2 && v2) {  // h2v2: column sums of the nearer and the further row
+        const int i = x >> 1, n = (x & 1) ? min(i + 1, cw - 1) : max(i - 1, 0);
+        const int r0 = y >> 1, r1 = (y & 1) ? min(r0 + 1, ch - 1) : max(r0 - 1, 0);
+        const int s0 = 3 * px(C, pw, r0, i) + px(C, pw, r1, i), s1 = 3 * px(C, pw, r0, n) + px(C, pw, r1, n);
+        return (3 * s0 + s1 + ((x & 1) ? 7 : 8)) >> 4;
+    }
+    return px(C, pw, y / (I.vmax / v), x / (I.hmax / h));
 }
 
+// JFIF YCbCr -> RGB with 16-bit fixed-point constants round(k * 2^16), rounded by adding 2^15, saturated
+__device__ __forceinline__ void ycc_rgb(int Y, int cb, int cr, int* r, int* g, int* b) {
+    cb -= 128, cr -= 128;
+    *r = min(max(Y + ((91881 * cr + 32768) >> 16), 0), 255);
+    *g = min(max(Y + ((-46802 * cr - 22554 * cb + 32768) >> 16), 0), 255);
+    *b = min(max(Y + ((116130 * cb + 32768) >> 16), 0), 255);
+}
+
+// cv2's CMYK -> BGR (icvCvt_CMYK2BGR_8u_C4C3R) of one ink
+__device__ __forceinline__ int ink(int x, int k) { return k - (((255 - x) * k) >> 8); }
+
+// libjpeg's conversion to what cv2 asks for (BGR from 1 or 3 components, CMYK from 4), then cv2's CMYK -> BGR:
+//   grayscale  replicated          YCbCr  the tables above          RGB  reordered
+//   CMYK       as stored           YCCK   C, M, Y = 255 - the R, G, B of (Y, Cb, Cr), K as stored
 __global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict__ imgs, const uint8_t* __restrict__ planes,
                                                      const int* __restrict__ status) {
     const DevImage& I = imgs[blockIdx.y];
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (int64_t)I.h * I.w || status[blockIdx.y] != SMAPB_JPEG_OK) return;
     const int y = (int)(t / I.w), x = (int)(t % I.w);
-    const int Y = px(planes + I.plane_off[0], I.plane_w[0], y, x);
-    int b = Y, g = Y, r = Y;
-    if (I.ncomp == 3) {
-        const int cw = (I.w + I.hmax - 1) / I.hmax, ch = (I.h + I.vmax - 1) / I.vmax;
-        const int cb = chroma_at(planes + I.plane_off[1], I.plane_w[1], cw, ch, I.hmax, I.vmax, y, x) - 128;
-        const int cr = chroma_at(planes + I.plane_off[2], I.plane_w[2], cw, ch, I.hmax, I.vmax, y, x) - 128;
-        // JFIF YCbCr -> RGB with 16-bit fixed-point constants round(k * 2^16), rounded by adding 2^15
-        r = Y + ((91881 * cr + 32768) >> 16);
-        g = Y + ((-46802 * cr - 22554 * cb + 32768) >> 16);
-        b = Y + ((116130 * cb + 32768) >> 16);
-        r = min(max(r, 0), 255), g = min(max(g, 0), 255), b = min(max(b, 0), 255);
+    const int s0 = sample_at(I, planes, 0, y, x);
+    int b = s0, g = s0, r = s0;
+    if (I.ncomp > 1) {
+        const int s1 = sample_at(I, planes, 1, y, x), s2 = sample_at(I, planes, 2, y, x);
+        if (I.colour == CS_RGB) {
+            r = s0, g = s1, b = s2;
+        } else if (I.colour == CS_CMYK) {
+            const int k = sample_at(I, planes, 3, y, x);
+            r = ink(s0, k), g = ink(s1, k), b = ink(s2, k);
+        } else {
+            ycc_rgb(s0, s1, s2, &r, &g, &b);
+            if (I.colour == CS_YCCK) {
+                const int k = sample_at(I, planes, 3, y, x);
+                r = ink(255 - r, k), g = ink(255 - g, k), b = ink(255 - b, k);
+            }
+        }
     }
     int oy, ox;
     orient_store_pos(I.orientation, I.h, I.w, y, x, &oy, &ox);
@@ -1297,6 +1368,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
         DevImage& I = imgs[k];
         memset(&I, 0, sizeof(I));
         I.h = h.h, I.w = h.w, I.out_h = h.out_h, I.out_w = h.out_w, I.orientation = h.orientation, I.ncomp = h.ncomp;
+        I.colour = h.colour;
         I.hmax = h.hmax, I.vmax = h.vmax, I.mcux = h.mcux, I.mcuy = h.mcuy, I.nmcu = h.nmcu;
         I.out = bgr[idx[k]];
         int j = 0;
@@ -1304,6 +1376,8 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             for (int v = 0; v < h.comp_v[c]; v++)
                 for (int u = 0; u < h.comp_h[c]; u++) I.blk_comp[j] = c, I.blk_dx[j] = u, I.blk_dy[j] = v, j++;
             I.comp_h[c] = h.comp_h[c], I.comp_v[c] = h.comp_v[c];
+            I.down_w[c] = (h.w * h.comp_h[c] + h.hmax - 1) / h.hmax;
+            I.down_h[c] = (h.h * h.comp_v[c] + h.vmax - 1) / h.vmax;
             I.plane_w[c] = h.mcux * h.comp_h[c] * 8;
             I.plane_h[c] = h.mcuy * h.comp_v[c] * 8;
             I.plane_off[c] = plane_total;
@@ -1360,6 +1434,9 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
                 D.h = h.comp_h[c], D.v = h.comp_v[c], D.j0 = j0c;  // used when the scan has one component
             }
             if (!D.inter) D.bpm = 1;
+            // the decoder state keeps the block within the MCU only to pick its tables; when they are all the same the
+            // bits cannot tell the blocks apart, and a speculative decoder would never fall into step with that index
+            D.tbl_bpm = P.one_table ? 1 : D.bpm;
             D.raw_off = raw_total;
             D.raw_len = P.seg_end.back() - P.seg_begin.front();
             raw_total += align_up(D.raw_len, 16);
@@ -1518,7 +1595,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             *launches += 2;
         }
         if (R.ndc) {
-            scan_dc_kernel<<<dim3(R.ndc, 3), 1024, 0, st>>>(d_img, d_scan, d_list + R.dc_off, d_status, ws->coef);
+            scan_dc_kernel<<<dim3(R.ndc, MAX_COMPS), 1024, 0, st>>>(d_img, d_scan, d_list + R.dc_off, d_status, ws->coef);
             DECODE_CK(cudaGetLastError());
             ++*launches;
         }
@@ -1555,7 +1632,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
 extern "C" {
 #pragma GCC visibility push(default)
 int smapb_jpeg_info_ex(const uint8_t* data, int64_t nbytes, int flags, int* h, int* w, int* orientation, int* status) {
-    if (!status || (flags & ~SMAPB_JPEG_SCANS)) return -1;
+    if (!status || (flags & ~(SMAPB_JPEG_SCANS | SMAPB_JPEG_COLOUR))) return -1;
     smapb::ScanHeader M;
     return smapb::report_info(smapb::jpeg_parse(data, nbytes, flags, &M), M.f, status, h, w, orientation);
 }

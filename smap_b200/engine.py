@@ -60,6 +60,7 @@ def get_tile_table():
 
 
 JPEG_SCANS = 1  # SMAPB_JPEG_SCANS
+JPEG_COLOUR = 2  # SMAPB_JPEG_COLOUR
 
 
 def _header_info(fn, data, *flags):
@@ -72,11 +73,16 @@ def _header_info(fn, data, *flags):
     return st.value, h.value, w.value, o.value
 
 
-def jpeg_info(data, scans=False):
+def _jpeg_flags(scans, colour):
+    return (JPEG_SCANS if scans else 0) | (JPEG_COLOUR if colour else 0)
+
+
+def jpeg_info(data, scans=False, colour=False):
     """Header walk of one JPEG file on the host (no GPU): -> (status, h, w, orientation).  status 0 = the GPU decoder
     handles it and cv2.imread returns an [h, w, 3] image; otherwise one of SMAPB_JPEG_* (include/smap_b200.h).
-    scans=True: the walk of Engine.decode_jpeg_ex, which also takes multi-scan sequential and progressive files."""
-    return _header_info(_lib.load().smapb_jpeg_info_ex, data, JPEG_SCANS if scans else 0)
+    scans=True: the walk of Engine.decode_jpeg_ex, which also takes multi-scan sequential and progressive files;
+    colour=True: it also takes CMYK, YCCK and RGB frames and every integral sampling (SMAPB_JPEG_COLOUR)."""
+    return _header_info(_lib.load().smapb_jpeg_info_ex, data, _jpeg_flags(scans, colour))
 
 
 def png_info(data):
@@ -236,13 +242,16 @@ class Engine:
         cv2.imdecode(file, IMREAD_COLOR), or None when the file is not one the GPU decoder handles (cv2 must read it)."""
         return self._decode(files, jpeg_info, self.lib.smapb_decode_jpeg)
 
-    def decode_jpeg_ex(self, files, scans=True):
+    def decode_jpeg_ex(self, files, scans=True, colour=False):
         """decode_jpeg for a batch that may also hold progressive Huffman files and sequential files with several scans
-        (smapb_decode_jpeg_ex with SMAPB_JPEG_SCANS; scans=False is decode_jpeg).  -> per file a CUDA uint8 BGR [H,W,3]
-        tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None (cv2 must read it).  Progressive files decode their AC
-        refinement scans sequentially within each restart segment (one warp per segment, the batch's images side by side),
-        so a batch takes about as long as its slowest image; run_inference sends the JPEGs decode_jpeg refuses here."""
-        return self._decode(files, lambda f: jpeg_info(f, scans), self.lib.smapb_decode_jpeg_ex, JPEG_SCANS if scans else 0)
+        (smapb_decode_jpeg_ex with SMAPB_JPEG_SCANS; scans=False and colour=False is decode_jpeg), and with colour=True
+        CMYK, YCCK and RGB frames and every integral sampling (SMAPB_JPEG_COLOUR: 4:1:1, 4:1:0, factors of 3, chroma
+        finer than luma).  -> per file a CUDA uint8 BGR [H,W,3] tensor equal to cv2.imdecode(file, IMREAD_COLOR), or None
+        (cv2 must read it).  Progressive files decode their AC refinement scans sequentially within each restart segment
+        (one warp per segment, the batch's images side by side), so a batch takes about as long as its slowest image;
+        run_inference sends the JPEGs decode_jpeg refuses here."""
+        return self._decode(files, lambda f: jpeg_info(f, scans, colour), self.lib.smapb_decode_jpeg_ex,
+                            _jpeg_flags(scans, colour))
 
     def decode_png(self, files):
         """files: list of bytes (whole PNG files) -> list with, per file, a CUDA uint8 BGR [H,W,3] tensor equal to
