@@ -1,7 +1,9 @@
 """GPU: SURVEY 8(f) f4 - (1) the GT-matching branch of register_pred + the float64 lift it implies (test_util.py:21-39),
 against the golden outputs of the unmodified reference functions (tests/golden/lift_gt_cases.npz) and the oracle;
 (2) association at a map size other than the reference's hard-coded 128x208 (extensions/association.cpp:21): 256x256 maps
-(config 5, a 1024x1024 input) and a small odd size, bit-exact against the oracle, and the whole path at 1024x1024."""
+(config 5, a 1024x1024 input: PAF gathers from global memory) and 64x96 (a small map: vectorised NMS, staged PAF),
+bit-exact against the oracle, and the whole path at 1024x1024.  tests/test_assoc_sizes_gpu.py checks these instances and
+the scalar NMS against the live reference and the oracle on the adversarial frames."""
 import os
 
 import numpy as np
