@@ -14,12 +14,12 @@ extern "C" {
 /* 64-bit position-weighted checksums of the output tensor of every op of the batch-B plan, as left by the last forward.
  * sums[max_ops]; desc (optional): max_ops strings of desc_stride bytes (512 is enough) describing each op.  Returns the number
  * of ops.  Op i here is dump index i of smapb_debug_dump.  A description is space-separated key=value fields:
- *   name=<unit name>  kind=conv | conv_f32 | stem_tc | stem | s2d | maxpool | upadd
+ *   name=<unit name>  kind=conv | conv_f32 | stem_tc | stem | s2d | maxpool
  *     conv: tensor-core conv with split-bf16 output; conv_f32: fp32 NHWC output (heads, *.tapexp); stem_tc: the 7x7/s2
  *     stem as a 4x1-tap conv over the s2d view; stem: the CUDA-core stem; s2d: space-to-depth of the image
- *   inputs by role, as dump indices, absent roles left out: in= res= p1= p2= in2= up= (convs), a= b= (maxpool, upadd);
+ *   inputs by role, as dump indices, absent roles left out: in= res= p1= p2= in2= up= (convs), a= (maxpool);
  *     in=x is the network input image
- *   convs:  tw= (patch width; 128 on the flat path) rev= (reverse tile order) k=<kh>x<kw> s= pad=<y>x<x> cin= cin2= s2=
+ *   convs:  tw= (patch width; 128 on the flat path) k=<kh>x<kw> s= pad=<y>x<x> cin= cin2= s2=
  *           cout= (padded) out=NxHxWxC bn= relu= hasres= post= upmode= tiles= nterms=
  *   others: out=NxHxWxC nterms= */
 int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int max_ops, char* desc, int desc_stride);
@@ -45,8 +45,8 @@ int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4);
  *   SMAPB_DEBUG_SYNC=1        synchronise the stream after every launch
  *   SMAPB_FORCE_TILE=bn       force a tile width (32, 64, 128) wherever it is valid, except where the tile table or the
  *                             autotuner picks one;  SMAPB_NO_AUTOTUNE=1  cost model only
- *   SMAPB_ONE_STREAM=1        no side stream;  SMAPB_NO_GRAPH=1  no CUDA graph replay;  SMAPB_PDL=1  programmatic dependent launch
- *   SMAPB_STEM=cuda           CUDA-core stem;  SMAPB_NO_FUSE_DS=1 / SMAPB_NO_FUSE_UP=1  unfused downsample / up-residual
+ *   SMAPB_NO_GRAPH=1          no CUDA graph replay
+ *   SMAPB_STEM=cuda           CUDA-core stem
  *   SMAPB_ROLES=1             per-role wait-cycle counters in smapb_conv_test
  *   SMAPB_ROLES_PLAN=file.csv the same counters for every conv launch of a profiled (smapb_profile_begin/end) run, i.e. inside the
  *                             real step (tools/roles_plan.py)

@@ -60,7 +60,6 @@ nms_flag_kernel(const float* __restrict__ hms, int nchan, int B, int h, int w, f
     const int lane = threadIdx.x & 31;
     const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-    pdl_wait();
     if (VEC) {
         // persistent: one wave of CTAs, every warp strides over 4-group (512-pixel, 2 KB) steps with all four 16-byte
         // loads of a lane in flight before any of them is consumed.  Pixels above the threshold (candidates) are NOT
@@ -161,7 +160,6 @@ nms_flag_kernel(const float* __restrict__ hms, int nchan, int B, int h, int w, f
             if (lane == 0) masks[wd] = m;
         }
     }
-    pdl_trigger();
 }
 
 __global__ void __launch_bounds__(NMSC_THREADS)
@@ -175,7 +173,6 @@ nms_compact_kernel(const float* __restrict__ hms, int nchan, int h, int w, const
     const uint32_t* mk = masks + ((size_t)img * NJ + c) * nwords;
     float* out = peaks + ((size_t)img * NJ + c) * (MAXP + 1) * 3;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    pdl_wait();
     // contiguous run of words per warp, lanes stride through the run; counts first
     const int wpw = (nwords + NMSC_WARPS - 1) / NMSC_WARPS;
     const int w0 = min(nwords, warp * wpw), w1 = min(nwords, w0 + wpw);
@@ -257,7 +254,6 @@ nms_compact_kernel(const float* __restrict__ hms, int nchan, int h, int w, const
     }
     // deterministic tail: slots the reference leaves uninitialised are zeroed
     for (int k = (count + 1) * 3 + threadIdx.x; k < (MAXP + 1) * 3; k += NMSC_THREADS) out[k] = 0.f;
-    pdl_trigger();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -339,7 +335,6 @@ paf_kernel(const float* __restrict__ hms, int nchan, int h, int w, const float* 
     const float* pB = peaks + ((size_t)img * NJ + partB) * (MAXP + 1) * 3;
     float* out = scores + ((size_t)img * NL + l) * MAXP * MAXP;
 
-    pdl_wait();
     const float* src = hms + ((size_t)img * nchan + NJ + 2 * l) * hw;
     // STAGED: the bulk copies of both planes are issued FIRST, before the candidate counts are even known; the counts and the
     // two peak lists (dependent global loads, ~1 us each) then arrive while the copy engine streams the 213 KB.  An item with
@@ -392,7 +387,6 @@ paf_kernel(const float* __restrict__ hms, int nchan, int h, int w, const float* 
             if (a >= nA || b >= nB) out[p] = -1.f;
         }
     }
-    pdl_trigger();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -566,7 +560,6 @@ group_kernel(const float* __restrict__ peaks, const float* __restrict__ scores, 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nthr = GROUP_WARPS * 32;
 
-    pdl_wait();
     const float* rootPeaks = pk + (size_t)root_idx * (MAXP + 1) * 3;
     const int P = (int)rootPeaks[0];
     if (tid == 0) counts[img] = P;
@@ -734,7 +727,6 @@ group_kernel(const float* __restrict__ peaks, const float* __restrict__ scores, 
         if (p < P) v = make_float4(s_body[p][j][0], s_body[p][j][1], 0.f, s_body[p][j][2]);
         reinterpret_cast<float4*>(outb)[i] = v;
     }
-    pdl_trigger();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -798,7 +790,6 @@ lift_kernel(const float* __restrict__ bodies, const int* __restrict__ counts, co
     T* pred2d = pred2d_base + (size_t)img * s2d;
     double* pred3d = pred3d_base + (size_t)img * s3d;
     double* root_depth = root_depth_base + (size_t)img * srd;
-    pdl_wait();
     const int P = counts[img];
     const float* b = bodies + (size_t)img * MAXP * NJ * 4;
     const float* dd = det_d + (size_t)img * NL * hw;
@@ -984,7 +975,6 @@ lift_kernel(const float* __restrict__ bodies, const int* __restrict__ counts, co
         counts_out[(size_t)img * scnt] = NP;
         if (scnt > 1) counts_out[(size_t)img * scnt + 1] = 0;  // smapb_record::pad_
     }
-    pdl_trigger();
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -74,10 +74,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
-// Programmatic dependent launch hooks (no-ops when the launch has no PDL attribute).
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // split-bf16 helpers: v ~= hi + lo with |v - hi - lo| <= 2^-17 |v|
 __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(v);

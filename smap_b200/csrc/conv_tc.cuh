@@ -57,8 +57,6 @@ struct alignas(64) ConvParams {
     float* out_f32;      // fp32 NHWC (heads), or null
     long long plane_stride;  // elements between the hi and lo planes (= N*H*W*Cout)
     int relu;
-    int reverse;    // walk the tile list back to front (the consumer of a tensor starts with the rows its producer wrote
-                    // last, which are the ones still resident in L2)
     // fused bilinear residual (Upsample_unit, model/smap.py:211-217): tmR[0] is a low-resolution tensor [N,Hi,Wi,C];
     // the ring carries the (ph x pw)-pixel patch under each output tile and the epilogue interpolates
     // (align_corners=True) before the ReLU.  up_mode = 0: plain residual.
@@ -321,9 +319,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
     const int tw = 1 << p.tw_log2;
 
     if (tl && threadIdx.x == 0) p.dbg_tl[1] = clock64();
-    pdl_wait();     // inputs of this layer are produced by the previous kernel in the stream
-    pdl_trigger();  // let the next kernel's CTAs be scheduled onto SMs as they drain (they block in their own wait)
-    const long long t_begin = p.dbg ? clock64() : 0;  // CTA lifetime from here: the wait for the previous kernel excluded
+    const long long t_begin = p.dbg ? clock64() : 0;  // CTA lifetime from here: barrier set-up excluded
 
     if (warp < 4) {
         // ============================ producer warpgroup ======================
@@ -334,8 +330,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
             uint32_t phase = 0;
             long long w_empty = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-                const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-                const int nt = te % p.n_tiles, mt = te / p.n_tiles;
+                const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
                 const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
                 const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
                 const int x_in0 = (tx << p.tw_log2) * p.stride - p.pad_x;
@@ -377,8 +372,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
             // of the two consumer warpgroups take their tiles' entries in that same order
             int cnt = 0;  // fills issued so far
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-                const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-                const int nt = te % p.n_tiles, mt = te / p.n_tiles;
+                const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
                 const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
                 const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
                 for (int c = 0; c < Cfg::CHUNKS; c++) {
@@ -421,8 +415,7 @@ __global__ void __launch_bounds__(384, 1) conv_tc_kernel(const __grid_constant__
         float acc[2][BLOCK_N / 2];  // [row half][wgmma fragment]
         for (int j = wg; j < n_cta; j += 2) {
             const int tile = blockIdx.x + j * gridDim.x;
-            const int te = p.reverse ? p.total_tiles - 1 - tile : tile;
-            const int nt = te % p.n_tiles, mt = te / p.n_tiles;
+            const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
             const int img = mt / tiles_per_img, r = mt - img * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
             const int n0 = nt * BLOCK_N;

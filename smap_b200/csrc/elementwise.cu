@@ -57,7 +57,6 @@ stem_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[147][6
     const int n = blockIdx.z;
     const int oy0 = blockIdx.y * ST_TH, ox0 = blockIdx.x * ST_TW;
     const int iy0 = oy0 * 2 - 3, ix0 = ox0 * 2 - 3;
-    pdl_wait();
     for (int i = threadIdx.x; i < 147 * 64; i += 256) s_w[i] = wgt[i];
     for (int i = threadIdx.x; i < 3 * ST_PH * ST_PW; i += 256) {
         const int c = i / (ST_PH * ST_PW), r = i - c * (ST_PH * ST_PW);
@@ -141,7 +140,6 @@ stem_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[147][6
         }
     }
     if constexpr (E::F16) saturation_add(sat, n_sat);
-    pdl_trigger();
 }
 template <class E>
 cudaError_t launch_stem_e(const float* x, const float* wgt, const float* bias, int N, int H, int W, __nv_bfloat16* out,
@@ -176,7 +174,6 @@ __global__ void s2d_kernel(const float* __restrict__ x, int N, int H, int W, __n
     const int H2 = H / 2, W2 = W / 2, WP = W2 + 3;
     const long long total = (long long)N * H2 * WP;
     int n_sat = 0;
-    pdl_wait();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int xp = (int)(i % WP);
         long long r = i / WP;
@@ -221,7 +218,6 @@ __global__ void s2d_kernel(const float* __restrict__ x, int N, int H, int W, __n
         }
     }
     if constexpr (E::F16) saturation_add(sat, n_sat);
-    pdl_trigger();
 }
 cudaError_t launch_s2d(const float* x, int N, int H, int W, __nv_bfloat16* out, long long plane_stride, int terms,
                        cudaStream_t st, bool f16, unsigned long long* sat) {
@@ -295,7 +291,6 @@ __global__ void maxpool_kernel(const __nv_bfloat16* __restrict__ in, long long i
     int n_sat = 0;  // the maximum of stored values is a stored value: nothing to clamp
     const int Ho = H / 2, Wo = W / 2, CG = C / 8;
     const long long total = (long long)N * Ho * Wo * CG;
-    pdl_wait();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int cg = (int)(i % CG);
         long long r = i / CG;
@@ -320,7 +315,6 @@ __global__ void maxpool_kernel(const __nv_bfloat16* __restrict__ in, long long i
         }
         store8<E>(out + (((long long)n * Ho + oy) * Wo + ox) * C + cg * 8, out_ps, terms, m, n_sat);
     }
-    pdl_trigger();
 }
 cudaError_t launch_maxpool(const __nv_bfloat16* in, long long in_ps, int N, int H, int W, int C, __nv_bfloat16* out,
                            long long out_ps, int terms, cudaStream_t st, bool f16) {
@@ -333,11 +327,7 @@ cudaError_t launch_maxpool(const __nv_bfloat16* in, long long in_ps, int N, int 
     return cudaGetLastError();
 }
 
-// ---------------------------------------------------------------------------------------------
-// out = relu(a + bilinear_up(t)), align_corners=True (model/smap.py:211-217 with the 1x1 up_conv commuted in
-// front of the interpolation: both are linear and the bilinear weights sum to 1).
-// a, out: [N,H,W,C]; t: [N,Hi,Wi,C].
-// ---------------------------------------------------------------------------------------------
+// bilinear source taps and weights of output index o, align_corners=True
 __device__ __forceinline__ void bilin_coeff(int o, int in, int out, int& i0, int& i1, float& l0, float& l1) {
     // ATen area_pixel_compute_source_index with align_corners: src = o * (in-1)/(out-1)
     const float scale = (out > 1) ? (float)(in - 1) / (float)(out - 1) : 0.f;
@@ -346,54 +336,6 @@ __device__ __forceinline__ void bilin_coeff(int o, int in, int out, int& i0, int
     i1 = i0 + ((i0 < in - 1) ? 1 : 0);
     l1 = src - (float)i0;
     l0 = 1.f - l1;
-}
-
-template <class E>
-__global__ void upadd_relu_kernel(const __nv_bfloat16* __restrict__ a, long long a_ps, const __nv_bfloat16* __restrict__ t,
-                                  long long t_ps, int N, int H, int W, int Hi, int Wi, int C,
-                                  __nv_bfloat16* __restrict__ out, long long out_ps, int terms, unsigned long long* sat) {
-    const int CG = C / 8;
-    const long long total = (long long)N * H * W * CG;
-    int n_sat = 0;
-    pdl_wait();
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int cg = (int)(i % CG);
-        long long r = i / CG;
-        const int x = (int)(r % W);
-        r /= W;
-        const int y = (int)(r % H);
-        const int n = (int)(r / H);
-        int y0, y1, x0, x1;
-        float hy0, hy1, wx0, wx1;
-        bilin_coeff(y, Hi, H, y0, y1, hy0, hy1);
-        bilin_coeff(x, Wi, W, x0, x1, wx0, wx1);
-        float v00[8], v01[8], v10[8], v11[8], va[8], o[8];
-        const long long tb = (long long)n * Hi * Wi;
-        load8<E>(t + ((tb + (long long)y0 * Wi + x0) * C) + cg * 8, t_ps, terms, v00);
-        load8<E>(t + ((tb + (long long)y0 * Wi + x1) * C) + cg * 8, t_ps, terms, v01);
-        load8<E>(t + ((tb + (long long)y1 * Wi + x0) * C) + cg * 8, t_ps, terms, v10);
-        load8<E>(t + ((tb + (long long)y1 * Wi + x1) * C) + cg * 8, t_ps, terms, v11);
-        load8<E>(a + i * 8, a_ps, terms, va);
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            const float up = hy0 * (wx0 * v00[j] + wx1 * v01[j]) + hy1 * (wx0 * v10[j] + wx1 * v11[j]);
-            o[j] = fmaxf(va[j] + up, 0.f);
-        }
-        store8<E>(out + i * 8, out_ps, terms, o, n_sat);
-    }
-    if constexpr (E::F16) saturation_add(sat, n_sat);
-    pdl_trigger();
-}
-cudaError_t launch_upadd_relu(const __nv_bfloat16* a, long long a_ps, const __nv_bfloat16* t, long long t_ps, int N,
-                              int H, int W, int Hi, int Wi, int C, __nv_bfloat16* out, long long out_ps, int terms,
-                              cudaStream_t st, bool f16, unsigned long long* sat) {
-    const long long total = (long long)N * H * W * (C / 8);
-    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
-    if (f16)
-        upadd_relu_kernel<ElemF16><<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms, sat);
-    else
-        upadd_relu_kernel<ElemBF16><<<blocks, 256, 0, st>>>(a, a_ps, t, t_ps, N, H, W, Hi, Wi, C, out, out_ps, terms, sat);
-    return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -419,7 +361,6 @@ head_merge_kernel(const float* __restrict__ r4, const float* __restrict__ r3, co
     __shared__ int s_xi[32][4];    // xa0, xa1, xb0, xb1
     __shared__ float s_xw[32][4];  // wa0, wa1, wb0, wb1
     const int x0 = blockIdx.x * 32, y = blockIdx.y, n = blockIdx.z;
-    pdl_wait();
     int y0a = 0, y1a = 0, y0b = 0, y1b = 0;
     float ha0 = 0, ha1 = 0, hb0 = 0, hb1 = 0;
     if (r3) bilin_coeff(y, H3, H, y0a, y1a, ha0, ha1);
@@ -477,7 +418,6 @@ head_merge_kernel(const float* __restrict__ r4, const float* __restrict__ r3, co
         const int x = x0 + px;
         if (x < W) out[(((size_t)n * Cout + c) * H + y) * W + x] = tile[c][px];
     }
-    pdl_trigger();
 }
 cudaError_t launch_head_merge(const float* r4, const float* r3, const float* r2, int N, int H, int W, int H3, int W3,
                               int H2, int W2, int Cpad, int Cout, float* out, cudaStream_t st) {
@@ -497,7 +437,6 @@ tapsum_kernel(const float* __restrict__ T, const float* __restrict__ bias, int N
               float* __restrict__ out) {
     __shared__ float tile[16][33];
     const int x0 = blockIdx.x * 32, y = blockIdx.y, n = blockIdx.z;
-    pdl_wait();
     for (int i = threadIdx.x; i < 32 * C; i += 256) {
         const int px = i / C, c = i - px * C;
         const int x = x0 + px;
@@ -524,7 +463,6 @@ tapsum_kernel(const float* __restrict__ T, const float* __restrict__ bias, int N
         const int x = x0 + px;
         if (x < W) out[(((size_t)n * C + c) * H + y) * W + x] = tile[c][px];
     }
-    pdl_trigger();
 }
 cudaError_t launch_tapsum(const float* T, const float* bias, int N, int H, int W, int Cpad, int C, float* out,
                           cudaStream_t st) {
@@ -546,7 +484,6 @@ __constant__ int c_flip_pair[43] = {0, 1, 2, 9, 10, 11, 12, 13, 14, 3, 4, 5, 6, 
 __global__ void merge_scale_kernel(float* __restrict__ hm, const float* __restrict__ hm_flip, int B, int h, int w,
                                    int do_scale) {
     const long long total = (long long)B * 43 * h * w;
-    pdl_wait();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int x = (int)(i % w);
         long long r = i / w;
@@ -568,7 +505,6 @@ __global__ void merge_scale_kernel(float* __restrict__ hm, const float* __restri
         if (do_scale) v = (c < 15) ? __fmul_rn(v, __fdiv_rn(1.f, 255.f)) : __fmul_rn(v, __fdiv_rn(1.f, 127.f));
         hm[i] = v;
     }
-    pdl_trigger();
 }
 cudaError_t launch_merge_scale(float* hm, const float* hm_flip, int B, int h, int w, int do_scale, cudaStream_t st) {
     const long long total = (long long)B * 43 * h * w;

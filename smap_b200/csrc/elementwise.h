@@ -16,9 +16,6 @@ cudaError_t launch_s2d(const float* x_nchw, int N, int H, int W, __nv_bfloat16* 
                        cudaStream_t st, bool f16 = false, unsigned long long* sat = nullptr);
 cudaError_t launch_maxpool(const __nv_bfloat16* in, long long in_ps, int N, int H, int W, int C, __nv_bfloat16* out,
                            long long out_ps, int terms, cudaStream_t st, bool f16 = false);
-cudaError_t launch_upadd_relu(const __nv_bfloat16* a, long long a_ps, const __nv_bfloat16* t, long long t_ps, int N,
-                              int H, int W, int Hi, int Wi, int C, __nv_bfloat16* out, long long out_ps, int terms,
-                              cudaStream_t st, bool f16 = false, unsigned long long* sat = nullptr);
 cudaError_t launch_head_merge(const float* r4, const float* r3, const float* r2, int N, int H, int W, int H3, int W3,
                               int H2, int W2, int Cpad, int Cout, float* out, cudaStream_t st);
 cudaError_t launch_tapsum(const float* T, const float* bias, int N, int H, int W, int Cpad, int C, float* out,

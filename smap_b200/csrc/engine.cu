@@ -132,10 +132,6 @@ int smapb_create(smapb_handle** out, int device, int max_batch, int in_h, int in
     h->in_h = in_h, h->in_w = in_w;
     h->h = in_h / 4, h->w = in_w / 4;
     h->sm_count = prop.multiProcessorCount;
-    // SMs left free by the persistent conv grids (see smapb_comm_create): a conv CTA takes a whole SM (227 KB of shared
-    // memory), so any other resident CTA - a spinning NCCL channel, the other handle's grouping kernel - pushes one conv
-    // CTA into a second wave
-    if (getenv("SMAPB_SM_RESERVE")) h->sm_reserve = std::max(0, std::min(32, atoi(getenv("SMAPB_SM_RESERVE"))));
     const size_t hw = (size_t)h->h * h->w;
     const size_t MB = max_batch;
     int rc = 0;

@@ -39,7 +39,7 @@ struct ConvLayer {
     float* bias_dev = nullptr;       // [Cout_pad]
 };
 
-enum OpKind { OP_STEM, OP_S2D, OP_MAXPOOL, OP_CONV, OP_UPADD, OP_HEADMERGE, OP_TAPSUM };
+enum OpKind { OP_STEM, OP_S2D, OP_MAXPOOL, OP_CONV, OP_HEADMERGE, OP_TAPSUM };
 struct Op {
     OpKind kind;
     // conv
@@ -47,7 +47,7 @@ struct Op {
     int block_n = 0;
     double flops = 0;
     // generic tensors
-    Act a, b, out;
+    Act a, out;
     ActF32 f4, f3, f2;
     int cout = 0;  // head merge real channel count
     int which_out = 0;  // tap sum output: 1 detd, 2 rootd
@@ -79,7 +79,6 @@ struct Plan {
 struct smapb_handle {
     int device = 0, max_batch = 0, in_h = 0, in_w = 0, h = 0, w = 0;
     int sm_count = 132;
-    int sm_reserve = 0;  // SMs the persistent conv grids leave to concurrent kernels
     std::string err;
     int64_t launches = 0;
     // weights
@@ -113,7 +112,6 @@ struct smapb_handle {
     float* scratch_rootd = nullptr;
     double* scales_dev = nullptr;
     smapb_record* records_dev = nullptr;
-    bool use_pdl = getenv("SMAPB_PDL") != nullptr;  // programmatic dependent launch between conv kernels
     // host-facing pipeline (smapb_submit_host / smapb_wait): two slots, H2D of slot s+1 overlaps the compute of slot s
     struct Slot {
         float* imgs = nullptr;
@@ -125,7 +123,6 @@ struct smapb_handle {
     } slots[2];
     cudaStream_t copy_stream = nullptr;
     bool autotune = getenv("SMAPB_NO_AUTOTUNE") == nullptr;
-    bool two_streams = getenv("SMAPB_ONE_STREAM") == nullptr;  // side branches (heads, skip convs) on a second stream
     cudaStream_t aux_stream = nullptr;  // side branches of the decoder (skip convs, heads) run here
     // Stream used when the caller passes NULL (= the legacy default stream).  It is NON-blocking - a blocking stream would
     // be fenced by every legacy-stream operation of the process (e.g. a collective issued by the host framework) - and is
@@ -156,7 +153,6 @@ struct smapb_handle {
     double* gt_dist = nullptr;           // [max_batch][127*127] distance matrices of the GT-matching lift
     bool nccl_in_graph = getenv("SMAPB_NCCL_EAGER") == nullptr;
     bool nvtx_ops = getenv("SMAPB_NVTX") != nullptr;  // one NVTX range per plan op (phase ranges are always emitted)
-    bool serpentine = getenv("SMAPB_SERPENTINE") != nullptr;
     // pre-processing (SURVEY 8(f) f1): resampling tables per source geometry, staging for host images
     struct PreEntry {
         smapb::ResizePlan plan;

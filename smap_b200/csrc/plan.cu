@@ -114,7 +114,7 @@ int make_w_map(smapb_handle* h, CUtensorMap* m, const __nv_bfloat16* ptr, int Ci
 // conv launch
 // ------------------------------------------------------------------------------------------------
 template <int BN, int NT, int RING, class E>
-cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
+cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t st) {
     using Cfg = ConvCfg<BN, NT, RING>;
     static bool configured = false;
     if (!configured) {
@@ -124,38 +124,25 @@ cudaError_t launch_conv_inst2(const ConvParams& cp, int sm_count, cudaStream_t s
         configured = true;
     }
     const int units = cp.total_tiles < sm_count ? cp.total_tiles : sm_count;  // persistent CTAs
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(units);
-    cfg.blockDim = dim3(384);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    int na = 0;
-    if (pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        na++;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, NT, RING, E>, cp);
+    conv_tc_kernel<BN, NT, RING, E><<<units, 384, Cfg::SMEM_BYTES, st>>>(cp);
+    return cudaGetLastError();
 }
 // The RING variant a conv runs: 2 = fused bilinear residual, 1 = residual / skip tensors, 0 = no epilogue inputs
 int conv_ring(const ConvParams& cp) { return cp.up_mode ? 2 : (cp.has_res + cp.n_post) ? 1 : 0; }
 template <int BN, int NT, class E = ElemBF16>
-cudaError_t launch_conv_inst(const ConvParams& cp, int sm_count, cudaStream_t st, bool pdl) {
+cudaError_t launch_conv_inst(const ConvParams& cp, int sm_count, cudaStream_t st) {
     switch (conv_ring(cp)) {
-        case 2: return launch_conv_inst2<BN, NT, 2, E>(cp, sm_count, st, pdl);
-        case 1: return launch_conv_inst2<BN, NT, 1, E>(cp, sm_count, st, pdl);
-        default: return launch_conv_inst2<BN, NT, 0, E>(cp, sm_count, st, pdl);
+        case 2: return launch_conv_inst2<BN, NT, 2, E>(cp, sm_count, st);
+        case 1: return launch_conv_inst2<BN, NT, 1, E>(cp, sm_count, st);
+        default: return launch_conv_inst2<BN, NT, 0, E>(cp, sm_count, st);
     }
 }
-cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, bool f16, int sm_count, cudaStream_t st, bool pdl) {
-#define SMAPB_CASE(BN)                                                                  \
-    case BN:                                                                            \
-        if (f16) return launch_conv_inst<BN, 1, ElemF16>(cp, sm_count, st, pdl);        \
-        return nterms == 3 ? launch_conv_inst<BN, 3>(cp, sm_count, st, pdl)             \
-                           : launch_conv_inst<BN, 1>(cp, sm_count, st, pdl);
+cudaError_t launch_conv(const ConvParams& cp, int block_n, int nterms, bool f16, int sm_count, cudaStream_t st) {
+#define SMAPB_CASE(BN)                                                             \
+    case BN:                                                                       \
+        if (f16) return launch_conv_inst<BN, 1, ElemF16>(cp, sm_count, st);        \
+        return nterms == 3 ? launch_conv_inst<BN, 3>(cp, sm_count, st)             \
+                           : launch_conv_inst<BN, 1>(cp, sm_count, st);
     switch (block_n) {
         SMAPB_CASE(128)
         SMAPB_CASE(64)
@@ -361,7 +348,7 @@ int table_tile(smapb_handle* h, const ConvLayer& L, const ConvIO& io, int* bn) {
         float ms_best_c = 1e30f;
         for (int rep = 0; rep < 4; rep++) {
             cudaEventRecord(e0, nullptr);
-            if (launch_conv(trial, c, h->nterms, h->f16, h->sm_count, nullptr, false) != cudaSuccess) {
+            if (launch_conv(trial, c, h->nterms, h->f16, h->sm_count, nullptr) != cudaSuccess) {
                 ms_best_c = 1e30f;
                 break;
             }
@@ -561,15 +548,6 @@ struct PlanBuilder {
         a.ptr = (float*)alloc((size_t)N * H * W * C * 4, "fp32 tensor");
         return a;
     }
-    // SMAPB_SERPENTINE: a conv walks its tile list in the opposite direction of the op that produced its input, so that it
-    // starts with the rows written last (still in L2) instead of the ones written first (evicted by then)
-    int reverse_for(const void* in_ptr) {
-        if (!h->serpentine) return 0;
-        auto it = plan->producer.find(in_ptr);
-        if (it == plan->producer.end()) return 1;
-        const Op& prod = plan->ops[it->second];
-        return prod.kind == OP_CONV ? !prod.cp.reverse : 1;
-    }
     const ConvLayer* layer(const std::string& name) {
         auto it = h->layers.find(name);
         if (it == h->layers.end()) {
@@ -601,7 +579,6 @@ struct PlanBuilder {
         if (!rc) rc = setup_conv(h, *L, io, op.block_n, &op.cp);
         op.flops = 2.0 * in.N * Ho * Wo * (double)L->Cout * (L->Cin * L->k * L->k + L->Cin2);
         op.name = name;
-        op.cp.reverse = reverse_for(in.ptr);
         op.dims[0] = in.N, op.dims[1] = Ho, op.dims[2] = Wo, op.dims[3] = L->Cout_pad;
         plan->ops.push_back(op);
         wire(f32 ? (const void*)f32->ptr : out.ptr, io.inputs());
@@ -628,21 +605,21 @@ std::string debug_op_desc(const smapb_handle* h, const Op& op, const std::map<co
     const bool stem_tc = is_conv && op.cp.kh == 4 && op.cp.kw == 1;
     const char* kind = is_conv ? (stem_tc ? "stem_tc" : op.cp.out ? "conv" : "conv_f32")
                        : op.kind == OP_STEM ? "stem" : op.kind == OP_S2D ? "s2d" : op.kind == OP_MAXPOOL ? "maxpool"
-                       : op.kind == OP_UPADD ? "upadd" : "other";
+                       : "other";
     std::string s = "name=" + (op.name.empty() ? std::string("?") : op.name) + " kind=" + kind;
     if (op.kind == OP_STEM || op.kind == OP_S2D) s += " in=x";  // the network input image
     for (size_t r = 0; r < op.inputs.size(); r++) {
         if (!op.inputs[r]) continue;
-        const char* role = is_conv ? (r < 6 ? CONV_ROLES[r] : "?") : (r == 0 ? "a" : "b");
+        const char* role = is_conv ? (r < 6 ? CONV_ROLES[r] : "?") : "a";
         auto it = dump_idx.find(op.inputs[r]);
         s += std::string(" ") + role + "=" + (it == dump_idx.end() ? std::string("?") : std::to_string(it->second));
     }
     char buf[320];
     if (is_conv) {
         snprintf(buf, sizeof buf,
-                 " tw=%d rev=%d k=%dx%d s=%d pad=%dx%d cin=%d cin2=%d s2=%d cout=%d out=%dx%dx%dx%d bn=%d relu=%d "
+                 " tw=%d k=%dx%d s=%d pad=%dx%d cin=%d cin2=%d s2=%d cout=%d out=%dx%dx%dx%d bn=%d relu=%d "
                  "hasres=%d post=%d upmode=%d tiles=%d nterms=%d",
-                 1 << op.cp.tw_log2, op.cp.reverse, op.cp.kh, op.cp.kw, op.cp.stride, op.cp.pad_y, op.cp.pad_x,
+                 1 << op.cp.tw_log2, op.cp.kh, op.cp.kw, op.cp.stride, op.cp.pad_y, op.cp.pad_x,
                  op.cp.kchunks * 64, op.cp.kchunks2 * 64, op.cp.stride2, op.cp.Cout, op.dims[0], op.dims[1], op.dims[2],
                  op.dims[3], op.block_n, op.cp.relu, op.cp.has_res, op.cp.n_post, op.cp.up_mode, op.cp.total_tiles,
                  h->nterms);
@@ -757,14 +734,10 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan) {
                 Act o2 = pb.conv(p + "conv_bn_relu2", {&o1, 1});
                 const bool last = (b == LAYERS[li] - 1) && s > 0;
                 ConvIO c3{&o2, 1};
-                if (b == 0 && !getenv("SMAPB_NO_FUSE_DS")) {
+                if (b == 0) {
                     // relu(conv3(o2) + downsample(x)) as one K-concatenated GEMM
                     c3.in2 = &t;
                     t = pb.conv(p + "fused_conv3_downsample", c3);
-                } else if (b == 0) {  // debug: separate downsample + residual
-                    Act idn = pb.conv(p + "downsample", {&t, 0});
-                    c3.res = &idn;
-                    t = pb.conv(p + "conv_bn_relu3", c3);
                 } else {
                     // out = relu(conv3 + x) [ + skip1 + skip2 ]   (model/smap.py:74-75,143)
                     c3.res = &t;
@@ -788,25 +761,13 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan) {
                 // interpolation (both linear, bilinear weights sum to 1) and the interpolation + add + ReLU run in the
                 // u_skip epilogue
                 Act tl = pb.conv(p + "up_conv", {&up_x, 0});
-                if (!getenv("SMAPB_NO_FUSE_UP")) {
-                    ConvIO io{&xin, 1};
-                    io.up = &tl;
-                    out = pb.conv(p + "u_skip", io);
-                } else {  // debug: separate bilinear + add + relu kernel
-                    Act a = pb.conv(p + "u_skip", {&xin, 0});
-                    out = pb.new_act(a.N, a.H, a.W, a.C);
-                    Op op;
-                    op.kind = OP_UPADD;
-                    op.a = a;
-                    op.b = tl;
-                    op.out = out;
-                    plan->ops.push_back(op);
-                    pb.wire(out.ptr, {a.ptr, tl.ptr});
-                }
+                ConvIO io{&xin, 1};
+                io.up = &tl;
+                out = pb.conv(p + "u_skip", io);
             }
             // Side branches (heads, skip convs) hang off `out` / `xin` and are only needed much later: they go to the
             // second stream and overlap the main chain, filling SMs that small layers leave idle.
-            pb.cur_stream = h->two_streams ? 1 : 0;
+            pb.cur_stream = 1;
             // heads: only those that reach the returned tensors (model/smap.py:418-419) are computed
             if (s == 2 && ind >= 1) {
                 Act r1 = pb.conv(p + "res_conv1", {&out, 1});
@@ -907,9 +868,9 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
                 if (h->profiling && h->roles_dev && h->roles_used < ROLES_CAP) {
                     ConvParams cp = op.cp;  // same launch with the wait-cycle counters of every warp role switched on
                     cp.dbg = h->roles_dev + 16 * h->roles_used++;
-                    CK(launch_conv(cp, op.block_n, h->nterms, h->f16, h->sm_count - h->sm_reserve, st, h->use_pdl));
+                    CK(launch_conv(cp, op.block_n, h->nterms, h->f16, h->sm_count, st));
                 } else {
-                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->f16, h->sm_count - h->sm_reserve, st, h->use_pdl));
+                    CK(launch_conv(op.cp, op.block_n, h->nterms, h->f16, h->sm_count, st));
                 }
                 if (h->profiling) {
                     char d[160];
@@ -919,11 +880,6 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
                     prof_mark(h, PK_CONV, st, d, op.flops);
                     if (h->roles_dev) h->roles_desc.push_back(op.name + "," + d);
                 }
-                break;
-            case OP_UPADD:
-                CK(launch_upadd_relu(op.a.ptr, op.a.plane(), op.b.ptr, op.b.plane(), B, op.a.H, op.a.W, op.b.H, op.b.W,
-                                     op.a.C, op.out.ptr, op.out.plane(), T, st, h->f16, h->sat_dev));
-                prof_mark(h, PK_ELEM, st, "upadd_relu");
                 break;
             case OP_TAPSUM: {
                 float* dst = op.which_out == 1 ? detd : rootd;
@@ -980,18 +936,20 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
             units.push_back(k.substr(0, k.size() - suf.size()));
     }
     if (units.empty()) return fail(h, -40, "no weights loaded");
-    std::map<std::string, std::pair<std::vector<float>, std::vector<float>>> folded;  // 1x1 units of bottleneck pairs
+    struct Folded {
+        ConvLayer L;  // the unit's geometry
+        std::vector<float> w, b;
+    };
+    std::map<std::string, Folded> folded;  // units the loops below build other layers from
     for (const std::string& name : units) {
         std::vector<float> wf, bf;
         int Cout, Cin, k;
         int rc = fold_unit(h, name, &wf, &bf, &Cout, &Cin, &k);
         if (rc) return rc;
-        if (name.find(".downsample.layer") != std::string::npos &&
-            (name.find(".0.conv_bn_relu3") != std::string::npos ||
-             (name.size() > 13 && name.compare(name.size() - 13, 13, ".0.downsample") == 0)))
-            folded[name] = {wf, bf};
-        if (name.find("res_d_conv2") != std::string::npos || name.find("res_rd_conv2") != std::string::npos)
-            folded[name] = {wf, bf};
+        // conv3 and downsample of a layer's first bottleneck: the plan only runs them as their fused pair
+        const bool pair_half = name.find(".downsample.layer") != std::string::npos &&
+                               (name.find(".0.conv_bn_relu3") != std::string::npos ||
+                                (name.size() > 13 && name.compare(name.size() - 13, 13, ".0.downsample") == 0));
         if (name == "top.conv") {
             if (Cin != 3 || Cout != 64 || k != 7) return fail(h, -40, "top.conv must be 3->64 7x7");
             std::vector<float> w2(147 * 64);
@@ -1026,7 +984,8 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
             if (rc) return rc;
             continue;
         }
-        ConvLayer& L = h->layers[name];
+        ConvLayer unit;
+        ConvLayer& L = pair_half ? unit : h->layers[name];
         L.name = name;
         L.Cin = Cin;
         L.Cout = Cout;
@@ -1046,6 +1005,13 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
                 if (li >= 2 && first && (is_c2 || is_ds)) L.stride = 2;
             }
         }
+        if (pair_half) {
+            if (h->f16 && check_f16_range(h, name, wf.data(), wf.size())) return -42;
+            folded[name] = {L, std::move(wf), std::move(bf)};
+            continue;
+        }
+        if (name.find("res_d_conv2") != std::string::npos || name.find("res_rd_conv2") != std::string::npos)
+            folded[name] = {L, wf, bf};
         int rc2 = upload_conv_layer(h, L, k * k, wf, bf);
         if (rc2) return rc2;
     }
@@ -1059,8 +1025,8 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
         const std::string base = n3.substr(0, pos), nds = base + ".0.downsample";
         auto ids = folded.find(nds);
         if (ids == folded.end()) return fail(h, -40, "missing downsample unit for " + n3);
-        const ConvLayer& L3 = h->layers[n3];
-        const ConvLayer& Lds = h->layers[nds];
+        const ConvLayer& L3 = kv.second.L;
+        const ConvLayer& Lds = ids->second.L;
         ConvLayer& F = h->layers[base + ".0.fused_conv3_downsample"];
         F.name = base + ".0.fused_conv3_downsample";
         F.Cin = L3.Cin;
@@ -1072,10 +1038,9 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
         const int cin = F.Cin + F.Cin2;
         std::vector<float> wf((size_t)F.Cout * cin), bf(F.Cout);
         for (int co = 0; co < F.Cout; co++) {
-            for (int ci = 0; ci < F.Cin; ci++) wf[(size_t)co * cin + ci] = kv.second.first[(size_t)co * F.Cin + ci];
-            for (int ci = 0; ci < F.Cin2; ci++)
-                wf[(size_t)co * cin + F.Cin + ci] = ids->second.first[(size_t)co * F.Cin2 + ci];
-            bf[co] = kv.second.second[co] + ids->second.second[co];
+            for (int ci = 0; ci < F.Cin; ci++) wf[(size_t)co * cin + ci] = kv.second.w[(size_t)co * F.Cin + ci];
+            for (int ci = 0; ci < F.Cin2; ci++) wf[(size_t)co * cin + F.Cin + ci] = ids->second.w[(size_t)co * F.Cin2 + ci];
+            bf[co] = kv.second.b[co] + ids->second.b[co];
         }
         int rc3 = upload_conv_layer(h, F, 1, wf, bf);
         if (rc3) return rc3;
@@ -1084,7 +1049,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
     for (auto& kv : folded) {
         const std::string& nm = kv.first;
         if (nm.find("res_d_conv2") == std::string::npos && nm.find("res_rd_conv2") == std::string::npos) continue;
-        const ConvLayer& L0 = h->layers[nm];
+        const ConvLayer& L0 = kv.second.L;
         if (L0.k != 3) continue;
         ConvLayer& E = h->layers[nm + ".tapexp"];
         E.name = nm + ".tapexp";
@@ -1096,7 +1061,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
         for (int c = 0; c < L0.Cout; c++)
             for (int ci = 0; ci < L0.Cin; ci++)
                 for (int t = 0; t < 9; t++)
-                    wf[(size_t)(t * L0.Cout + c) * E.Cin + ci] = kv.second.first[((size_t)c * L0.Cin + ci) * 9 + t];
+                    wf[(size_t)(t * L0.Cout + c) * E.Cin + ci] = kv.second.w[((size_t)c * L0.Cin + ci) * 9 + t];
         int rc4 = upload_conv_layer(h, E, 1, wf, bf);
         if (rc4) return rc4;
     }
@@ -1357,7 +1322,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         CKT(cudaMalloc((void**)&tl_dev, 16 * sizeof(long long)));
         tmp.push_back(tl_dev);
     }
-    CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));  // warm-up + result
+    CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));  // warm-up + result
     cp.sat = nullptr;  // the saturation counter counts the result launch; the time-line and timed re-runs leave it alone
     if (dbg_dev) {
         long long d[16];
@@ -1378,7 +1343,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     if (tl_dev) {  // time line of CTA 0 of one warm launch (cycles since kernel entry)
         CKT(cudaMemset(tl_dev, 0, 16 * sizeof(long long)));
         cp.dbg_tl = tl_dev;
-        CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));
+        CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
         cp.dbg_tl = nullptr;
         long long t[16];
         CKT(cudaMemcpy(t, tl_dev, sizeof t, cudaMemcpyDeviceToHost));
@@ -1388,7 +1353,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     }
     const int reps = ms_out ? 5 : 0;
     cudaEventRecord(e0, st);
-    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st, false));
+    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
     cudaEventRecord(e1, st);
     h->launches += 1 + reps;
     // convert (split outputs) + de-pad

@@ -1,6 +1,6 @@
 """The per-op checker of the backbone plan, one for every precision (bf16x3, bf16, fp16), and what the GPU tests around
 it share: plan introspection (smapb_debug_checksums, smapb_debug_dump), float64 references of one layer fed the exact
-inputs the op consumed, the op loop check_ops, plan switches that must not change a bit, and the single-conv checker
+inputs the op consumed, the op loop check_ops, forced tile widths that must not change a bit, and the single-conv checker
 (conv_op, check_conv: a conv_test call described as a plan op and judged by the same judge()) of
 tests/test_conv_gpu.py, tests/test_fp16_gpu.py and tests/test_conv_edges_gpu.py.
 
@@ -35,7 +35,7 @@ MAX_OPS = 1024
 TOL_HEADS = 1e-5
 FP16_MAX = 65504.0
 SEED = 5
-ROLES = ("in", "in2", "res", "p1", "p2", "up", "a", "b")  # the inputs an op description may name
+ROLES = ("in", "in2", "res", "p1", "p2", "up", "a")  # the inputs an op description may name
 
 
 def no_tf32():
@@ -301,10 +301,6 @@ def reference(op, get, wts, image, mut=None, squares=False, get_lo=None):
         W, b, Wlo = unit(name)
         r = cv("in", W, Wlo, pad=int(op["pad"].split("x")[0])) + b
         return r, r, False
-    if kind == "upadd":
-        a, t = A(get("a")), A(get("b"))
-        pre = a + _up(t, a.shape[1], a.shape[2], mut != "align_false")
-        return (pre if squares else F.relu(pre)), pre, True
     assert kind == "conv", "no reference for op kind %r (%s)" % (kind, name)
     stride, pad = int(op["s"]), int(op["pad"].split("x")[0])
     def last_kb(W, Wlo):  # the weights of the conv's last k-block (tap ky = kh-1, kx = kw-1, last 64 channels) zeroed
@@ -373,7 +369,7 @@ def half_ulp16(y):
 
 def _K(op):
     """Products one output element accumulates.  The CUDA-core stem: 7x7x3 fp32 FMAs (then the bias, one of the 8
-    roundings _acc_bound adds).  upadd: none; its bilinear term and add are 7 fp32 roundings, within those 8."""
+    roundings _acc_bound adds)."""
     if op["kind"] == "stem":
         return 147
     kh, kw = (int(v) for v in op.get("k", "1x1").split("x"))
@@ -430,7 +426,7 @@ def clamp_check(y, r, b):
 # per-op parity of one plan
 # ---------------------------------------------------------------------------------------------------------------------
 _MUTATIONS = {  # deliberately wrong reference -> op classes it applies to (largest_k: the conv with the most products)
-    "align_false": ("up_residual", "upadd"),
+    "align_false": ("up_residual",),
     "drop_post2": ("res_p1_p2",),
     "shift_ds": ("fused_pair_s2",),
     "bias_shift": ("conv1x1",),
@@ -701,7 +697,7 @@ def assert_checked(s, precision):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# plan switches do not change the bits
+# forced tile widths do not change the bits
 # ---------------------------------------------------------------------------------------------------------------------
 def run_sums(H, W, B, sd, x, precision):
     from smap_b200.engine import Engine
@@ -718,9 +714,9 @@ def run_sums(H, W, B, sd, x, precision):
 
 
 def check_switches(geom, monkeypatch, precision):
-    """Reverse tile order, PDL, one stream and every forced tile width (tile table rewritten, autotuner off) give every op
-    of the plan at geometry (H, W, B) in `precision` the bits of the default plan.  (Switches held in function-local
-    statics, SMAPB_NO_GRAPH / SMAPB_DEBUG_STOP, cannot be toggled in one process.)"""
+    """Every forced tile width (tile table rewritten, autotuner off) gives every op of the plan at geometry (H, W, B) in
+    `precision` the bits of the default plan.  (Switches held in function-local statics, SMAPB_NO_GRAPH /
+    SMAPB_DEBUG_STOP, cannot be toggled in one process.)"""
     from smap_b200 import _lib
     from smap_b200.engine import get_tile_table
 
@@ -735,14 +731,6 @@ def check_switches(geom, monkeypatch, precision):
         assert not diff, "%s: %d ops differ from the default plan, first %s" % (tag, len(diff), diff[:3])
         for a, b in zip(outs, base_outs):
             assert torch.equal(a, b), tag
-
-    for var in ("SMAPB_SERPENTINE", "SMAPB_PDL", "SMAPB_ONE_STREAM"):
-        with monkeypatch.context() as m:
-            m.setenv(var, "1")
-            sums, ops, outs = run_sums(H, W, B, sd, x, precision)
-        if var == "SMAPB_SERPENTINE":
-            assert any(o.get("rev") == "1" for o in ops) and all(o.get("rev", "0") == "0" for o in base_ops)
-        same(var, sums, ops, outs)
 
     lib = _lib.load()
     table = get_tile_table()

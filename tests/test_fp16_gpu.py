@@ -7,8 +7,8 @@
   * saturation: outputs beyond +-65504 are exactly +-65504, never inf / NaN, and counted; folded weights beyond the range
     are rejected by finalize;
   * every op of the real plan against a float64 reference of its own layer, by the checker of tests/plan_check.py that
-    tests/test_plan_ops_gpu.py runs for bf16x3 and bf16 (wrong references flagged, heads checked), and plan switches
-    that must not change a bit;
+    tests/test_plan_ops_gpu.py runs for bf16x3 and bf16 (wrong references flagged, heads checked), and forced tile
+    widths that must not change a bit;
   * the whole backbone against the fp32 oracle next to bf16 and cuDNN with TF32 (the reference's own GPU numerics);
   * the whole path (records) on bench.py's first batch next to bf16x3.
 
@@ -145,17 +145,19 @@ def test_saturation_clamps_counts_and_resets(eng):
 def test_finalize_rejects_weights_beyond_the_fp16_range():
     from smap_b200.engine import Engine, SmapB200Error
 
-    sd = smap_torch.make_state_dict(0, "identity")
-    unit = "stage1.downsample.layer2.1.conv_bn_relu2"
-    sd[unit + ".conv.weight"] = sd[unit + ".conv.weight"].clone()
-    sd[unit + ".conv.weight"][3, 1, 0, 0] = 1.0e5
+    x = smap_torch.make_input(1, 64, 96, seed=1).cuda()
     e = Engine(0, max_batch=1, in_h=64, in_w=96)
     try:
-        with pytest.raises(SmapB200Error, match=unit.replace(".", r"\.")):
-            e.load_state_dict(sd, "fp16")
-        x = smap_torch.make_input(1, 64, 96, seed=1).cuda()
-        with pytest.raises(SmapB200Error, match="not finalized"):
-            e.forward(x)
+        # a unit the plan runs on its own, and one it runs only inside a fused conv3 + downsample pair: the error names
+        # the state-dict unit either way
+        for unit in ("stage1.downsample.layer2.1.conv_bn_relu2", "stage0.downsample.layer3.0.downsample"):
+            sd = dict(smap_torch.make_state_dict(0, "identity"))
+            sd[unit + ".conv.weight"] = sd[unit + ".conv.weight"].clone()
+            sd[unit + ".conv.weight"][3, 1, 0, 0] = 1.0e5
+            with pytest.raises(SmapB200Error, match=unit.replace(".", r"\.") + " exceeds"):
+                e.load_state_dict(sd, "fp16")
+            with pytest.raises(SmapB200Error, match="not finalized"):
+                e.forward(x)
         e.load_state_dict(sd, "bf16x3")  # bf16 keeps fp32's range
         e.forward(x)
         torch.cuda.synchronize()
@@ -180,7 +182,7 @@ def test_plan_ops_fp16(geom):
 
 
 @pytest.mark.parametrize("geom", [(64, 96, 2), (512, 832, 2)], ids=_gid)
-def test_fp16_plan_switches_keep_the_bits(geom, monkeypatch):
+def test_fp16_forced_tile_widths_keep_the_bits(geom, monkeypatch):
     from smap_b200.engine import get_tile_table
 
     check_switches(geom, monkeypatch, "fp16")

@@ -1,5 +1,5 @@
 """GPU: fp16's range guard.  In the fp16 precision every kernel that stores an fp16 activation it computed (the conv epilogue
-in all its variants, the CUDA-core stem, s2d, upadd_relu) must store exactly +-65504 for a value beyond the range, never
+in all its variants, the CUDA-core stem, s2d) must store exactly +-65504 for a value beyond the range, never
 inf or NaN, and add one to the handle's saturation counter per clamped element - the counter is the only sign a user gets
 that the outputs are not the model's.
 
@@ -12,7 +12,7 @@ A forward's device count must lie in [sum sure-over, sum sure-over + sum band] o
 dicts keep the band smaller than the sure-over count of every op class that saturates, so a class whose clamps go
 uncounted (or a count of rows outside the output) fails.
 
-  * whole plans (default, and the CUDA-core stem + upadd_relu fallback) at 96x64 B2, 288x224 B5 (odd levels: partial tiles
+  * whole plans (default, and the CUDA-core stem fallback) at 96x64 B2, 288x224 B5 (odd levels: partial tiles
     both ways) and 32x32 B2 (1x1 deepest level, flat M = 2), with state dicts that drive chosen units over the range
     through their BN bias (positive, and negative on a unit without a ReLU) and keep the saturated channels from
     spreading: consumers' weights on them are zeroed, residual consumers' biases send them below the ReLU;
@@ -43,8 +43,7 @@ GEOMS = [(64, 96, 2), (224, 288, 5), (32, 32, 2)]
 PLANS = {
     "default": ({}, ("conv1x1", "conv3x3", "residual", "fused_pair_s1", "fused_pair_s2", "up_residual", "res_p1_p2",
                      "stem_tc")),
-    "cuda_stem_upadd": ({"SMAPB_STEM": "cuda", "SMAPB_NO_FUSE_UP": "1"},
-                        ("conv3x3", "residual", "fused_pair_s2", "res_p1_p2", "stem", "upadd")),
+    "cuda_stem": ({"SMAPB_STEM": "cuda"}, ("conv3x3", "residual", "fused_pair_s2", "res_p1_p2", "stem")),
 }
 
 
@@ -77,7 +76,7 @@ def op_graph(H, W, B):
     """The plan's op descriptions under the current environment (they do not depend on the weights)."""
     from smap_b200.engine import Engine
 
-    key = (H, W, B, os.environ.get("SMAPB_STEM"), os.environ.get("SMAPB_NO_FUSE_UP"))
+    key = (H, W, B, os.environ.get("SMAPB_STEM"))
     if key not in _GRAPHS:
         eng = Engine(0, max_batch=B, in_h=H, in_w=W)
         try:
@@ -108,8 +107,6 @@ def _containable(ops, uses, i, sign):
                 continue
             elif c["kind"] == "conv" and role in ("res", "up") and int(c["relu"]) and "p1" not in c:
                 continue
-            elif c["kind"] == "upadd" and role == "b" and sign < 0:
-                continue
             else:
                 return False
     return True
@@ -132,8 +129,6 @@ def _contain(sd, ops, uses, i, cs, sign):
 def _units_of_target(ops, op):
     if op["kind"] in ("stem_tc", "stem"):
         return ["top.conv"]
-    if op["kind"] == "upadd":  # both inputs over the range: the sum is ~2 x 65504
-        return [ops[int(op["a"])]["name"], ops[int(op["b"])]["name"]]
     return [_unit_of(op, "in")]
 
 

@@ -4,17 +4,17 @@ plan paths no other test builds, and the association at map sizes that take its 
   * edge geometries (in_h x in_w, B): 32x32 B=2 (deepest level 1x1, flat M = 2), 32x992 B=2 (levels one row high),
     1024x32 B=1 (levels one column wide, 64x2 levels tiled tw = 2), 224x288 B=5 (odd levels 7x9 ... 56x72, ragged flat
     M): every op against its float64 reference, every wrong reference that applies flagged;
-  * the fallback plans (SMAPB_STEM=cuda: the CUDA-core stem; SMAPB_NO_FUSE_DS: a separate 1x1 stride-2 downsample and a
-    residual conv; SMAPB_NO_FUSE_UP: upadd_relu_kernel after a plain u_skip conv), which include/smap_b200_debug.h
-    recommends for bisection, checked the same way;
+  * the fallback plan (SMAPB_STEM=cuda: the CUDA-core stem, which the library also takes when the driver rejects the
+    tensor-core stem's overlapped TMA view), checked the same way;
   * plans with B < max_batch on one handle give every op the bits of the same images in the B = max_batch plan;
   * forced tile widths change no bit at the edge geometries;
   * association (extract, connect) bit-exact against the oracle at heat-map sizes with h*w % 128 != 0 (scalar NMS flag
     kernel), with peaks on and next to the border;
   * the whole path (records) against the oracle chain at small geometries, and two handles of different geometry
     alternating in one process.
-Coverage assertions (test_edge_plans_cover_what_they_are_for) read the op descriptions, so that this file cannot quietly
-stop checking what it is for.  `-s` prints the worst |y - r| / bound per op kind of every checked plan."""
+Coverage assertions (test_edge_and_stem_fallback_plans_cover_what_they_are_for) read the op descriptions, so that this
+file cannot quietly stop checking what it is for.  `-s` prints the worst |y - r| / bound per op kind of every checked
+plan."""
 import os
 import sys
 
@@ -34,8 +34,7 @@ pytestmark = pytest.mark.gpu
 
 EDGE_GEOMS = [(32, 32, 2), (32, 992, 2), (1024, 32, 1), (224, 288, 5)]  # all in bf16x3
 SMALL_GEOMS = [(32, 32, 2), (1024, 32, 1)]  # also in bf16 and fp16
-FALLBACKS = {"stem_cuda": ("SMAPB_STEM", "cuda"), "no_fuse_ds": ("SMAPB_NO_FUSE_DS", "1"),
-             "no_fuse_up": ("SMAPB_NO_FUSE_UP", "1")}
+FALLBACKS = {"stem_cuda": ("SMAPB_STEM", "cuda")}
 FALLBACK_RUNS = [("bf16x3", (32, 32, 2)), ("fp16", (32, 32, 2)), ("bf16x3", (96, 160, 3)), ("fp16", (96, 160, 3)),
                  ("bf16x3", (512, 832, 2))]
 
@@ -60,19 +59,13 @@ def test_fallback_plan_ops(fallback, precision, geom):
     s = plan_summary(precision, geom, FALLBACKS[fallback])
     assert_checked(s, precision)
     ops = s["ops"]
-    kinds, classes = {o["kind"] for o in ops}, {op_class(o) for o in ops}
-    if fallback == "stem_cuda":  # the CUDA-core stem replaces s2d + the tensor-core stem
-        assert "stem" in kinds and not kinds & {"stem_tc", "s2d"}, kinds
-    elif fallback == "no_fuse_ds":  # a separate downsample conv (1x1 stride 2 in layers 2-4) + a residual conv3
-        assert not classes & {"fused_pair_s1", "fused_pair_s2"}, classes
-        ds = [o for o in ops if o["kind"] == "conv" and o["name"].endswith(".downsample")]
-        assert ds and any(o["k"] == "1x1" and o["s"] == "2" for o in ds), [o["name"] for o in ds]
-    else:  # upadd_relu after a plain u_skip conv
-        assert "upadd" in kinds and "up_residual" not in classes, classes
+    kinds = {o["kind"] for o in ops}
+    # the CUDA-core stem replaces s2d + the tensor-core stem
+    assert "stem" in kinds and not kinds & {"stem_tc", "s2d"}, kinds
 
 
-def test_edge_plans_cover_what_they_are_for():
-    """Across this file's checked plans: 1-pixel levels, images smaller than one tile, tw = 2, and the fallback kinds."""
+def test_edge_and_stem_fallback_plans_cover_what_they_are_for():
+    """Across this file's checked plans: 1-pixel levels, images smaller than one tile, tw = 2, and the fallback stem."""
     runs = [plan_summary("bf16x3", g) for g in EDGE_GEOMS]
     runs += [plan_summary(p, g) for p in ("bf16", "fp16") for g in SMALL_GEOMS]
     runs += [plan_summary(p, g, FALLBACKS[f]) for f in sorted(FALLBACKS) for p, g in FALLBACK_RUNS]
@@ -80,8 +73,8 @@ def test_edge_plans_cover_what_they_are_for():
     for s in runs:
         ops = s["ops"]
         for o in ops:
-            if o["kind"] in ("stem", "upadd"):
-                seen.add("kind " + o["kind"])
+            if o["kind"] == "stem":
+                seen.add("kind stem")
             if o["kind"] not in ("conv", "conv_f32"):
                 continue
             N, H, W, _ = _dims(o)
@@ -101,15 +94,13 @@ def test_edge_plans_cover_what_they_are_for():
             if not flat and tw == 2:
                 seen.add("tw = 2")
     need = {"conv with a 1-pixel output dimension", "3x3 conv on a 1x1 input", "up-residual from a 1-pixel level",
-            "flat conv with N*Ho*Wo < 128", "patch conv on an image smaller than one tile", "tw = 2", "kind stem",
-            "kind upadd"}
+            "flat conv with N*Ho*Wo < 128", "patch conv on an image smaller than one tile", "tw = 2", "kind stem"}
     assert need <= seen, "not covered: %s" % sorted(need - seen)
 
 
 @pytest.mark.parametrize("geom", [(1024, 32, 1), (224, 288, 5)], ids=_gid)
-def test_edge_geometry_plan_switches_keep_the_bits(geom, monkeypatch):
-    """Reverse tile order, PDL, one stream and every forced tile width (tile table rewritten, autotuner off) give the
-    bits of the autotuned plan."""
+def test_edge_geometry_forced_tile_widths_keep_the_bits(geom, monkeypatch):
+    """Every forced tile width (tile table rewritten, autotuner off) gives the bits of the autotuned plan."""
     check_switches(geom, monkeypatch, "bf16x3")
 
 

@@ -7,8 +7,8 @@ checker of tests/plan_check.py (check_ops; the bounds are given there).  For bf1
 per-channel max|y - r| / max|r_channel| (floored at 1e-3 max|r|) against the device-operand reference and against the
 float64 layer computed from the unfolded state dict.  It is not asserted: channels that the ReLU or cancellation leave
 small carry the error of their inputs' magnitude (up to a few 1e-3 at 832x512).
-The checker is shown to flag deliberately wrong references, and plan switches (reverse tile order, PDL, one stream,
-forced tile widths) are shown not to change a single bit of any op, in bf16x3 and in bf16."""
+The checker is shown to flag deliberately wrong references, and forced tile widths are shown not to change a single bit
+of any op, in bf16x3 and in bf16."""
 import os
 import re
 import sys
@@ -55,7 +55,7 @@ def test_checker_flags_wrong_references(precision):
 def test_plan_op_coverage():
     """Across the checked geometries every op kind of interest occurs, and no dumped op went unchecked."""
     seen, bns, up_tw, up_levels = set(), set(), set(), set()
-    known = {"s2d", "stem_tc", "stem", "maxpool", "upadd", "conv_f32", "conv"}
+    known = {"s2d", "stem_tc", "stem", "maxpool", "conv_f32", "conv"}
     for g in BF16X3_GEOMS:
         for op in plan_summary("bf16x3", g)["ops"]:
             assert op["kind"] in known, op  # check_ops fails on any kind it has no reference for
@@ -76,7 +76,7 @@ def test_plan_op_coverage():
 
 @pytest.mark.parametrize("geom", SWITCH_GEOMS, ids=_gid)
 @pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
-def test_plan_switches_keep_the_bits(precision, geom, monkeypatch):
-    """Reverse tile order, PDL, one stream and every forced tile width give every op the same bits as the default plan.
-    (Switches held in function-local statics, SMAPB_NO_GRAPH / SMAPB_DEBUG_STOP, cannot be toggled in one process.)"""
+def test_forced_tile_widths_keep_the_bits(precision, geom, monkeypatch):
+    """Every forced tile width gives every op the same bits as the default plan.  (Switches held in function-local
+    statics, SMAPB_NO_GRAPH / SMAPB_DEBUG_STOP, cannot be toggled in one process.)"""
     check_switches(geom, monkeypatch, precision)
