@@ -221,6 +221,28 @@ int smapb_submit_host(smapb_handle* h, int slot, const float* imgs_nchw_host, co
                       smapb_record* records_host);
 int smapb_wait(smapb_handle* h, int slot);
 
+/* ---- JPEG encoding (annotated frames; run_inference --vis_dir) -------------------------------------------------------- */
+/* Encodes n uint8 BGR frames bgr_dev[i] [img_h[i], img_w[i], 3] (device, sides 1..16384, not modified) into the bytes
+ * cv2.imencode(".jpg", frame, [IMWRITE_JPEG_QUALITY, quality]) writes (libjpeg-turbo's defaults: baseline, 4:2:0, standard
+ * Huffman tables, JFIF APP0), quality 1..100.  records_dev (NULL: none) are smapb_record[n] as smapb_infer_device wrote
+ * them, with scales_dev float64 [n][SMAPB_SCALE_LEN] the frames' scale rows: each frame is encoded with its skeletons
+ * drawn opaquely over it.
+ * Overlay: joint j of row p < count is drawn when pred2d[p][j][3] > 0; its frame pixel is rint((x - pad_l) / scale),
+ * rint((y - pad_t) / scale) in float64 (half to even, clamped to +-32768), with pad_l / pad_t the integer letterbox
+ * smapb_preprocess applied.  Limbs are the 14 joint pairs of lib/preprocess/data_format.md whose joints are both drawn.
+ * A pixel is in a joint's disc if its squared distance to it is <= R^2, and in a limb a-b if, by the clamped projection
+ * of (p - a) . (b - a), its squared distance to the nearer endpoint is <= r^2 or cross^2 <= r^2 |b - a|^2 (exact integers).
+ * r = max(1, min(w, h) / 400), R = max(2, min(w, h) / 200) (integer division).  Painter's order: persons in row order,
+ * each one's limbs then its joints; limbs take the person's colour, cycling through BGR (0,0,255), (0,255,0), (255,0,0),
+ * (0,255,255), (0,0,0), (255,0,255) as lib/visualize/vis.py cycles its colours; joints are white.
+ * nbytes_host[i] receives each stream's size; smapb_encoded_jpeg gives its bytes, in a pinned buffer the handle owns, valid
+ * until the next smapb_encode_jpeg on the handle.  Each phase is one launch for the whole batch; the workspace grows on
+ * demand; the call synchronises `stream`, so it cannot be captured into a CUDA graph. */
+int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
+                      const smapb_record* records_dev, const double* scales_dev, int64_t* nbytes_host, void* stream);
+/* Stream i of the last smapb_encode_jpeg: *data = its first byte, *nbytes (may be NULL) its size.  -1 for i out of range. */
+int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes);
+
 /* ---- multi-GPU: frames are sharded over ranks, ONE exchange step per batch --------------------------------------- */
 /* The reference's inference path is single-GPU (exps/stage3_root2/test.py:198 calls get_test_loader with num_gpu=1);
  * its data loader's rank split (lib/utils/dataloader.py:80-85: contiguous blocks of frames per rank) is the sharding

@@ -208,6 +208,7 @@ void smapb_destroy(smapb_handle* h) {
     for (auto& e : h->pre_cache) cudaFree(e.second.buf);
     smapb::jpeg_workspace_destroy(h->jpeg);
     smapb::png_workspace_destroy(h->png);
+    smapb::jpeg_enc_workspace_destroy(h->jpeg_enc);
     delete h;
 }
 
@@ -420,6 +421,21 @@ int smapb_decode_png(smapb_handle* h, int n, const uint8_t* const* png_host, con
     cudaSetDevice(h->device);
     if (!h->png) h->png = smapb::png_workspace_create();
     return smapb::png_decode(h->png, n, png_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
+                      const smapb_record* records_dev, const double* scales_dev, int64_t* nbytes_host, void* stream) {
+    if (!h) return -1;
+    cudaSetDevice(h->device);
+    if (!h->jpeg_enc) h->jpeg_enc = smapb::jpeg_enc_workspace_create();
+    return smapb::jpeg_encode(h->jpeg_enc, n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, nbytes_host,
+                              (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes) {
+    if (!h || !data) return -1;
+    *data = smapb::jpeg_enc_result(h->jpeg_enc, i, nbytes);
+    return *data ? 0 : -1;
 }
 
 int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4) {

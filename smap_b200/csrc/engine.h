@@ -14,6 +14,7 @@
 #include "../../include/smap_b200.h"
 #include "conv_tc.cuh"
 #include "jpeg.h"
+#include "jpeg_enc.h"
 #include "png.h"
 #include "preprocess.h"
 #include "refine.h"
@@ -164,6 +165,7 @@ struct smapb_handle {
     size_t pre_stage_bytes = 0;
     smapb::JpegWorkspace* jpeg = nullptr;  // JPEG decoding (smapb_decode_jpeg), created on first use
     smapb::PngWorkspace* png = nullptr;    // PNG decoding (smapb_decode_png), created on first use
+    smapb::JpegEncWorkspace* jpeg_enc = nullptr;  // JPEG encoding (smapb_encode_jpeg), created on first use
     // RefineNet (optional post-processing step, SURVEY 8(f) f2)
     std::map<std::string, std::vector<float>> refine_raw;
     float* refine_buf = nullptr;  // folded, transposed weights + biases of the five layers

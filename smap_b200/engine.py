@@ -265,6 +265,43 @@ class Engine:
         self._check(self.lib.smapb_png_inflate_stats(self._h, v), "smapb_png_inflate_stats")
         return dict(zip(("candidates", "false_positives", "confirmed", "serial"), list(v)))
 
+    # ---- image encoding --------------------------------------------------------------------------
+    def encode_jpeg(self, frames, quality=95, records=None, scales=None):
+        """frames: list of uint8 BGR [H,W,3] tensors (cuda, or cpu / numpy arrays, which are uploaded) -> list of bytes, per
+        frame what cv2.imencode(".jpg", frame, [IMWRITE_JPEG_QUALITY, quality]) writes.  records (uint8 [n, RECORD_BYTES],
+        as infer_device returns them) with scales (float64 [n, 9], the frames' scale rows from preprocess): each frame is
+        encoded with its skeletons drawn over it (smapb_encode_jpeg, include/smap_b200.h).  The frames are not modified."""
+        n = len(frames)
+        if n == 0:
+            return []
+        if (records is None) != (scales is None):
+            raise ValueError("encode_jpeg: records and scales go together")
+        dev = []
+        for f in frames:
+            if not torch.is_tensor(f):
+                f = torch.from_numpy(np.ascontiguousarray(f))
+            if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+                raise ValueError("encode_jpeg: uint8 BGR [H,W,3] frames expected")
+            dev.append(f.to(self.device).contiguous())
+        ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in dev])
+        hs = (ctypes.c_int * n)(*[f.shape[0] for f in dev])
+        ws = (ctypes.c_int * n)(*[f.shape[1] for f in dev])
+        rec = sc = None
+        if records is not None:
+            rec = records.to(self.device).contiguous()
+            sc = torch.as_tensor(scales, dtype=torch.float64).to(self.device).contiguous()
+            if rec.dtype != torch.uint8 or tuple(rec.shape) != (n, RECORD_BYTES) or tuple(sc.shape) != (n, SCALE_LEN):
+                raise ValueError("encode_jpeg: records uint8 [n, %d] and scales float64 [n, %d] expected" % (RECORD_BYTES, SCALE_LEN))
+        sizes = (ctypes.c_int64 * n)()
+        self._check(self.lib.smapb_encode_jpeg(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), sizes, self._st()),
+                    "smapb_encode_jpeg")
+        out = []
+        for i in range(n):
+            p = ctypes.POINTER(ctypes.c_uint8)()
+            self._check(self.lib.smapb_encoded_jpeg(self._h, i, ctypes.byref(p), None), "smapb_encoded_jpeg")
+            out.append(ctypes.string_at(p, sizes[i]))
+        return out
+
     # ---- pre-processing ------------------------------------------------------------------------
     def preprocess(self, images, out=None):
         """images: list of uint8 BGR [H,W,3] tensors (cuda or cpu; numpy arrays are taken as host images) ->

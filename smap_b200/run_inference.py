@@ -3,6 +3,7 @@ path: images on disk -> result JSON.
 
     python -m smap_b200.run_inference -p SMAP.pth [-rp RefineNet.pth] --dataset_path DIR --batch_size 8 --do_flip 1 \
         [--json_name SUFFIX] [--output_dir OUT] [--dataset_name CMU] [--precision {bf16x3,fp16,bf16}] [--jpeg_colour 1]
+        [--vis_dir DIR [--vis_quality 95]]
 
 Same flags and the same output file name / schema as the reference ('{OUT}/stage3_root2_run_inference_{data_mode}_{suffix}.json',
 test.py:147-152).  Differences, both deliberate: images are visited in sorted path order unless --glob_order 1 (the
@@ -55,6 +56,29 @@ def list_images(dataset_path, glob_order=False):
 def image_name(path, dataset_path):
     """dataset/custom_dataset.py:29."""
     return path.rstrip().replace(dataset_path, "").lstrip("/")
+
+
+def vis_names(paths, dataset_path):
+    """-> per image the relative path of its annotated frame under --vis_dir: its image name with the extension replaced
+    by .jpg.  Raises ValueError naming both inputs when two images would write the same file (a.png and a.jpg)."""
+    names, seen = [], {}
+    for p in paths:
+        name = osp.splitext(image_name(p, dataset_path))[0] + ".jpg"
+        if name in seen:
+            raise ValueError("--vis_dir: %s and %s would both be written to %s" % (seen[name], p, name))
+        seen[name] = p
+        names.append(name)
+    return names
+
+
+def write_vis(eng, vis_dir, quality, names, frames, records, scales):
+    """Encodes the frames with their skeletons drawn (Engine.encode_jpeg on the device records and scale rows) and writes
+    them to vis_dir/names[i], creating subdirectories."""
+    for name, data in zip(names, eng.encode_jpeg(frames, quality, records, scales)):
+        path = osp.join(vis_dir, name)
+        os.makedirs(osp.dirname(path) or ".", exist_ok=True)
+        with open(path, "wb") as f:
+            f.write(data)
 
 
 def read_frames(eng, paths, imread, jpeg_colour=False):
@@ -114,30 +138,36 @@ def _load_weights(eng, smap_state_dict, refine_state_dict, precision):
 
 
 def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False, dataset_name="CMU",
-        device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None, jpeg_colour=False):
+        device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None, jpeg_colour=False,
+        vis_dir=None, vis_quality=95):
     """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3], used for every file; by default .jpg/.jpeg
     and .png files are decoded on the GPU (Engine.decode_jpeg, then Engine.decode_jpeg_ex for the progressive and
     multi-scan JPEGs decode_jpeg leaves, and Engine.decode_png; byte-identical to cv2.imread) and the
     files they do not handle, as every other file, go through cv2.imread(path, IMREAD_COLOR).  jpeg_colour=True: CMYK,
     YCCK and RGB JPEGs and every integral sampling are decoded on the GPU too (Engine.decode_jpeg_ex(colour=True));
     off by default, so those files keep going to cv2.imread.  precision: one of engine.PRECISIONS.  stats (a dict,
-    optional) receives "saturation": the fp16 clamp count."""
+    optional) receives "saturation": the fp16 clamp count.  vis_dir: also write every image with its skeletons drawn,
+    JPEG-encoded at vis_quality on the GPU (write_vis), to vis_dir/<image name with a .jpg extension>."""
     if precision not in PRECISIONS:
         raise ValueError("unknown precision %r (choose from %s)" % (precision, ", ".join(PRECISIONS)))
+    paths = list_images(dataset_path, glob_order)
+    names = vis_names(paths, dataset_path) if vis_dir else None
     eng = Engine(device, max_batch=batch_size, in_h=in_h, in_w=in_w)
     try:
         _load_weights(eng, smap_state_dict, refine_state_dict, precision)
-        paths = list_images(dataset_path, glob_order)
         read = frame_reader(eng, imread, jpeg_colour)
         host = torch.empty(batch_size, RECORD_BYTES, dtype=torch.uint8).pin_memory()
         with ResultWriter(output_file, dataset_name) as w:
             for lo in range(0, len(paths), batch_size):
                 chunk = paths[lo:lo + batch_size]
-                imgs, scales = eng.preprocess(read(chunk))
+                frames = read(chunk)
+                imgs, scales = eng.preprocess(frames)
                 rec = eng.infer_device(imgs, scales.to(imgs.device), do_flip=bool(do_flip))
                 host[:len(chunk)].copy_(rec)
                 torch.cuda.current_stream().synchronize()
                 w.append(host[:len(chunk)], [image_name(p, dataset_path) for p in chunk])
+                if vis_dir:
+                    write_vis(eng, vis_dir, vis_quality, names[lo:lo + batch_size], frames, rec, scales)
         if stats is not None:
             stats["saturation"] = eng.saturation_count()
         return len(paths)
@@ -221,9 +251,10 @@ def drive(n, batch, steps, append):
 class _GatherSteps:
     """The GPU side of drive() on one rank: frames read on the rank's engine and pre-processed into fixed buffers (so
     every step replays the same captured graph), padded with zero images to max_batch; the whole path and the all-gather
-    with infer_device(gather=True, defer=True); the gathered records copied to a pinned host buffer."""
+    with infer_device(gather=True, defer=True); the gathered records copied to a pinned host buffer.  vis(indices, frames,
+    records, scales) (optional) runs in collect() with the global indices of the step's real frames, the frames with this rank's slice of the gathered device records."""
 
-    def __init__(self, eng, read, paths, do_flip):
+    def __init__(self, eng, read, paths, do_flip, vis=None):
         dev = eng.device
         self.eng, self.read, self.paths, self.do_flip, self.B = eng, read, paths, do_flip, eng.max_batch
         self.imgs = torch.empty(self.B, 3, eng.in_h, eng.in_w, device=dev)
@@ -232,12 +263,15 @@ class _GatherSteps:
         self.host = torch.empty(eng.world * self.B, RECORD_BYTES, dtype=torch.uint8).pin_memory()
         self.blank = torch.zeros(eng.in_h, eng.in_w, 3, dtype=torch.uint8, device=dev)
         self.n, self.before, self.excess = self.B, None, 0
+        self.vis, self.frames, self.indices = vis, [], []
 
     def prepare(self, frames):
         ims = self.read([self.paths[i] for i in frames]) if len(frames) else []
         _, scales = self.eng.preprocess(ims + [self.blank] * (self.B - len(ims)), out=self.imgs)
         self.scales.copy_(scales)
         self.n = len(ims)
+        if self.vis is not None:
+            self.frames, self.indices = ims, list(frames)
 
     def submit(self):
         self.before = self.eng.saturation_count() if self.n < self.B else None
@@ -253,6 +287,9 @@ class _GatherSteps:
                 if self.n:
                     self.eng.infer_device(self.imgs[:self.n], self.scales[:self.n], do_flip=self.do_flip)
                 self.excess += padded
+        if self.vis is not None and self.n:
+            lo = self.eng.rank * self.B
+            self.vis(self.indices, self.frames, self.out[lo:lo + self.n], self.scales[:self.n])
         return self.host
 
     def saturation(self):
@@ -261,10 +298,11 @@ class _GatherSteps:
 
 def run_distributed(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False,
                     dataset_name="CMU", device=None, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3",
-                    stats=None, jpeg_colour=False):
+                    stats=None, jpeg_colour=False, vis_dir=None, vis_quality=95):
     """run() on every rank of torch.distributed's default group (gloo), with the same arguments; batch_size frames per
     rank and step, device None = LOCAL_RANK.  Rank 0 lists the images and alone writes output_file, byte-identical to
-    run()'s.  -> number of images; stats["saturation"] = the fp16 clamp count summed over the ranks.  When any rank
+    run()'s; with vis_dir every rank writes the annotated frames of its own shard.  -> number of images;
+    stats["saturation"] = the fp16 clamp count summed over the ranks.  When any rank
     fails, every rank raises: the failing one its own error, the others RankFailed."""
     import torch.distributed as dist
 
@@ -291,7 +329,13 @@ def run_distributed(smap_state_dict, dataset_path, output_file, refine_state_dic
         box = [list_images(dataset_path, glob_order) if rank == 0 else None]
         dist.broadcast_object_list(box, src=0)
         paths = box[0]
-        steps = _GatherSteps(eng, frame_reader(eng, imread, jpeg_colour), paths, bool(do_flip))
+        vis = None
+        if vis_dir:
+            names = vis_names(paths, dataset_path)  # the same list on every rank: all of them refuse a collision
+
+            def vis(indices, frames, records, scales):
+                write_vis(eng, vis_dir, vis_quality, [names[i] for i in indices], frames, records, scales)
+        steps = _GatherSteps(eng, frame_reader(eng, imread, jpeg_colour), paths, bool(do_flip), vis)
         saturation = drive(len(paths), batch_size, steps,
                            lambda rec, frames: writer.append(rec, [image_name(paths[i], dataset_path) for i in frames]))
         if stats is not None:
@@ -331,7 +375,12 @@ def main(argv=None):
     ap.add_argument("--jpeg_colour", type=int, default=0, choices=[0, 1],
                     help="1: also decode CMYK, YCCK and RGB JPEGs and every integral sampling (4:1:1, 4:1:0, ...) on the "
                          "GPU instead of with cv2.imread")
+    ap.add_argument("--vis_dir", default="", help="also write every image with its skeletons drawn, JPEG-encoded on the GPU, "
+                                                  "to VIS_DIR/<image name with a .jpg extension>")
+    ap.add_argument("--vis_quality", type=int, default=95, help="JPEG quality of --vis_dir, 1..100 (cv2's default 95)")
     a = ap.parse_args(argv)
+    if not 1 <= a.vis_quality <= 100:
+        ap.error("--vis_quality must be in 1..100")
     if "WORLD_SIZE" in os.environ:
         return _main_distributed(a)
     try:
@@ -343,9 +392,14 @@ def main(argv=None):
     out = result_file_name(a.output_dir, a.test_mode, a.data_mode, a.json_name)
     stats = {}
     n = run(sd, a.dataset_path, out, rsd, a.batch_size, a.do_flip, a.dataset_name, glob_order=bool(a.glob_order),
-            precision=a.precision, stats=stats, jpeg_colour=bool(a.jpeg_colour))
+            precision=a.precision, stats=stats, jpeg_colour=bool(a.jpeg_colour), **_vis_kwargs(a))
     _report(out, n, stats)
     return 0
+
+
+def _vis_kwargs(a):
+    """--vis_dir / --vis_quality as run()'s keyword arguments; none without --vis_dir, so that run is called as before."""
+    return dict(vis_dir=a.vis_dir, vis_quality=a.vis_quality) if a.vis_dir else {}
 
 
 def _load_checkpoints(a):
@@ -389,7 +443,7 @@ def _main_distributed(a):
         stats = {}
         n = run_distributed(sd, a.dataset_path, out, rsd, a.batch_size, a.do_flip, a.dataset_name,
                             glob_order=bool(a.glob_order), precision=a.precision, stats=stats,
-                            jpeg_colour=bool(a.jpeg_colour))
+                            jpeg_colour=bool(a.jpeg_colour), **_vis_kwargs(a))
     except (FileNotFoundError, RankFailed) as e:
         print("rank {}: {}".format(rank, e), flush=True)
         return 1
