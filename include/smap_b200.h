@@ -240,7 +240,35 @@ int smapb_wait(smapb_handle* h, int slot);
  * demand; the call synchronises `stream`, so it cannot be captured into a CUDA graph. */
 int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
                       const smapb_record* records_dev, const double* scales_dev, int64_t* nbytes_host, void* stream);
-/* Stream i of the last smapb_encode_jpeg: *data = its first byte, *nbytes (may be NULL) its size.  -1 for i out of range. */
+/* Flags of smapb_encode_jpeg_ex; 0 = exactly smapb_encode_jpeg.
+ * SMAPB_ENCODE_VIEW3D (records required) encodes each h x w frame as an h x (w + h) composite: columns 0..w-1 are the
+ * frame with its overlay exactly as smapb_encode_jpeg draws it (radii from h x w, elements clipped at column w), columns
+ * w..w+h-1 a P x P panel (P = h) with the record's 3D skeletons seen from lib/visualize/vis.py's viewpoint
+ * (view_init(azim=-90, elev=-45)), orthographic and with one scale on both axes, so bone lengths compare:
+ *   placed   joint j of row p < count is placed when pred3d[p][j][3] > 0 and X, Y, Z are finite with |.| <= 1e15 (with
+ *            RefineNet every joint of a kept person is; without it gen_3d_pose's zeroed joints are not);
+ *   limbs    limb k (the 14 pairs above) is drawn when both of its joints are placed; the fit set is the joints of drawn
+ *            limbs; with an empty fit set the panel is plain white;
+ *   view     screen right is +X, screen up (Z - Y) / sqrt(2), the viewer looks along +(Y + Z): per joint a = X,
+ *            b = (Z - Y) * S with S = 0.7071067811865476, view depth d = Y + Z;
+ *   fit      m = P / 20, avail = P - 1 - 2m (integer); amin, amax, bmin, bmax over the fit set, ea = amax - amin,
+ *            eb = bmax - bmin, span = max(ea, eb); k = avail / span when span > 0, avail > 0 and the quotient is finite,
+ *            else 0; ox = m + (avail - ea * k) / 2, oy = m + (avail - eb * k) / 2; a point's pixel is
+ *            x = rint(ox + (a - amin) * k), y = rint(oy + (bmax - b) * k), clamped to +-32768;
+ *            all float64, each operation rounded in this order, no fused multiply-add, rint half to even;
+ *   order    first the 12 edges of the fit set's box [Xmin, Xmax] x [Ymin, Ymax] x [Zmin, Zmax] in grey BGR (160, 160, 160):
+ *            with corner c taking the maximum of X, Y, Z where bit 0, 1, 2 of c is set, the edges 0-1, 2-3, 4-5, 6-7
+ *            (along X), 0-2, 1-3, 4-6, 5-7 (along Y), 0-4, 1-5, 2-6, 3-7 (along Z); then the drawn limbs by descending
+ *            depth d_a + d_b ((Y_a + Z_a) + (Y_b + Z_b)), ties in ascending (row, limb); each later element over the
+ *            earlier ones; a limb takes the overlay colour of person p % 6;
+ *   coverage the overlay's limb test with half-width r = max(1, P / 400) on a white background.
+ * The panel takes two more launches (a set-up CTA per image, a paint CTA per element).  -1, with the frame named, when
+ * w + h > 16384; -1 for unknown flags or the flag without records. */
+#define SMAPB_ENCODE_VIEW3D 1
+int smapb_encode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
+                         const smapb_record* records_dev, const double* scales_dev, int flags, int64_t* nbytes_host,
+                         void* stream);
+/* Stream i of the last smapb_encode_jpeg(_ex): *data = its first byte, *nbytes (may be NULL) its size.  -1 for i out of range. */
 int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes);
 
 /* ---- multi-GPU: frames are sharded over ranks, ONE exchange step per batch --------------------------------------- */

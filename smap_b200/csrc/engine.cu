@@ -423,13 +423,18 @@ int smapb_decode_png(smapb_handle* h, int n, const uint8_t* const* png_host, con
     return smapb::png_decode(h->png, n, png_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
 }
 
-int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
-                      const smapb_record* records_dev, const double* scales_dev, int64_t* nbytes_host, void* stream) {
+int smapb_encode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
+                         const smapb_record* records_dev, const double* scales_dev, int flags, int64_t* nbytes_host, void* stream) {
     if (!h) return -1;
     cudaSetDevice(h->device);
     if (!h->jpeg_enc) h->jpeg_enc = smapb::jpeg_enc_workspace_create();
-    return smapb::jpeg_encode(h->jpeg_enc, n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, nbytes_host,
+    return smapb::jpeg_encode(h->jpeg_enc, n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, flags, nbytes_host,
                               (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
+                      const smapb_record* records_dev, const double* scales_dev, int64_t* nbytes_host, void* stream) {
+    return smapb_encode_jpeg_ex(h, n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, 0, nbytes_host, stream);
 }
 
 int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes) {

@@ -25,7 +25,9 @@
 
 #include "decode_host.h"
 #include "jpeg_enc.h"
+#include "paint.cuh"
 #include "preprocess.h"
+#include "view3d.h"
 
 namespace smapb {
 
@@ -34,13 +36,13 @@ namespace {
 constexpr int NELEM = SMAPB_NL + SMAPB_NJ;  // 14 limbs then 15 joints per person: paint rank person * 29 + element + 1
 constexpr int BLOCK_BITS_MAX = 22 + 63 * 26;  // the longest DC token + 63 tokens of run 0 / size 10 (jpeg_encode_numpy)
 constexpr int SCAN_THREADS = 1024, SCAN_ITEMS = 4, SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
-constexpr int COORD_MAX = 32768;  // frame coordinates of joints are clamped to +-COORD_MAX (so the limb test fits int64)
 
-__constant__ int kPairs[SMAPB_NL][2] = {{0, 1}, {0, 2}, {0, 9}, {9, 10}, {10, 11}, {0, 3}, {3, 4},
-                                        {4, 5}, {2, 12}, {12, 13}, {13, 14}, {2, 6}, {6, 7}, {7, 8}};
 // BGR limb colours per person (cycling), and the joint colour (include/smap_b200.h, smapb_encode_jpeg)
 __constant__ uint8_t kPalette[6][3] = {{0, 0, 255}, {0, 255, 0}, {255, 0, 0}, {0, 255, 255}, {0, 0, 0}, {255, 0, 255}};
 __constant__ uint8_t kJoint[3] = {255, 255, 255};
+// the 3D panel's background and fit-box colour
+__constant__ uint8_t kWhite[3] = {255, 255, 255};
+__constant__ uint8_t kGrey[3] = {160, 160, 160};
 
 const int kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
                          41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
@@ -83,9 +85,10 @@ struct EncTables {
 };
 
 struct EncImg {
-    const uint8_t* src;  // BGR [h][w][3]
+    const uint8_t* src;  // BGR [h][fw][3]
     const smapb_record* rec;  // NULL: no overlay
-    int h, w, mx, my, bw, bh;  // MCU columns / rows, luma block columns / rows
+    int h, w, mx, my, bw, bh;  // the encoded image's size, MCU columns / rows, luma block columns / rows
+    int fw;  // the frame's width: w, or w - h with the 3D panel in columns fw..w-1
     int r, R;  // limb half-width and joint radius (overlay)
     int pad_l, pad_t;  // letterbox of the net input (make_resize_plan)
     double scale;
@@ -93,7 +96,7 @@ struct EncImg {
     long long plane0;  // Y plane [16 my][16 mx], then Cb and Cr [8 my][8 mx]
     long long word0;  // first word of the image's bit buffer
     long long bound_bits;  // blocks * BLOCK_BITS_MAX
-    long long label0;  // first label of the image's plane [h][w] (overlay only)
+    long long label0;  // first label of the image's plane [h][w] (overlay only; the panel's labels from column fw)
 };
 
 // per-image results of the totals kernel
@@ -120,19 +123,6 @@ __device__ __forceinline__ bool joint_xy(const EncImg& I, const float* pj, long 
     return true;
 }
 
-__device__ __forceinline__ bool in_disc(long long dx, long long dy, long long rr) { return dx * dx + dy * dy <= rr * rr; }
-
-// clamped-projection test of pixel (x, y) against the limb a-b of half-width r, exact in int64
-__device__ __forceinline__ bool in_limb(long long x, long long y, long long ax, long long ay, long long bx, long long by, long long r) {
-    const long long vx = bx - ax, vy = by - ay, px = x - ax, py = y - ay;
-    const long long dot = px * vx + py * vy, len2 = vx * vx + vy * vy;
-    if (dot <= 0) return in_disc(px, py, r);
-    if (dot >= len2) return in_disc(x - bx, y - by, r);
-    const long long cross = px * vy - py * vx;
-    if (cross > (1ll << 31) || cross < -(1ll << 31)) return false;  // cross^2 > 2^62 > r^2 |b-a|^2
-    return cross * cross <= r * r * len2;
-}
-
 __global__ void __launch_bounds__(256) overlay_kernel(const EncImg* __restrict__ imgs, int* __restrict__ labels) {
     const EncImg& I = imgs[blockIdx.y];
     if (!I.rec) return;
@@ -147,43 +137,29 @@ __global__ void __launch_bounds__(256) overlay_kernel(const EncImg* __restrict__
         if (!joint_xy(I, P + 4 * (e - SMAPB_NL), &ax, &ay)) return;
         bx = ax, by = ay, rad = I.R;
     }
-    const int rank = p * NELEM + e + 1;
-    int* L = labels + I.label0;
-    // Candidates: along the segment's major axis, its range widened by rad; across it, a band of +-(2 rad + 2) around
-    // the segment's (clamped, rounded) centre line.  A covered pixel is within rad of some segment point, so within
-    // sqrt(2) rad + 1/2 of that line across the major axis: the band holds every pixel the exact test accepts, and a
-    // long diagonal limb costs its length times the band instead of its bounding box.  (A joint is a limb a = b.)
-    const bool xmajor = llabs(bx - ax) >= llabs(by - ay);
-    const long long am = xmajor ? ax : ay, bm = xmajor ? bx : by, an = xmajor ? ay : ax, bn = xmajor ? by : bx;
-    const long long lim_m = xmajor ? I.w : I.h, lim_n = xmajor ? I.h : I.w;
-    const long long m0 = max(0ll, min(am, bm) - rad), m1 = min(lim_m - 1, max(am, bm) + rad);
-    if (m0 > m1) return;
-    const long long band = 2 * rad + 2, span = 2 * band + 1, count = (m1 - m0 + 1) * span;
-    for (long long k = threadIdx.x; k < count; k += blockDim.x) {
-        const long long m = m0 + k / span;
-        const long long mc = min(max(m, min(am, bm)), max(am, bm));
-        const long long c = bm == am ? an : (long long)rint(an + (double)(mc - am) * (double)(bn - an) / (double)(bm - am));
-        const long long nn = c + k % span - band;
-        if (nn < 0 || nn >= lim_n) continue;
-        const long long x = xmajor ? m : nn, y = xmajor ? nn : m;
-        const bool hit = e < SMAPB_NL ? in_limb(x, y, ax, ay, bx, by, rad) : in_disc(x - ax, y - ay, rad);
-        if (hit) atomicMax(&L[y * I.w + x], rank);
-    }
+    // the frame's columns only: with a 3D panel the label plane is as wide as the composite
+    paint_band(labels + I.label0, I.w, I.fw, I.h, ax, ay, bx, by, rad, p * NELEM + e + 1);
 }
 
 // ---- colour ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void load_pixel(const EncImg& I, const int* __restrict__ labels, int x, int y, int* b, int* g, int* r) {
     const size_t i = (size_t)y * I.w + x;
-    const uint8_t* s = I.src + i * 3;
-    *b = s[0], *g = s[1], *r = s[2];
-    if (I.rec) {
+    const uint8_t* c = nullptr;
+    if (x >= I.fw) {  // the 3D panel: white, or its element's colour (view3d.h)
         const int l = labels[I.label0 + i];
-        if (l > 0) {
-            const int e = (l - 1) % NELEM, p = (l - 1) / NELEM;
-            const uint8_t* c = e < SMAPB_NL ? kPalette[p % 6] : kJoint;
-            *b = c[0], *g = c[1], *r = c[2];
+        c = l == 0 ? kWhite : (l & 7) == PANEL_GREY ? kGrey : kPalette[l & 7];
+    } else {
+        const uint8_t* s = I.src + ((size_t)y * I.fw + x) * 3;
+        *b = s[0], *g = s[1], *r = s[2];
+        if (I.rec) {
+            const int l = labels[I.label0 + i];
+            if (l > 0) {
+                const int e = (l - 1) % NELEM, p = (l - 1) / NELEM;
+                c = e < SMAPB_NL ? kPalette[p % 6] : kJoint;
+            }
         }
     }
+    if (c) *b = c[0], *g = c[1], *r = c[2];
 }
 
 // libjpeg-turbo's RGB -> YCbCr: 16-bit fixed point, Cb and Cr rounded with 1/2 - epsilon
@@ -675,6 +651,8 @@ struct JpegEncWorkspace {
     size_t ffoff_cap = 0;
     unsigned long long* tiles = nullptr;
     size_t tiles_cap = 0;
+    PanelSeg* segs = nullptr;  // [n][PANEL_ELEMS] (3D panel)
+    size_t segs_cap = 0;
     uint32_t* words = nullptr;
     size_t words_cap = 0;
     uint8_t* out = nullptr;
@@ -691,7 +669,7 @@ void jpeg_enc_workspace_destroy(JpegEncWorkspace* ws) {
     void* pinned[] = {ws->host, ws->scales_host, ws->tot_host, ws->result};
     for (void* p : pinned)
         if (p) cudaFreeHost(p);
-    void* dev[] = {ws->dev_in, ws->tot, ws->planes, ws->labels, ws->coef, ws->counts, ws->off, ws->ffoff, ws->tiles, ws->words, ws->out};
+    void* dev[] = {ws->dev_in, ws->tot, ws->planes, ws->labels, ws->coef, ws->counts, ws->off, ws->ffoff, ws->tiles, ws->segs, ws->words, ws->out};
     for (void* p : dev)
         if (p) cudaFree(p);
     delete ws;
@@ -716,12 +694,21 @@ static int scan_counts(JpegEncWorkspace* ws, const uint32_t* in, long long n, un
 }
 
 int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const int* img_h, const int* img_w, int quality,
-                const smapb_record* records, const double* scales, int64_t* nbytes, cudaStream_t st, int64_t* launches,
-                std::string* err) {
+                const smapb_record* records, const double* scales, int flags, int64_t* nbytes, cudaStream_t st,
+                int64_t* launches, std::string* err) {
     ws->res_off.clear();
     ws->res_len.clear();
     if (n < 0 || (n > 0 && (!bgr || !img_h || !img_w || !nbytes)) || (records && !scales)) {
         *err = "smapb_encode_jpeg: null argument";
+        return -1;
+    }
+    if (flags & ~SMAPB_ENCODE_VIEW3D) {
+        *err = "smapb_encode_jpeg_ex: unknown flags " + std::to_string(flags);
+        return -1;
+    }
+    const bool view3d = flags & SMAPB_ENCODE_VIEW3D;
+    if (view3d && !records) {
+        *err = "smapb_encode_jpeg_ex: SMAPB_ENCODE_VIEW3D needs records";
         return -1;
     }
     if (quality < 1 || quality > 100) {
@@ -738,6 +725,12 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
                    std::to_string(img_h[i]) + " (sides must be 1..16384)";
             return -1;
         }
+        if (view3d && img_w[i] + img_h[i] > 16384) {
+            *err = "smapb_encode_jpeg_ex: frame " + std::to_string(i) + " is " + std::to_string(img_w[i]) + "x" +
+                   std::to_string(img_h[i]) + ": with its 3D panel it would be " + std::to_string(img_w[i] + img_h[i]) +
+                   " wide (sides must be 1..16384)";
+            return -1;
+        }
     }
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     DECODE_CK(cudaStreamIsCapturing(st, &cap));
@@ -752,12 +745,14 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
     }
     DECODE_CK(cudaStreamSynchronize(st));  // the scales, and the workspace the previous call may still use
     std::vector<EncImg> imgs(n);
+    std::vector<PanelImg> panels(view3d ? n : 0);
     long long nblk = 0, plane_total = 0, word_total = 0, label_total = 0;
     for (int i = 0; i < n; i++) {
         EncImg& I = imgs[i];
         memset(&I, 0, sizeof(I));
         I.src = bgr[i];
-        I.h = img_h[i], I.w = img_w[i];
+        I.h = img_h[i], I.fw = img_w[i];
+        I.w = view3d ? I.fw + I.h : I.fw;
         I.mx = (I.w + 15) / 16, I.my = (I.h + 15) / 16, I.bw = (I.w + 7) / 8, I.bh = (I.h + 7) / 8;
         I.blk0 = nblk;
         const long long nb = 6ll * I.mx * I.my;
@@ -771,17 +766,18 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         if (records) {
             const double* row = ws->scales_host + (size_t)i * SMAPB_SCALE_LEN;
             ResizePlan P;
-            if (row[1] != I.w || row[2] != I.h || !make_resize_plan(I.w, I.h, (int)row[3], (int)row[4], &P)) {
+            if (row[1] != I.fw || row[2] != I.h || !make_resize_plan(I.fw, I.h, (int)row[3], (int)row[4], &P)) {
                 *err = "smapb_encode_jpeg: the scale row of frame " + std::to_string(i) + " does not describe a " +
-                       std::to_string(I.w) + "x" + std::to_string(I.h) + " frame";
+                       std::to_string(I.fw) + "x" + std::to_string(I.h) + " frame";
                 return -1;
             }
             I.rec = records + i;
             I.scale = row[0], I.pad_l = P.pad_l, I.pad_t = P.pad_t;
-            const int m = std::min(I.w, I.h);
+            const int m = std::min(I.fw, I.h);
             I.r = std::max(1, m / 400), I.R = std::max(2, m / 200);
             I.label0 = label_total;
             label_total += (long long)I.w * I.h;
+            if (view3d) panels[i] = PanelImg{I.rec, I.h, I.w, I.label0 + I.fw};
         }
     }
     EncTables T;
@@ -794,10 +790,15 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         huff_codes(kDcBits[t], dcv, T.dc_code[t], T.dc_len[t]);
         huff_codes(kAcBits[t], kAcVals[t], T.ac_code[t], T.ac_len[t]);
     }
-    const size_t o_tab = align_up(sizeof(EncImg) * n, 256), total_in = o_tab + sizeof(EncTables);
+    const size_t o_tab = align_up(sizeof(EncImg) * n, 256), o_pan = align_up(o_tab + sizeof(EncTables), 256);
+    const size_t total_in = o_pan + sizeof(PanelImg) * panels.size();
     DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total_in));
     memcpy(ws->host, imgs.data(), sizeof(EncImg) * n);
     memcpy(ws->host + o_tab, &T, sizeof(T));
+    if (view3d) {
+        memcpy(ws->host + o_pan, panels.data(), sizeof(PanelImg) * n);
+        DECODE_CK(grow(&ws->segs, &ws->segs_cap, (size_t)n * PANEL_ELEMS));
+    }
     DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total_in));
     DECODE_CK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
     DECODE_CK(grow(&ws->coef, &ws->coef_cap, (size_t)nblk * 64));
@@ -817,6 +818,10 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         DECODE_CK(cudaMemsetAsync(ws->labels, 0, sizeof(int) * label_total, st));
         overlay_kernel<<<dim3(SMAPB_MAXP * NELEM, n), 256, 0, st>>>(d_img, ws->labels);
         ++*launches;
+        if (view3d) {
+            panel_launch((const PanelImg*)(ws->dev_in + o_pan), n, ws->segs, ws->labels, st);
+            *launches += 2;
+        }
     }
     const unsigned fgrid = (unsigned)((nblk + 127) / 128), bgrid = (unsigned)((nblk + 255) / 256);
     colour_kernel<<<dim3((unsigned)((64ll * max_mcus + 255) / 256), n), 256, 0, st>>>(d_img, ws->labels, ws->planes);

@@ -61,6 +61,7 @@ def get_tile_table():
 
 JPEG_SCANS = 1  # SMAPB_JPEG_SCANS
 JPEG_COLOUR = 2  # SMAPB_JPEG_COLOUR
+ENCODE_VIEW3D = 1  # SMAPB_ENCODE_VIEW3D
 
 
 def _header_info(fn, data, *flags):
@@ -266,12 +267,16 @@ class Engine:
         return dict(zip(("candidates", "false_positives", "confirmed", "serial"), list(v)))
 
     # ---- image encoding --------------------------------------------------------------------------
-    def encode_jpeg(self, frames, quality=95, records=None, scales=None):
+    def encode_jpeg(self, frames, quality=95, records=None, scales=None, view3d=False):
         """frames: list of uint8 BGR [H,W,3] tensors (cuda, or cpu / numpy arrays, which are uploaded) -> list of bytes, per
         frame what cv2.imencode(".jpg", frame, [IMWRITE_JPEG_QUALITY, quality]) writes.  records (uint8 [n, RECORD_BYTES],
         as infer_device returns them) with scales (float64 [n, 9], the frames' scale rows from preprocess): each frame is
-        encoded with its skeletons drawn over it (smapb_encode_jpeg, include/smap_b200.h).  The frames are not modified."""
+        encoded with its skeletons drawn over it (smapb_encode_jpeg, include/smap_b200.h).  view3d (records required):
+        each H x W frame is encoded as an H x (W + H) composite, the drawn frame and an H x H panel of its 3D skeletons
+        (smapb_encode_jpeg_ex with SMAPB_ENCODE_VIEW3D; oracle/view3d_numpy.py).  The frames are not modified."""
         n = len(frames)
+        if view3d and records is None:
+            raise ValueError("encode_jpeg: view3d needs records and scales")
         if n == 0:
             return []
         if (records is None) != (scales is None):
@@ -293,8 +298,12 @@ class Engine:
             if rec.dtype != torch.uint8 or tuple(rec.shape) != (n, RECORD_BYTES) or tuple(sc.shape) != (n, SCALE_LEN):
                 raise ValueError("encode_jpeg: records uint8 [n, %d] and scales float64 [n, %d] expected" % (RECORD_BYTES, SCALE_LEN))
         sizes = (ctypes.c_int64 * n)()
-        self._check(self.lib.smapb_encode_jpeg(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), sizes, self._st()),
-                    "smapb_encode_jpeg")
+        if view3d:
+            self._check(self.lib.smapb_encode_jpeg_ex(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), ENCODE_VIEW3D,
+                                                      sizes, self._st()), "smapb_encode_jpeg_ex")
+        else:
+            self._check(self.lib.smapb_encode_jpeg(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), sizes,
+                                                   self._st()), "smapb_encode_jpeg")
         out = []
         for i in range(n):
             p = ctypes.POINTER(ctypes.c_uint8)()

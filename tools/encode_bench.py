@@ -3,8 +3,9 @@
     python tools/encode_bench.py [--repeats 3] [--cli_frames 64]
 
 Prints one JSON line per measurement, each with the card's name and power limit read in the same process:
-  encode   GPU frames/s for batches of 8 frames (1920x1080 and 4032x3024, q95), plain and with a crowded overlay (127
-           persons per frame), after a warm-up of the same shapes; host clock around calls that end in a device
+  encode   GPU frames/s for batches of 8 frames (1920x1080 and 4032x3024, q95), plain, with a crowded overlay (127
+           persons per frame) and with that overlay plus the 3D panel of the same 127 persons (view3d: an h x (w + h)
+           composite per frame), after a warm-up of the same shapes; host clock around calls that end in a device
            synchronisation (encode_jpeg returns once the bytes are on the host);
   cv2      cv2.imencode frames/s on one thread and on every host thread (a thread pool; cv2 releases the GIL);
   cli      run_inference.run frames/s on a directory of 1080p JPEGs (identity weights), bf16x3 and fp16, with and without
@@ -51,6 +52,8 @@ def crowd(n, h, w, seed):
     rec["pred2d"][..., 0] = rng.uniform(0, 832, (n, 127, 15))
     rec["pred2d"][..., 1] = rng.uniform(0, 512, (n, 127, 15))
     rec["pred2d"][..., 3] = 1
+    rec["pred3d"][..., :3] = rng.normal([0, -20, 400], [70, 90, 120], (n, 127, 15, 3))
+    rec["pred3d"][..., 3] = 1  # every joint placed, as RefineNet leaves them: 1778 limbs per panel
     sc = np.stack([scale_row(lift_numpy.default_scale(w, h))] * n)
     return torch.from_numpy(rec.view(np.uint8).reshape(n, -1)).cuda(), torch.from_numpy(sc).cuda()
 
@@ -70,6 +73,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--cli_frames", type=int, default=64)
+    ap.add_argument("--skip_cli", action="store_true", help="only the encode and cv2 legs")
     a = ap.parse_args()
     gpu = card()
     eng = Engine(0, max_batch=8)
@@ -77,18 +81,19 @@ def main():
     for h, w in ((1080, 1920), (3024, 4032)):
         frames = [torch.from_numpy(photo(h, w, s)).cuda() for s in range(B)]
         host = [f.cpu().numpy() for f in frames]
-        for overlay in (False, True):
+        for overlay, view3d in ((False, False), (True, False), (True, True)):
             extra = crowd(B, h, w, 1) if overlay else (None, None)
-            eng.encode_jpeg(frames, 95, *extra)  # warm-up: workspace growth, module load
+            kw = dict(view3d=True) if view3d else {}
+            eng.encode_jpeg(frames, 95, *extra, **kw)  # warm-up: workspace growth, module load
             iters = 20 if h == 1080 else 5
             rates = []
             for _ in range(a.repeats):
                 torch.cuda.synchronize()
                 t = time.perf_counter()
                 for _ in range(iters):
-                    eng.encode_jpeg(frames, 95, *extra)
+                    eng.encode_jpeg(frames, 95, *extra, **kw)
                 rates.append(iters * B / (time.perf_counter() - t))
-            print(json.dumps({"what": "encode", "size": "%dx%d" % (w, h), "batch": B, "overlay": overlay,
+            print(json.dumps({"what": "encode", "size": "%dx%d" % (w, h), "batch": B, "overlay": overlay, "view3d": view3d,
                               "frames_per_s": stats(rates), "gpu": gpu}), flush=True)
         for threads in (1, os.cpu_count()):
             cv2.setNumThreads(1)
@@ -102,6 +107,8 @@ def main():
             print(json.dumps({"what": "cv2", "size": "%dx%d" % (w, h), "threads": threads, "frames_per_s": stats(rates),
                               "gpu": gpu}), flush=True)
     eng.close()
+    if a.skip_cli:
+        return
     with tempfile.TemporaryDirectory() as tmp:
         data = os.path.join(tmp, "imgs")
         os.makedirs(data)
