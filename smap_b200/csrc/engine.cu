@@ -2,7 +2,6 @@
 // and profiling entry points of the C ABI (include/smap_b200.h).  The execution plan and the weights are in plan.cu.
 #include <dlfcn.h>
 #include <math.h>
-#include <nvtx3/nvToolsExt.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -86,6 +85,17 @@ int on_stream(smapb_handle* h, void* stream, F&& body) {
     return 0;
 }
 
+// Every stream and every event of a handle.  smapb_create makes them all, so that the lazy set-ups of the whole path only
+// allocate device memory; smapb_destroy destroys those that exist.
+std::vector<cudaStream_t*> handle_streams(smapb_handle* h) {
+    return {&h->own_stream, &h->aux_stream, &h->copy_stream, &h->gather_stream};
+}
+std::vector<cudaEvent_t*> handle_events(smapb_handle* h) {
+    return {&h->bridge_in, &h->bridge_out, &h->rec_ready[0], &h->rec_ready[1], &h->gather_done[0], &h->gather_done[1],
+            &h->slots[0].h2d, &h->slots[0].done, &h->slots[0].rec_ready, &h->slots[1].h2d, &h->slots[1].done,
+            &h->slots[1].rec_ready};
+}
+
 }  // namespace
 
 void smapb::drop_graphs(smapb_handle* h, bool gather_only) {
@@ -153,10 +163,10 @@ int smapb_create(smapb_handle** out, int device, int max_batch, int in_h, int in
         delete h;
         return -10;
     }
-    if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->bridge_in, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->bridge_out, cudaEventDisableTiming) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking) != cudaSuccess) {
+    bool made = true;
+    for (cudaStream_t* s : handle_streams(h)) made = made && cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
+    for (cudaEvent_t* e : handle_events(h)) made = made && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
+    if (!made) {
         g_create_error = "smapb_create: stream / event creation failed";
         smapb_destroy(h);
         return -10;
@@ -179,27 +189,17 @@ void smapb_destroy(smapb_handle* h) {
         cudaFree(S.scales);
         cudaFree(S.records);
         cudaFree(S.records_all);
-        if (S.h2d) cudaEventDestroy(S.h2d);
-        if (S.done) cudaEventDestroy(S.done);
-        if (S.rec_ready) cudaEventDestroy(S.rec_ready);
     }
     if (h->comm && h->comm_owned && nccl_api().CommDestroy) nccl_api().CommDestroy(h->comm);
-    if (h->gather_stream) cudaStreamDestroy(h->gather_stream);
-    for (int i = 0; i < 2; i++) {
-        if (h->rec_ready[i]) cudaEventDestroy(h->rec_ready[i]);
-        if (h->gather_done[i]) cudaEventDestroy(h->gather_done[i]);
-        cudaFree(h->rec_buf[i]);
-    }
-    if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    if (h->aux_stream) cudaStreamDestroy(h->aux_stream);
-    if (h->bridge_in) cudaEventDestroy(h->bridge_in);
-    if (h->bridge_out) cudaEventDestroy(h->bridge_out);
+    cudaFree(h->rec_buf[0]);
+    for (cudaStream_t* s : handle_streams(h))
+        if (*s) cudaStreamDestroy(*s);
+    for (cudaEvent_t* e : handle_events(h))
+        if (*e) cudaEventDestroy(*e);
     for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
     free_layers(h);
-    void* ptrs[] = {h->peaks, h->scores, h->bodies, h->counts, h->imgs_dev, h->imgs_flip, h->hm, h->hm_flip, h->detd,
-                    h->rootd, h->scratch_detd, h->scratch_rootd, h->scales_dev, h->records_dev, h->stem_w, h->stem_b,
-                    h->gather_dev, h->gt_dist, h->nms_masks, h->sat_dev};
+    void* ptrs[] = {h->peaks, h->scores, h->bodies, h->counts, h->imgs_dev, h->imgs_flip, h->hm, h->detd, h->rootd,
+                    h->scales_dev, h->records_dev, h->stem_w, h->stem_b, h->gather_dev, h->gt_dist, h->nms_masks, h->sat_dev};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (h->refine_buf) cudaFree(h->refine_buf);
@@ -568,35 +568,35 @@ __global__ void flip_w_kernel(const float* __restrict__ in, float* __restrict__ 
     }
 }
 
+// A smapb_record array as the lift and RefineNet kernels take it: record 0's fields, and the record stride in 4 and 8 bytes
+struct RecordFields {
+    float* pred2d;
+    double *pred3d, *root_depth;
+    int* count;
+    static constexpr long long s4 = sizeof(smapb_record) / 4, s8 = sizeof(smapb_record) / 8;
+    explicit RecordFields(smapb_record* r)
+        : pred2d(r->pred2d[0][0]), pred3d(r->pred3d[0][0]), root_depth(r->root_depth), count(&r->count) {}
+};
+
 static int infer_body(smapb_handle* h, Plan* plan, const float* imgs, const double* scales, int B, int do_flip,
                       smapb_record* records, cudaStream_t st) {
-    nvtxRangePushA("smapb.backbone");
-    int rc = run_plan(h, plan, imgs, h->hm, h->detd, h->rootd, st);
-    if (rc) {
-        nvtxRangePop();
-        return rc;
-    }
-    const size_t hw = (size_t)h->h * h->w;
+    NvtxScope range("smapb.backbone");
+    if (int rc = run_plan(h, plan, imgs, h->hm, h->detd, h->rootd, st)) return rc;
     if (do_flip) {
-        const size_t MB = h->max_batch;
-        if (!h->imgs_flip) {
-            if (dev_alloc(h, &h->imgs_flip, MB * 3 * h->in_h * h->in_w)) return -10;
-            if (dev_alloc(h, &h->hm_flip, MB * NC2D * hw)) return -10;
-            if (dev_alloc(h, &h->scratch_detd, MB * NL * hw)) return -10;
-            if (dev_alloc(h, &h->scratch_rootd, MB * hw)) return -10;
+        if (!h->imgs_flip) {  // one allocation, so that a failed set-up leaves nothing behind and is tried again
+            const size_t MB = h->max_batch, hw = (size_t)h->h * h->w, frames = MB * 3 * h->in_h * h->in_w;
+            if (dev_alloc(h, &h->imgs_flip, frames + MB * (NC2D + NL + 1) * hw)) return -10;
+            h->hm_flip = h->imgs_flip + frames;  // every part 256-byte aligned: in_h and in_w are multiples of 32
+            h->scratch_detd = h->hm_flip + MB * NC2D * hw;
+            h->scratch_rootd = h->scratch_detd + MB * NL * hw;
         }
         flip_w_kernel<<<132 * 8, 256, 0, st>>>(imgs, h->imgs_flip, (long long)B * 3 * h->in_h, h->in_w);
         CK(cudaGetLastError());
         prof_mark(h, PK_ELEM, st, "flip_w");
         h->launches++;
-        rc = run_plan(h, plan, h->imgs_flip, h->hm_flip, h->scratch_detd, h->scratch_rootd, st);
-        if (rc) {
-            nvtxRangePop();
-            return rc;
-        }
+        if (int rc = run_plan(h, plan, h->imgs_flip, h->hm_flip, h->scratch_detd, h->scratch_rootd, st)) return rc;
     }
-    nvtxRangePop();
-    nvtxRangePushA("smapb.association");
+    range.next("smapb.association");
     CK(launch_merge_scale(h->hm, do_flip ? h->hm_flip : nullptr, B, h->h, h->w, 1, st));
     prof_mark(h, PK_ELEM, st, "merge_scale");
     CK(launch_nms(h->hm, NC2D, B, h->h, h->w, 0.2f, h->peaks, h->nms_masks, st));
@@ -605,26 +605,17 @@ static int infer_body(smapb_handle* h, Plan* plan, const float* imgs, const doub
     prof_mark(h, PK_ASSOC, st, "paf");
     CK(launch_group(h->peaks, h->scores, h->rootd, B, h->h, h->w, 2, 1, h->bodies, h->counts, st));
     prof_mark(h, PK_ASSOC, st, "group");
-    nvtxRangePop();
-    nvtxRangePushA("smapb.lift");
-    char* rb = reinterpret_cast<char*>(records);
-    CK(launch_lift(h->bodies, h->counts, h->detd, h->rootd, scales, B, h->h, h->w, 2,
-                   reinterpret_cast<float*>(rb + offsetof(smapb_record, pred2d)),
-                   reinterpret_cast<double*>(rb + offsetof(smapb_record, pred3d)),
-                   reinterpret_cast<double*>(rb + offsetof(smapb_record, root_depth)),
-                   reinterpret_cast<int*>(rb + offsetof(smapb_record, count)), sizeof(smapb_record) / 4,
-                   sizeof(smapb_record) / 8, sizeof(smapb_record) / 8, sizeof(smapb_record) / 4, st));
+    range.next("smapb.lift");
+    const RecordFields r(records);
+    CK(launch_lift(h->bodies, h->counts, h->detd, h->rootd, scales, B, h->h, h->w, 2, r.pred2d, r.pred3d, r.root_depth,
+                   r.count, r.s4, r.s8, r.s8, r.s4, st));
     prof_mark(h, PK_LIFT, st, "lift");
     h->launches += 6;
     if (h->refine_on) {  // refined poses replace pred3d, as save_result(pred_bodys_2d, new_pred_bodys_3d, ...) does (test.py:137-145)
-        double* p3 = reinterpret_cast<double*>(rb + offsetof(smapb_record, pred3d));
-        CK(launch_refine_records(h->refine_w, reinterpret_cast<float*>(rb + offsetof(smapb_record, pred2d)), p3,
-                                 reinterpret_cast<int*>(rb + offsetof(smapb_record, count)), B, 2, sizeof(smapb_record) / 4,
-                                 sizeof(smapb_record) / 8, sizeof(smapb_record) / 4, p3, sizeof(smapb_record) / 8, st));
+        CK(launch_refine_records(h->refine_w, r.pred2d, r.pred3d, r.count, B, 2, r.s4, r.s8, r.s4, r.pred3d, r.s8, st));
         prof_mark(h, PK_LIFT, st, "refine");
         h->launches++;
     }
-    nvtxRangePop();
     return 0;
 }
 
@@ -638,16 +629,24 @@ static int gather_records(smapb_handle* h, void* comm, const smapb_record* send,
     return 0;
 }
 
-// Whole path on stream `st` (never NULL here).  gather != 0: followed by the all-gather of the records over the handle's
-// communicator; `records` then receives comm_world * B records in rank order.
+// What every whole-path entry needs, checked before the entry changes any state of the handle; selects the handle's device.
+// gather: the records are exchanged over the handle's communicator.  slot: that of the submit forms, 0 for the others.
+static int check_whole_path(smapb_handle* h, const char* fn, int B, bool gather, int slot = 0) {
+    if (!h) return -1;
+    if (!h->finalized) return fail(h, -2, std::string(fn) + ": weights not finalized");
+    if (slot < 0 || slot > 1) return fail(h, -1, std::string(fn) + ": slot must be 0 or 1");
+    if (gather && (!h->comm || !h->gather_dev))  // gather_dev: allocated when the communicator was attached
+        return fail(h, -52, std::string(fn) + ": no communicator attached (smapb_comm_create / smapb_comm_attach)");
+    cudaSetDevice(h->device);
+    return check_assoc(h, B);  // B in [1, max_batch], and a map size the association can stage
+}
+
+// Whole path on stream `st` (never NULL here), for arguments check_whole_path accepted.  gather != 0: followed by the
+// all-gather of the records over the handle's communicator; `records` then receives comm_world * B records in rank order.
 static int infer_device_impl(smapb_handle* h, const float* imgs, const double* scales, int B, int do_flip, int gather,
                              smapb_record* records, cudaStream_t st) {
-    int rc = check_assoc(h, B);
-    if (rc) return rc;
-    if (gather && !h->comm) return fail(h, -52, "smapb_infer_*_gather: no communicator attached (smapb_comm_create / smapb_comm_attach)");
-    if (gather && !h->gather_dev) return fail(h, -52, "gather buffer missing");
     Plan* plan = nullptr;
-    rc = build_plan(h, B, &plan);
+    int rc = build_plan(h, B, &plan);
     if (rc) return rc;
     do_flip = do_flip ? 1 : 0;
     gather = gather ? 1 : 0;
@@ -683,6 +682,7 @@ static int infer_device_impl(smapb_handle* h, const float* imgs, const double* s
         if (!rc && gather_in_graph) rc = gather_records(h, h->comm, h->records_dev, h->gather_dev, B, st);
         cudaGraph_t graph = nullptr;
         cudaError_t ce = cudaStreamEndCapture(st, &graph);
+        const int64_t launches = h->launches - launches_before;
         h->launches = launches_before;
         if (rc) {
             if (graph) cudaGraphDestroy(graph);
@@ -693,12 +693,12 @@ static int infer_device_impl(smapb_handle* h, const float* imgs, const double* s
         ce = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
         if (ce != cudaSuccess) return fail(h, -10, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
-        h->graphs.push_back({B, do_flip, gather, imgs, scales, exec, 0});
+        h->graphs.push_back({B, do_flip, gather, imgs, scales, exec, 0, launches});
         ge = &h->graphs.back();
     }
     ge->stamp = ++h->graph_clock;
     CK(cudaGraphLaunch(ge->exec, st));
-    h->launches += (int64_t)plan->ops.size() * (do_flip ? 2 : 1) + 6 + (do_flip ? 1 : 0) + (h->refine_on ? 1 : 0);
+    h->launches += ge->launches;
     const smapb_record* src = h->records_dev;
     if (gather) {
         if (!gather_in_graph) {  // NCCL outside the graph, still stream-ordered on the compute stream
@@ -712,22 +712,23 @@ static int infer_device_impl(smapb_handle* h, const float* imgs, const double* s
     return 0;
 }
 
-static int gather_side_init(smapb_handle* h) {
-    if (h->gather_stream) return 0;
-    CK(cudaStreamCreateWithFlags(&h->gather_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-        CK(cudaEventCreateWithFlags(&h->rec_ready[i], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&h->gather_done[i], cudaEventDisableTiming));
-        if (dev_alloc(h, &h->rec_buf[i], (size_t)h->max_batch)) return -10;
-    }
+// The exchange behind an event: the gather stream waits until `st` has written `send`, all-gathers it into `recv` and,
+// with `host`, copies the comm_world * B records there; `done` marks the end of it on the gather stream.
+static int decoupled_exchange(smapb_handle* h, cudaStream_t st, const smapb_record* send, smapb_record* recv, int B,
+                              smapb_record* host, cudaEvent_t ready, cudaEvent_t done) {
+    CK(cudaEventRecord(ready, st));
+    CK(cudaStreamWaitEvent(h->gather_stream, ready, 0));
+    if (int rc = gather_records(h, h->comm, send, recv, B, h->gather_stream)) return rc;
+    if (host)
+        CK(cudaMemcpyAsync(host, recv, (size_t)B * h->comm_world * sizeof(smapb_record), cudaMemcpyDeviceToHost,
+                           h->gather_stream));
+    CK(cudaEventRecord(done, h->gather_stream));
     return 0;
 }
 
 static int infer_device_entry(smapb_handle* h, const float* imgs, const double* scales, int B, int do_flip, int gather,
                               smapb_record* records, void* stream) {
-    if (!h) return -1;
-    if (!h->finalized) return fail(h, -2, "smapb_infer_device: weights not finalized");
-    cudaSetDevice(h->device);
+    if (int rc = check_whole_path(h, gather ? "smapb_infer_device_gather" : "smapb_infer_device", B, gather)) return rc;
     return on_stream(h, stream,
                      [&](cudaStream_t st) { return infer_device_impl(h, imgs, scales, B, do_flip, gather, records, st); });
 }
@@ -747,22 +748,18 @@ int smapb_infer_device_gather(smapb_handle* h, const float* imgs, const double* 
 // double-buffered, so a call only waits for the exchange issued two calls earlier.
 int smapb_infer_device_gather_async(smapb_handle* h, const float* imgs, const double* scales, int B, int do_flip,
                                     smapb_record* all_records, void* stream) {
-    if (!h) return -1;
-    if (!h->finalized) return fail(h, -2, "smapb_infer_device_gather_async: weights not finalized");
-    if (!h->comm) return fail(h, -52, "smapb_infer_device_gather_async: no communicator attached");
-    cudaSetDevice(h->device);
-    if (const int rc = gather_side_init(h)) return rc;
+    if (int rc = check_whole_path(h, "smapb_infer_device_gather_async", B, true)) return rc;
+    if (!h->rec_buf[0]) {  // both in one allocation, so that a failed set-up leaves nothing behind and is tried again
+        if (dev_alloc(h, &h->rec_buf[0], 2 * (size_t)h->max_batch)) return -10;
+        h->rec_buf[1] = h->rec_buf[0] + h->max_batch;
+    }
     return on_stream(h, stream, [&](cudaStream_t st) {
         const int idx = h->gather_idx;
         h->gather_idx ^= 1;
         if (h->gather_used[idx]) CK(cudaStreamWaitEvent(st, h->gather_done[idx], 0));
         int rc = infer_device_impl(h, imgs, scales, B, do_flip, 0, h->rec_buf[idx], st);
+        if (!rc) rc = decoupled_exchange(h, st, h->rec_buf[idx], all_records, B, nullptr, h->rec_ready[idx], h->gather_done[idx]);
         if (rc) return rc;
-        CK(cudaEventRecord(h->rec_ready[idx], st));
-        CK(cudaStreamWaitEvent(h->gather_stream, h->rec_ready[idx], 0));
-        rc = gather_records(h, h->comm, h->rec_buf[idx], all_records, B, h->gather_stream);
-        if (rc) return rc;
-        CK(cudaEventRecord(h->gather_done[idx], h->gather_stream));
         h->gather_used[idx] = true;
         return 0;
     });
@@ -777,16 +774,19 @@ int smapb_gather_sync(smapb_handle* h, void* stream) {
     return 0;
 }
 
+static int upload_batch(smapb_handle* h, const float* imgs, const double* scales, int B, float* to_imgs, double* to_scales,
+                        cudaStream_t st) {  // the B frames and scale rows of a host batch
+    CK(cudaMemcpyAsync(to_imgs, imgs, (size_t)B * 3 * h->in_h * h->in_w * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(to_scales, scales, (size_t)B * SMAPB_SCALE_LEN * sizeof(double), cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
 int smapb_infer_host(smapb_handle* h, const float* imgs_host, const double* scales_host, int B, int do_flip,
                      smapb_record* records_host, void* stream) {
-    if (!h) return -1;
-    if (!h->finalized) return fail(h, -2, "smapb_infer_host: weights not finalized");
-    if (B < 1 || B > h->max_batch) return fail(h, -1, "smapb_infer_host: B outside [1, max_batch]");
-    cudaSetDevice(h->device);
+    if (int rc = check_whole_path(h, "smapb_infer_host", B, false)) return rc;
     return on_stream(h, stream, [&](cudaStream_t st) {
-        CK(cudaMemcpyAsync(h->imgs_dev, imgs_host, (size_t)B * 3 * h->in_h * h->in_w * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(h->scales_dev, scales_host, (size_t)B * SMAPB_SCALE_LEN * 8, cudaMemcpyHostToDevice, st));
-        const int rc = infer_device_impl(h, h->imgs_dev, h->scales_dev, B, do_flip, 0, h->records_dev, st);
+        int rc = upload_batch(h, imgs_host, scales_host, B, h->imgs_dev, h->scales_dev, st);
+        if (!rc) rc = infer_device_impl(h, h->imgs_dev, h->scales_dev, B, do_flip, 0, h->records_dev, st);
         if (rc) return rc;
         CK(cudaMemcpyAsync(records_host, h->records_dev, (size_t)B * sizeof(smapb_record), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
@@ -796,32 +796,28 @@ int smapb_infer_host(smapb_handle* h, const float* imgs_host, const double* scal
 
 static int submit_host_impl(smapb_handle* h, int slot, const float* imgs_host, const double* scales_host, int B, int do_flip,
                             int gather, smapb_record* records_host) {
-    if (!h) return -1;
-    if (!h->finalized) return fail(h, -2, "smapb_submit_host: weights not finalized");
-    if (slot < 0 || slot > 1) return fail(h, -1, "smapb_submit_host: slot must be 0 or 1");
-    if (B < 1 || B > h->max_batch) return fail(h, -1, "smapb_submit_host: B outside [1, max_batch]");
-    if (gather && !h->comm) return fail(h, -52, "smapb_submit_host_gather: no communicator attached");
-    cudaSetDevice(h->device);
+    if (int rc = check_whole_path(h, gather ? "smapb_submit_host_gather" : "smapb_submit_host", B, gather, slot)) return rc;
     smapb_handle::Slot& S = h->slots[slot];
-    if (!S.imgs) {
+    if (!S.imgs) {  // into locals first, so that a failed set-up leaves nothing behind and is tried again
         const size_t MB = h->max_batch;
-        if (dev_alloc(h, &S.imgs, MB * 3 * h->in_h * h->in_w)) return -10;
-        if (dev_alloc(h, &S.scales, MB * SMAPB_SCALE_LEN)) return -10;
-        if (dev_alloc(h, &S.records, MB)) return -10;
-        CK(cudaEventCreateWithFlags(&S.h2d, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&S.done, cudaEventDisableTiming));
-        if (!h->copy_stream) CK(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+        float* imgs = nullptr;
+        double* scales = nullptr;
+        smapb_record* records = nullptr;
+        if (dev_alloc(h, &imgs, MB * 3 * h->in_h * h->in_w) || dev_alloc(h, &scales, MB * SMAPB_SCALE_LEN) ||
+            dev_alloc(h, &records, MB)) {
+            cudaFree(imgs), cudaFree(scales), cudaFree(records);
+            return -10;
+        }
+        S.imgs = imgs, S.scales = scales, S.records = records;
     }
     if (gather && !S.records_all && dev_alloc(h, &S.records_all, (size_t)h->max_batch * h->comm_world)) return -10;
     // the slot's buffers are free once its previous submission has completed
     if (S.used) CK(cudaStreamWaitEvent(h->copy_stream, S.done, 0));
-    CK(cudaMemcpyAsync(S.imgs, imgs_host, (size_t)B * 3 * h->in_h * h->in_w * 4, cudaMemcpyHostToDevice, h->copy_stream));
-    CK(cudaMemcpyAsync(S.scales, scales_host, (size_t)B * SMAPB_SCALE_LEN * 8, cudaMemcpyHostToDevice, h->copy_stream));
+    if (int rc = upload_batch(h, imgs_host, scales_host, B, S.imgs, S.scales, h->copy_stream)) return rc;
     CK(cudaEventRecord(S.h2d, h->copy_stream));
     cudaStream_t st = h->own_stream;
     CK(cudaStreamWaitEvent(st, S.h2d, 0));
-    int rc = infer_device_impl(h, S.imgs, S.scales, B, do_flip, 0, S.records, st);
-    if (rc) return rc;
+    if (int rc = infer_device_impl(h, S.imgs, S.scales, B, do_flip, 0, S.records, st)) return rc;
     if (!gather) {
         CK(cudaMemcpyAsync(records_host, S.records, (size_t)B * sizeof(smapb_record), cudaMemcpyDeviceToHost, st));
         CK(cudaEventRecord(S.done, st));
@@ -829,16 +825,7 @@ static int submit_host_impl(smapb_handle* h, int slot, const float* imgs_host, c
         // The exchange and the D2H of its result run on the gather stream: the compute stream goes straight on to the next
         // slot's batch and never waits for a peer.  The records are exchanged on the device (NVLink) and leave in ONE D2H -
         // nothing is re-uploaded.
-        rc = gather_side_init(h);
-        if (rc) return rc;
-        if (!S.rec_ready) CK(cudaEventCreateWithFlags(&S.rec_ready, cudaEventDisableTiming));
-        CK(cudaEventRecord(S.rec_ready, st));
-        CK(cudaStreamWaitEvent(h->gather_stream, S.rec_ready, 0));
-        rc = gather_records(h, h->comm, S.records, S.records_all, B, h->gather_stream);
-        if (rc) return rc;
-        CK(cudaMemcpyAsync(records_host, S.records_all, (size_t)B * h->comm_world * sizeof(smapb_record), cudaMemcpyDeviceToHost,
-                           h->gather_stream));
-        CK(cudaEventRecord(S.done, h->gather_stream));
+        if (int rc = decoupled_exchange(h, st, S.records, S.records_all, B, records_host, S.rec_ready, S.done)) return rc;
     }
     S.used = true;
     return 0;

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <nvtx3/nvToolsExt.h>
 #include <stdint.h>
 #include <stdlib.h>
 
@@ -104,7 +105,7 @@ struct smapb_handle {
     uint32_t* nms_masks = nullptr;  // one ballot bit per pixel of the key-point planes
     // whole-path workspace
     float* imgs_dev = nullptr;
-    float* imgs_flip = nullptr;
+    float* imgs_flip = nullptr;  // one allocation with hm_flip, scratch_detd and scratch_rootd
     float* hm = nullptr;
     float* hm_flip = nullptr;
     float* detd = nullptr;
@@ -136,6 +137,7 @@ struct smapb_handle {
         const void* scales;
         cudaGraphExec_t exec;
         uint64_t stamp;  // last use (LRU eviction)
+        int64_t launches;  // counted while the graph was captured; each replay adds them to `launches`
     };
     std::vector<GraphEntry> graphs;  // whole-path CUDA graphs keyed by (B, flip, gather, input pointers)
     uint64_t graph_clock = 0;
@@ -148,7 +150,7 @@ struct smapb_handle {
     // behind an event, so a rank's compute stream never waits for its peers
     cudaStream_t gather_stream = nullptr;
     cudaEvent_t rec_ready[2] = {nullptr, nullptr}, gather_done[2] = {nullptr, nullptr};
-    smapb_record* rec_buf[2] = {nullptr, nullptr};  // [max_batch] each: the records of the two most recent async calls
+    smapb_record* rec_buf[2] = {nullptr, nullptr};  // [max_batch] each, one allocation: the two latest async calls' records
     bool gather_used[2] = {false, false};
     int gather_idx = 0;
     double* gt_dist = nullptr;           // [max_batch][127*127] distance matrices of the GT-matching lift
@@ -201,10 +203,20 @@ inline int fail(smapb_handle* h, int code, const std::string& msg) {
     } while (0)
 
 template <typename T>
-int dev_alloc(smapb_handle* h, T** p, size_t count) {
-    CK(cudaMalloc((void**)p, count * sizeof(T)));
+int dev_alloc(smapb_handle* h, T** p, size_t count) {  // *p is written only on success
+    void* q = nullptr;
+    if (cudaMalloc(&q, count * sizeof(T)) != cudaSuccess)  // cudaGetLastError clears it for the next launch check
+        return fail(h, -10, std::string("cudaMalloc: ") + cudaGetErrorString(cudaGetLastError()));
+    *p = (T*)q;
     return 0;
 }
+
+struct NvtxScope {  // NVTX range that every return from its scope pops; next() ends it and opens the next one
+    const bool on;
+    explicit NvtxScope(const char* name, bool enable = true) : on(enable) { if (on) nvtxRangePushA(name); }
+    void next(const char* name) { if (on) nvtxRangePop(), nvtxRangePushA(name); }
+    ~NvtxScope() { if (on) nvtxRangePop(); }
+};
 
 enum ProfKind { PK_START = -1, PK_CONV = 0, PK_STEM = 1, PK_ELEM = 2, PK_ASSOC = 3, PK_LIFT = 4, PK_COPY = 5 };
 inline void prof_mark(smapb_handle* h, int kind, cudaStream_t st, const char* desc = "", double flops = 0) {

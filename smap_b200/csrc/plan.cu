@@ -1,7 +1,6 @@
 // Execution plan of libsmap_b200's backbone: conv set-up and tile choice, BN folding and weight repacking, the plan builder,
 // the plan runner, and the C ABI entry points that work on them (include/smap_b200.h, include/smap_b200_debug.h).
 #include <math.h>
-#include <nvtx3/nvToolsExt.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -848,7 +847,7 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
         st = (multi && op.stream == 1) ? h->aux_stream : main_st;
         if (multi)
             for (int w : op.waits) CK(cudaStreamWaitEvent(st, plan->ops[w].ev, 0));
-        if (h->nvtx_ops) nvtxRangePushA(op.name.empty() ? "smapb.op" : op.name.c_str());
+        const NvtxScope range(op.name.empty() ? "smapb.op" : op.name.c_str(), h->nvtx_ops);
         switch (op.kind) {
             case OP_STEM:
                 CK(launch_stem(imgs, h->stem_w, h->stem_b, B, h->in_h, h->in_w, op.out.ptr, op.out.plane(), T, st, h->f16,
@@ -893,7 +892,6 @@ int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float*
                 prof_mark(h, PK_ELEM, st, "head_merge");
                 break;
         }
-        if (h->nvtx_ops) nvtxRangePop();
         h->launches++;
         if (multi && op.record) CK(cudaEventRecord(op.ev, st));
         static const bool debug_sync = getenv("SMAPB_DEBUG_SYNC") != nullptr;
