@@ -1,10 +1,12 @@
-// Host pieces the JPEG and PNG batch drivers share (jpeg.cu, png.cu): buffer growth, the CUDA check, the buffers both
-// workspaces hold, the start of a batch decode and the report of the header-only info entry points.
+// Host pieces the JPEG and PNG batch drivers share (jpeg.cu, png.cu), and the JPEG encoder (jpeg_enc.cu) and the
+// handle (engine.h) with them: the owning device and pinned buffer, the CUDA check, the capture refusal, the start of a
+// batch decode and the report of the header-only info entry points.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/smap_b200.h"
@@ -24,42 +26,64 @@ namespace smapb {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// Makes *p hold at least n elements, device memory or pinned host memory; a buffer that grows loses its contents.
-template <typename T>
-cudaError_t grow_buffer(T** p, size_t* cap, size_t n, bool pinned) {
-    if (n <= *cap) return cudaSuccess;
-    if (*p) pinned ? cudaFreeHost(*p) : cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    cudaError_t e = pinned ? cudaMallocHost((void**)p, n * sizeof(T)) : cudaMalloc((void**)p, n * sizeof(T));
-    if (e == cudaSuccess) *cap = n;
-    return e;
-}
+// n elements of T in device memory (cudaMalloc) or, Pinned, in page-locked host memory (cudaMallocHost), freed by the
+// destructor.  Move-only; it converts to T*, so kernel launches and ConvParams take it as they take a raw pointer.
+template <typename T, bool Pinned>
+class Buffer {
+  public:
+    Buffer() = default;
+    Buffer(Buffer&& o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr, o.cap_ = 0; }
+    Buffer& operator=(Buffer&& o) noexcept {
+        if (this != &o) {
+            reset();
+            std::swap(p_, o.p_);
+            std::swap(cap_, o.cap_);
+        }
+        return *this;
+    }
+    ~Buffer() { reset(); }
 
-template <typename T>
-cudaError_t grow(T** p, size_t* cap, size_t n) { return grow_buffer(p, cap, n, false); }
+    // Makes the buffer hold at least n elements; one that grows loses its contents.  A failed allocation leaves it empty
+    // and is taken off the runtime's last-error state, so that the next launch check does not report it.
+    cudaError_t grow(size_t n) {
+        if (n <= cap_) return cudaSuccess;
+        reset();
+        void* q = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&q, n * sizeof(T)) : cudaMalloc(&q, n * sizeof(T));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return e;
+        }
+        p_ = (T*)q, cap_ = n;
+        return cudaSuccess;
+    }
+    void reset() {
+        if (p_) Pinned ? cudaFreeHost(p_) : cudaFree(p_);
+        p_ = nullptr, cap_ = 0;
+    }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+    size_t capacity() const { return cap_; }
 
-template <typename T>
-cudaError_t grow_pinned(T** p, size_t* cap, size_t n) { return grow_buffer(p, cap, n, true); }
-
-// The buffers of both workspaces: the pinned staging area of a batch (descriptors and file bytes, one upload per batch),
-// its device copy, a small device area (statuses and counters, laid out by each driver) and its pinned mirror.
-struct DecodeBuffers {
-    uint8_t* host = nullptr;
-    size_t host_cap = 0;
-    uint8_t* dev_in = nullptr;
-    size_t dev_in_cap = 0;
-    int* small = nullptr;
-    size_t small_cap = 0;
-    int* small_host = nullptr;
-    size_t small_host_cap = 0;
+  private:
+    T* p_ = nullptr;
+    size_t cap_ = 0;  // elements
 };
+template <typename T>
+using DeviceBuffer = Buffer<T, false>;
+template <typename T>
+using PinnedBuffer = Buffer<T, true>;
 
-inline void free_decode_buffers(DecodeBuffers* b) {
-    if (b->host) cudaFreeHost(b->host);
-    if (b->small_host) cudaFreeHost(b->small_host);
-    if (b->dev_in) cudaFree(b->dev_in);
-    if (b->small) cudaFree(b->small);
+// Refuses a stream under capture: the codecs synchronise and may grow their workspaces.  0, or -1 with the text, prefixed
+// by name, in *err (-10 when the stream cannot be queried).
+inline int refuse_capture(const char* name, cudaStream_t st, std::string* err) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    DECODE_CK(cudaStreamIsCapturing(st, &cap));
+    if (cap != cudaStreamCaptureStatusNone) {
+        *err = std::string(name) + ": not capturable (it synchronises and may grow its workspace)";
+        return -1;
+    }
+    return 0;
 }
 
 // The start of a batch decode.  Checks the arguments, refuses a stream under capture (the drivers synchronise and may
@@ -73,12 +97,7 @@ int decode_preamble(const char* name, int n, const uint8_t* const* data, const i
         *err = std::string(name) + ": null argument";
         return -1;
     }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    DECODE_CK(cudaStreamIsCapturing(st, &cap));
-    if (cap != cudaStreamCaptureStatusNone) {
-        *err = std::string(name) + ": not capturable (it synchronises and may grow its workspace)";
-        return -1;
-    }
+    if (int rc = refuse_capture(name, st, err)) return rc;
     H->resize(n);
     for (int i = 0; i < n; i++) {
         status[i] = walk(data[i], nbytes[i], &(*H)[i]);

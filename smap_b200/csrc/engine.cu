@@ -145,18 +145,18 @@ int smapb_create(smapb_handle** out, int device, int max_batch, int in_h, int in
     const size_t hw = (size_t)h->h * h->w;
     const size_t MB = max_batch;
     int rc = 0;
-    rc |= dev_alloc(h, &h->peaks, MB * NJ * (MAXP + 1) * 3);
-    rc |= dev_alloc(h, &h->scores, MB * NL * MAXP * MAXP);
-    rc |= dev_alloc(h, &h->bodies, MB * MAXP * NJ * 4);
-    rc |= dev_alloc(h, &h->counts, MB);
-    rc |= dev_alloc(h, &h->nms_masks, nms_mask_words(max_batch, h->h, h->w));
-    rc |= dev_alloc(h, &h->imgs_dev, MB * 3 * in_h * in_w);
-    rc |= dev_alloc(h, &h->hm, MB * NC2D * hw);
-    rc |= dev_alloc(h, &h->detd, MB * NL * hw);
-    rc |= dev_alloc(h, &h->rootd, MB * hw);
-    rc |= dev_alloc(h, &h->scales_dev, MB * SMAPB_SCALE_LEN);
-    rc |= dev_alloc(h, &h->records_dev, MB);
-    rc |= dev_alloc(h, &h->sat_dev, 1);
+    rc |= dev_alloc(h, h->peaks, MB * NJ * (MAXP + 1) * 3);
+    rc |= dev_alloc(h, h->scores, MB * NL * MAXP * MAXP);
+    rc |= dev_alloc(h, h->bodies, MB * MAXP * NJ * 4);
+    rc |= dev_alloc(h, h->counts, MB);
+    rc |= dev_alloc(h, h->nms_masks, nms_mask_words(max_batch, h->h, h->w));
+    rc |= dev_alloc(h, h->imgs_dev, MB * 3 * in_h * in_w);
+    rc |= dev_alloc(h, h->hm, MB * NC2D * hw);
+    rc |= dev_alloc(h, h->detd, MB * NL * hw);
+    rc |= dev_alloc(h, h->rootd, MB * hw);
+    rc |= dev_alloc(h, h->scales_dev, MB * SMAPB_SCALE_LEN);
+    rc |= dev_alloc(h, h->records_dev, MB);
+    rc |= dev_alloc(h, h->sat_dev, 1);
     if (!rc && cudaMemset(h->sat_dev, 0, sizeof(unsigned long long)) != cudaSuccess) rc = -10;
     if (rc) {
         g_create_error = h->err;
@@ -182,34 +182,14 @@ void smapb_destroy(smapb_handle* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
-    for (auto& kv : h->plans) free_plan(kv.second.get());
     drop_graphs(h);
-    for (auto& S : h->slots) {
-        cudaFree(S.imgs);
-        cudaFree(S.scales);
-        cudaFree(S.records);
-        cudaFree(S.records_all);
-    }
     if (h->comm && h->comm_owned && nccl_api().CommDestroy) nccl_api().CommDestroy(h->comm);
-    cudaFree(h->rec_buf[0]);
     for (cudaStream_t* s : handle_streams(h))
         if (*s) cudaStreamDestroy(*s);
     for (cudaEvent_t* e : handle_events(h))
         if (*e) cudaEventDestroy(*e);
     for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
-    free_layers(h);
-    void* ptrs[] = {h->peaks, h->scores, h->bodies, h->counts, h->imgs_dev, h->imgs_flip, h->hm, h->detd, h->rootd,
-                    h->scales_dev, h->records_dev, h->stem_w, h->stem_b, h->gather_dev, h->gt_dist, h->nms_masks, h->sat_dev};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    if (h->refine_buf) cudaFree(h->refine_buf);
-    if (h->roles_dev) cudaFree(h->roles_dev);
-    if (h->pre_stage) cudaFree(h->pre_stage);
-    for (auto& e : h->pre_cache) cudaFree(e.second.buf);
-    smapb::jpeg_workspace_destroy(h->jpeg);
-    smapb::png_workspace_destroy(h->png);
-    smapb::jpeg_enc_workspace_destroy(h->jpeg_enc);
-    delete h;
+    delete h;  // the plans, weights, buffers and codec workspaces free themselves
 }
 
 int smapb_load_weight(smapb_handle* h, const char* key, const float* host, const int64_t* shape, int ndim) {
@@ -301,7 +281,7 @@ int smapb_lift3d_gt(smapb_handle* h, const float* bodies, const int* counts, con
     cudaSetDevice(h->device);
     if (B < 1 || B > h->max_batch) return fail(h, -1, "smapb_lift3d_gt: B outside [1, max_batch]");
     if (gmax < 1) return fail(h, -1, "smapb_lift3d_gt: gmax < 1");
-    if (!h->gt_dist && dev_alloc(h, &h->gt_dist, (size_t)h->max_batch * MAXP * MAXP)) return -10;
+    if (dev_alloc(h, h->gt_dist, (size_t)h->max_batch * MAXP * MAXP)) return -10;
     CK(launch_lift_gt(bodies, counts, detd, rootd, scales, gt_roots, gt_counts, gmax, h->gt_dist, B, h->h, h->w, 2, pred2d,
                       pred3d, root_depth, counts_out, (cudaStream_t)stream));
     h->launches++;
@@ -324,15 +304,13 @@ static int pre_entry(smapb_handle* h, int img_h, int img_w, smapb_handle::PreEnt
         }
         if (h->pre_cache.size() >= 256) {  // bound the cache: drop everything (streams are idle after the sync)
             cudaDeviceSynchronize();
-            for (auto& e : h->pre_cache) cudaFree(e.second.buf);
             h->pre_cache.clear();
         }
         const ResizePlan& P = E.plan;
         const size_t nx = P.xofs.size(), ny = P.yofs.size();  // ny = 2 * dst_h
         const size_t bytes = nx * 4 + ny * 4 + nx * 2 * 2 + ny * 2 + 64;
-        CK(cudaMalloc(&E.buf, bytes));
-        char* d = (char*)E.buf;
-        int* xo = (int*)d;
+        CK(E.buf.grow(bytes));
+        int* xo = (int*)E.buf.get();
         int* yo = xo + nx;
         short* xc = (short*)(yo + ny);
         short* yc = xc + 2 * nx;
@@ -340,10 +318,7 @@ static int pre_entry(smapb_handle* h, int img_h, int img_w, smapb_handle::PreEnt
         if (ce == cudaSuccess) ce = cudaMemcpy(yo, P.yofs.data(), ny * 4, cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(xc, P.xcoef.data(), nx * 2 * 2, cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(yc, P.ycoef.data(), ny * 2, cudaMemcpyHostToDevice);
-        if (ce != cudaSuccess) {
-            cudaFree(E.buf);
-            return fail(h, -10, std::string("smapb_preprocess: table upload: ") + cudaGetErrorString(ce));
-        }
+        if (ce != cudaSuccess) return fail(h, -10, std::string("smapb_preprocess: table upload: ") + cudaGetErrorString(ce));
         E.tab = {xo, xc, yo, yc};
         it = h->pre_cache.emplace(key, std::move(E)).first;
     }
@@ -385,13 +360,9 @@ int smapb_preprocess_host(smapb_handle* h, const uint8_t* bgr_host, int img_h, i
     int rc = pre_entry(h, img_h, img_w, &E);  // refuse the geometry before staging its pixels
     if (rc) return rc;
     const size_t bytes = (size_t)img_h * img_w * 3;
-    if (bytes > h->pre_stage_bytes) {
-        cudaDeviceSynchronize();
-        if (h->pre_stage) cudaFree(h->pre_stage);
-        h->pre_stage = nullptr;
-        h->pre_stage_bytes = 0;
-        CK(cudaMalloc((void**)&h->pre_stage, bytes));
-        h->pre_stage_bytes = bytes;
+    if (bytes > h->pre_stage.capacity()) {
+        cudaDeviceSynchronize();  // a pending copy may still read the old staging buffer
+        CK(h->pre_stage.grow(bytes));
     }
     CK(cudaMemcpyAsync(h->pre_stage, bgr_host, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return smapb_preprocess(h, h->pre_stage, img_h, img_w, out_nchw_dev, scale_row_host, stream);
@@ -405,8 +376,8 @@ int smapb_decode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* jpeg_host
         return -1;
     }
     cudaSetDevice(h->device);
-    if (!h->jpeg) h->jpeg = smapb::jpeg_workspace_create();
-    return smapb::jpeg_decode(h->jpeg, n, jpeg_host, nbytes, bgr_dev, flags, status_host, (cudaStream_t)stream, &h->launches,
+    if (!h->jpeg) h->jpeg.reset(smapb::jpeg_workspace_create());
+    return smapb::jpeg_decode(h->jpeg.get(), n, jpeg_host, nbytes, bgr_dev, flags, status_host, (cudaStream_t)stream, &h->launches,
                               &h->err);
 }
 
@@ -419,16 +390,16 @@ int smapb_decode_png(smapb_handle* h, int n, const uint8_t* const* png_host, con
                      int* status_host, void* stream) {
     if (!h) return -1;
     cudaSetDevice(h->device);
-    if (!h->png) h->png = smapb::png_workspace_create();
-    return smapb::png_decode(h->png, n, png_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
+    if (!h->png) h->png.reset(smapb::png_workspace_create());
+    return smapb::png_decode(h->png.get(), n, png_host, nbytes, bgr_dev, status_host, (cudaStream_t)stream, &h->launches, &h->err);
 }
 
 int smapb_encode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w, int quality,
                          const smapb_record* records_dev, const double* scales_dev, int flags, int64_t* nbytes_host, void* stream) {
     if (!h) return -1;
     cudaSetDevice(h->device);
-    if (!h->jpeg_enc) h->jpeg_enc = smapb::jpeg_enc_workspace_create();
-    return smapb::jpeg_encode(h->jpeg_enc, n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, flags, nbytes_host,
+    if (!h->jpeg_enc) h->jpeg_enc.reset(smapb::jpeg_enc_workspace_create());
+    return smapb::jpeg_encode(h->jpeg_enc.get(), n, bgr_dev, img_h, img_w, quality, records_dev, scales_dev, flags, nbytes_host,
                               (cudaStream_t)stream, &h->launches, &h->err);
 }
 
@@ -439,13 +410,13 @@ int smapb_encode_jpeg(smapb_handle* h, int n, const uint8_t* const* bgr_dev, con
 
 int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes) {
     if (!h || !data) return -1;
-    *data = smapb::jpeg_enc_result(h->jpeg_enc, i, nbytes);
+    *data = smapb::jpeg_enc_result(h->jpeg_enc.get(), i, nbytes);
     return *data ? 0 : -1;
 }
 
 int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4) {
     if (!h || !counts4) return -1;
-    smapb::png_last_stats(h->png, counts4);
+    smapb::png_last_stats(h->png.get(), counts4);
     return 0;
 }
 
@@ -513,7 +484,7 @@ int smapb_refine_finalize(smapb_handle* h) {
         }
         off += (size_t)K * N + N;
     }
-    if (!h->refine_buf) CK(cudaMalloc((void**)&h->refine_buf, total * sizeof(float)));
+    CK(h->refine_buf.grow(total));
     CK(cudaMemcpy(h->refine_buf, buf.data(), total * sizeof(float), cudaMemcpyHostToDevice));
     for (int l = 0; l < RF_LAYERS; l++) {
         h->refine_w.w[l] = h->refine_buf + w_off[l];
@@ -585,7 +556,7 @@ static int infer_body(smapb_handle* h, Plan* plan, const float* imgs, const doub
     if (do_flip) {
         if (!h->imgs_flip) {  // one allocation, so that a failed set-up leaves nothing behind and is tried again
             const size_t MB = h->max_batch, hw = (size_t)h->h * h->w, frames = MB * 3 * h->in_h * h->in_w;
-            if (dev_alloc(h, &h->imgs_flip, frames + MB * (NC2D + NL + 1) * hw)) return -10;
+            if (dev_alloc(h, h->imgs_flip, frames + MB * (NC2D + NL + 1) * hw)) return -10;
             h->hm_flip = h->imgs_flip + frames;  // every part 256-byte aligned: in_h and in_w are multiples of 32
             h->scratch_detd = h->hm_flip + MB * NC2D * hw;
             h->scratch_rootd = h->scratch_detd + MB * NL * hw;
@@ -749,16 +720,15 @@ int smapb_infer_device_gather(smapb_handle* h, const float* imgs, const double* 
 int smapb_infer_device_gather_async(smapb_handle* h, const float* imgs, const double* scales, int B, int do_flip,
                                     smapb_record* all_records, void* stream) {
     if (int rc = check_whole_path(h, "smapb_infer_device_gather_async", B, true)) return rc;
-    if (!h->rec_buf[0]) {  // both in one allocation, so that a failed set-up leaves nothing behind and is tried again
-        if (dev_alloc(h, &h->rec_buf[0], 2 * (size_t)h->max_batch)) return -10;
-        h->rec_buf[1] = h->rec_buf[0] + h->max_batch;
-    }
+    // both in one allocation, so that a failed set-up leaves nothing behind and is tried again
+    if (dev_alloc(h, h->rec_buf, 2 * (size_t)h->max_batch)) return -10;
     return on_stream(h, stream, [&](cudaStream_t st) {
         const int idx = h->gather_idx;
         h->gather_idx ^= 1;
         if (h->gather_used[idx]) CK(cudaStreamWaitEvent(st, h->gather_done[idx], 0));
-        int rc = infer_device_impl(h, imgs, scales, B, do_flip, 0, h->rec_buf[idx], st);
-        if (!rc) rc = decoupled_exchange(h, st, h->rec_buf[idx], all_records, B, nullptr, h->rec_ready[idx], h->gather_done[idx]);
+        smapb_record* const rec = h->rec_buf + (size_t)idx * h->max_batch;
+        int rc = infer_device_impl(h, imgs, scales, B, do_flip, 0, rec, st);
+        if (!rc) rc = decoupled_exchange(h, st, rec, all_records, B, nullptr, h->rec_ready[idx], h->gather_done[idx]);
         if (rc) return rc;
         h->gather_used[idx] = true;
         return 0;
@@ -800,17 +770,15 @@ static int submit_host_impl(smapb_handle* h, int slot, const float* imgs_host, c
     smapb_handle::Slot& S = h->slots[slot];
     if (!S.imgs) {  // into locals first, so that a failed set-up leaves nothing behind and is tried again
         const size_t MB = h->max_batch;
-        float* imgs = nullptr;
-        double* scales = nullptr;
-        smapb_record* records = nullptr;
-        if (dev_alloc(h, &imgs, MB * 3 * h->in_h * h->in_w) || dev_alloc(h, &scales, MB * SMAPB_SCALE_LEN) ||
-            dev_alloc(h, &records, MB)) {
-            cudaFree(imgs), cudaFree(scales), cudaFree(records);
+        DeviceBuffer<float> imgs;
+        DeviceBuffer<double> scales;
+        DeviceBuffer<smapb_record> records;
+        if (dev_alloc(h, imgs, MB * 3 * h->in_h * h->in_w) || dev_alloc(h, scales, MB * SMAPB_SCALE_LEN) ||
+            dev_alloc(h, records, MB))
             return -10;
-        }
-        S.imgs = imgs, S.scales = scales, S.records = records;
+        S.imgs = std::move(imgs), S.scales = std::move(scales), S.records = std::move(records);
     }
-    if (gather && !S.records_all && dev_alloc(h, &S.records_all, (size_t)h->max_batch * h->comm_world)) return -10;
+    if (gather && dev_alloc(h, S.records_all, (size_t)h->max_batch * h->comm_world)) return -10;
     // the slot's buffers are free once its previous submission has completed
     if (S.used) CK(cudaStreamWaitEvent(h->copy_stream, S.done, 0));
     if (int rc = upload_batch(h, imgs_host, scales_host, B, S.imgs, S.scales, h->copy_stream)) return rc;
@@ -870,13 +838,9 @@ static int set_comm(smapb_handle* h, void* comm, bool owned, int rank, int world
     for (auto& kv : h->eager_runs)
         if (kv.first.second & 1) kv.second = 0;
     h->comm = comm, h->comm_owned = owned, h->comm_rank = rank, h->comm_world = world;
-    if (h->gather_dev) cudaFree(h->gather_dev);
-    h->gather_dev = nullptr;
-    for (auto& S : h->slots) {
-        cudaFree(S.records_all);
-        S.records_all = nullptr;
-    }
-    if (dev_alloc(h, &h->gather_dev, (size_t)world * h->max_batch)) return -10;
+    h->gather_dev.reset();
+    for (auto& S : h->slots) S.records_all.reset();
+    if (dev_alloc(h, h->gather_dev, (size_t)world * h->max_batch)) return -10;
     return 0;
 }
 
@@ -929,7 +893,7 @@ int smapb_profile_begin(smapb_handle* h) {
     h->prof_used = 0;
     if (getenv("SMAPB_ROLES_PLAN")) {
         cudaSetDevice(h->device);
-        if (!h->roles_dev) CK(cudaMalloc((void**)&h->roles_dev, ROLES_CAP * 16 * sizeof(long long)));
+        CK(h->roles_dev.grow(ROLES_CAP * 16));
         CK(cudaMemset(h->roles_dev, 0, ROLES_CAP * 16 * sizeof(long long)));
         h->roles_used = 0;
         h->roles_desc.clear();

@@ -14,6 +14,7 @@
 
 #include "../../include/smap_b200.h"
 #include "conv_tc.cuh"
+#include "decode_host.h"
 #include "jpeg.h"
 #include "jpeg_enc.h"
 #include "png.h"
@@ -33,12 +34,14 @@ struct ActF32 {
     int N = 0, H = 0, W = 0, C = 0;
 };
 
-struct ConvLayer {
+struct ConvGeom {
     std::string name;
     int Cin = 0, Cout = 0, Cout_pad = 0, k = 1, stride = 1, pad = 0;
     int Cin2 = 0, stride2 = 1;  // K-concatenated second 1x1 input (weights hold Cin + Cin2 columns)
-    __nv_bfloat16* w_dev = nullptr;  // [T][taps][Cout_pad][Cin]
-    float* bias_dev = nullptr;       // [Cout_pad]
+};
+struct ConvLayer : ConvGeom {
+    DeviceBuffer<__nv_bfloat16> w_dev;  // [T][taps][Cout_pad][Cin]
+    DeviceBuffer<float> bias_dev;       // [Cout_pad]
 };
 
 enum OpKind { OP_STEM, OP_S2D, OP_MAXPOOL, OP_CONV, OP_HEADMERGE, OP_TAPSUM };
@@ -66,10 +69,16 @@ struct Op {
     int dims[4] = {0, 0, 0, 0};
 };
 
-struct Plan {
+struct Plan {  // owns its tensors and the events of its ops
+    Plan() = default;
+    Plan(const Plan&) = delete;
+    ~Plan() {
+        for (Op& op : ops)
+            if (op.ev) cudaEventDestroy(op.ev);
+    }
     int B = 0;
     std::vector<Op> ops;
-    std::vector<void*> allocs;
+    std::vector<DeviceBuffer<uint8_t>> allocs;
     int n_conv = 0;
     double conv_flops = 0;
     std::map<const void*, int> producer;  // tensor -> index of the op that writes it (build time)
@@ -87,39 +96,39 @@ struct smapb_handle {
     std::map<std::string, std::vector<float>> raw;
     std::map<std::string, std::vector<int64_t>> raw_shape;
     std::map<std::string, smapb::ConvLayer> layers;
-    float* stem_w = nullptr;  // [147][64]
+    smapb::DeviceBuffer<float> stem_w;  // [147][64]
     smapb::ConvLayer stem_tc;  // space-to-depth tensor-core stem (4 ky-blocks x 64 k)
     int stem_tc_ok = -1;      // -1 untested, 0 overlapped TMA view rejected (CUDA-core stem), 1 in use
-    float* stem_b = nullptr;
+    smapb::DeviceBuffer<float> stem_b;
     int nterms = 3;  // MMA terms (3 = bf16x3, 1 = bf16 or fp16)
     int planes = 2;  // activation planes (2 or 1)
     bool f16 = false;  // element format of weights and activations: fp16 (SMAPB_PREC_FP16) instead of bf16
-    unsigned long long* sat_dev = nullptr;  // fp16: activation elements clamped to +-65504 (smapb_saturation_count)
+    smapb::DeviceBuffer<unsigned long long> sat_dev;  // fp16: activation elements clamped to +-65504 (smapb_saturation_count)
     bool finalized = false;
     std::map<int, std::unique_ptr<smapb::Plan>> plans;
     // association workspace (sized for max_batch)
-    float* peaks = nullptr;
-    float* scores = nullptr;
-    float* bodies = nullptr;
-    int* counts = nullptr;
-    uint32_t* nms_masks = nullptr;  // one ballot bit per pixel of the key-point planes
+    smapb::DeviceBuffer<float> peaks;
+    smapb::DeviceBuffer<float> scores;
+    smapb::DeviceBuffer<float> bodies;
+    smapb::DeviceBuffer<int> counts;
+    smapb::DeviceBuffer<uint32_t> nms_masks;  // one ballot bit per pixel of the key-point planes
     // whole-path workspace
-    float* imgs_dev = nullptr;
-    float* imgs_flip = nullptr;  // one allocation with hm_flip, scratch_detd and scratch_rootd
-    float* hm = nullptr;
+    smapb::DeviceBuffer<float> imgs_dev;
+    smapb::DeviceBuffer<float> imgs_flip;  // one allocation with hm_flip, scratch_detd and scratch_rootd
+    smapb::DeviceBuffer<float> hm;
     float* hm_flip = nullptr;
-    float* detd = nullptr;
-    float* rootd = nullptr;
+    smapb::DeviceBuffer<float> detd;
+    smapb::DeviceBuffer<float> rootd;
     float* scratch_detd = nullptr;
     float* scratch_rootd = nullptr;
-    double* scales_dev = nullptr;
-    smapb_record* records_dev = nullptr;
+    smapb::DeviceBuffer<double> scales_dev;
+    smapb::DeviceBuffer<smapb_record> records_dev;
     // host-facing pipeline (smapb_submit_host / smapb_wait): two slots, H2D of slot s+1 overlaps the compute of slot s
     struct Slot {
-        float* imgs = nullptr;
-        double* scales = nullptr;
-        smapb_record* records = nullptr;
-        smapb_record* records_all = nullptr;  // [comm_world * max_batch], gathered variant
+        smapb::DeviceBuffer<float> imgs;
+        smapb::DeviceBuffer<double> scales;
+        smapb::DeviceBuffer<smapb_record> records;
+        smapb::DeviceBuffer<smapb_record> records_all;  // [comm_world * max_batch], gathered variant
         cudaEvent_t h2d = nullptr, done = nullptr, rec_ready = nullptr;
         bool used = false;
     } slots[2];
@@ -145,32 +154,34 @@ struct smapb_handle {
     void* comm = nullptr;  // ncclComm_t
     bool comm_owned = false;
     int comm_rank = 0, comm_world = 1;
-    smapb_record* gather_dev = nullptr;  // [comm_world * max_batch]
+    smapb::DeviceBuffer<smapb_record> gather_dev;  // [comm_world * max_batch]
     // decoupled exchange (smapb_infer_device_gather_async / smapb_submit_host_gather): the all-gather runs on its own stream
     // behind an event, so a rank's compute stream never waits for its peers
     cudaStream_t gather_stream = nullptr;
     cudaEvent_t rec_ready[2] = {nullptr, nullptr}, gather_done[2] = {nullptr, nullptr};
-    smapb_record* rec_buf[2] = {nullptr, nullptr};  // [max_batch] each, one allocation: the two latest async calls' records
+    smapb::DeviceBuffer<smapb_record> rec_buf;  // [2][max_batch]: the two latest async calls' records
     bool gather_used[2] = {false, false};
     int gather_idx = 0;
-    double* gt_dist = nullptr;           // [max_batch][127*127] distance matrices of the GT-matching lift
+    smapb::DeviceBuffer<double> gt_dist;  // [max_batch][127*127] distance matrices of the GT-matching lift
     bool nccl_in_graph = getenv("SMAPB_NCCL_EAGER") == nullptr;
     bool nvtx_ops = getenv("SMAPB_NVTX") != nullptr;  // one NVTX range per plan op (phase ranges are always emitted)
     // pre-processing (SURVEY 8(f) f1): resampling tables per source geometry, staging for host images
     struct PreEntry {
         smapb::ResizePlan plan;
         smapb::ResizeTablesDev tab{};
-        void* buf = nullptr;
+        smapb::DeviceBuffer<char> buf;
     };
     std::map<std::pair<int, int>, PreEntry> pre_cache;
-    uint8_t* pre_stage = nullptr;
-    size_t pre_stage_bytes = 0;
-    smapb::JpegWorkspace* jpeg = nullptr;  // JPEG decoding (smapb_decode_jpeg), created on first use
-    smapb::PngWorkspace* png = nullptr;    // PNG decoding (smapb_decode_png), created on first use
-    smapb::JpegEncWorkspace* jpeg_enc = nullptr;  // JPEG encoding (smapb_encode_jpeg), created on first use
+    smapb::DeviceBuffer<uint8_t> pre_stage;
+    // JPEG decoding (smapb_decode_jpeg), PNG decoding (smapb_decode_png) and JPEG encoding (smapb_encode_jpeg), created on
+    // first use
+    std::unique_ptr<smapb::JpegWorkspace, void (*)(smapb::JpegWorkspace*)> jpeg{nullptr, smapb::jpeg_workspace_destroy};
+    std::unique_ptr<smapb::PngWorkspace, void (*)(smapb::PngWorkspace*)> png{nullptr, smapb::png_workspace_destroy};
+    std::unique_ptr<smapb::JpegEncWorkspace, void (*)(smapb::JpegEncWorkspace*)> jpeg_enc{nullptr,
+                                                                                          smapb::jpeg_enc_workspace_destroy};
     // RefineNet (optional post-processing step, SURVEY 8(f) f2)
     std::map<std::string, std::vector<float>> refine_raw;
-    float* refine_buf = nullptr;  // folded, transposed weights + biases of the five layers
+    smapb::DeviceBuffer<float> refine_buf;  // folded, transposed weights + biases of the five layers
     smapb::RefineWeights refine_w{};
     bool refine_ready = false, refine_on = false;
     std::map<std::pair<int, int>, int> eager_runs;  // (B, flip) -> number of eager executions so far
@@ -182,7 +193,7 @@ struct smapb_handle {
     std::vector<double> prof_flops;
     size_t prof_used = 0;
     // per-launch role counters of the conv kernels inside a profiled (eager) run: SMAPB_ROLES_PLAN=<csv path>
-    long long* roles_dev = nullptr;  // [ROLES_CAP][16]
+    smapb::DeviceBuffer<long long> roles_dev;  // [ROLES_CAP][16]
     size_t roles_used = 0;
     std::vector<std::string> roles_desc;
 };
@@ -203,12 +214,9 @@ inline int fail(smapb_handle* h, int code, const std::string& msg) {
     } while (0)
 
 template <typename T>
-int dev_alloc(smapb_handle* h, T** p, size_t count) {  // *p is written only on success
-    void* q = nullptr;
-    if (cudaMalloc(&q, count * sizeof(T)) != cudaSuccess)  // cudaGetLastError clears it for the next launch check
-        return fail(h, -10, std::string("cudaMalloc: ") + cudaGetErrorString(cudaGetLastError()));
-    *p = (T*)q;
-    return 0;
+int dev_alloc(smapb_handle* h, DeviceBuffer<T>& b, size_t count) {  // b.grow(count), its failure reported as fail() does
+    const cudaError_t e = b.grow(count);
+    return e == cudaSuccess ? 0 : fail(h, -10, std::string("cudaMalloc: ") + cudaGetErrorString(e));
 }
 
 struct NvtxScope {  // NVTX range that every return from its scope pops; next() ends it and opens the next one
@@ -239,8 +247,6 @@ inline void prof_mark(smapb_handle* h, int kind, cudaStream_t st, const char* de
 // plan.cu
 int build_plan(smapb_handle* h, int B, Plan** out_plan);
 int run_plan(smapb_handle* h, Plan* plan, const float* imgs, float* hm2d, float* detd, float* rootd, cudaStream_t st);
-void free_plan(Plan* plan);
-void free_layers(smapb_handle* h);  // the device weights of every conv layer, the tensor-core stem's included
 // engine.cu
 void drop_graphs(smapb_handle* h, bool gather_only = false);  // destroys the cached whole-path graphs (or those with the all-gather)
 

@@ -1299,21 +1299,18 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevImage* __restrict_
 }  // namespace
 
 // staging: descriptors and scan bytes; small: status[m] then changed[passes]
-struct JpegWorkspace : DecodeBuffers {
-    uint8_t* unst = nullptr;
-    size_t unst_cap = 0;
-    SubState* st[2] = {nullptr, nullptr};
-    size_t st_cap[2] = {0, 0};
-    int* base = nullptr;
-    size_t base_cap = 0;
-    int16_t* coef = nullptr;
-    size_t coef_cap = 0;
-    unsigned long long* acr_mask = nullptr;  // AC refinement: history masks and records of a round's blocks
-    size_t acr_mask_cap = 0;
-    AcrRecord* acr_rec = nullptr;
-    size_t acr_rec_cap = 0;
-    uint8_t* planes = nullptr;
-    size_t planes_cap = 0;
+struct JpegWorkspace {
+    PinnedBuffer<uint8_t> host;
+    DeviceBuffer<uint8_t> dev_in;
+    DeviceBuffer<int> small;
+    PinnedBuffer<int> small_host;
+    DeviceBuffer<uint8_t> unst;
+    DeviceBuffer<SubState> st[2];
+    DeviceBuffer<int> base;
+    DeviceBuffer<int16_t> coef;
+    DeviceBuffer<unsigned long long> acr_mask;  // AC refinement: history masks and records of a round's blocks
+    DeviceBuffer<AcrRecord> acr_rec;
+    DeviceBuffer<uint8_t> planes;
     int sub_bits = SUB_BITS;  // subsequence length of the Huffman passes (SMAPB_JPEG_SUB_BITS)
 };
 
@@ -1326,14 +1323,7 @@ JpegWorkspace* jpeg_workspace_create() {
     return ws;
 }
 
-void jpeg_workspace_destroy(JpegWorkspace* ws) {
-    if (!ws) return;
-    free_decode_buffers(ws);
-    void* d[] = {ws->unst, ws->st[0], ws->st[1], ws->base, ws->coef, ws->acr_mask, ws->acr_rec, ws->planes};
-    for (void* p : d)
-        if (p) cudaFree(p);
-    delete ws;
-}
+void jpeg_workspace_destroy(JpegWorkspace* ws) { delete ws; }
 
 namespace {
 // What one round (the r-th scan of every image that has one) launches: subsequences [sub_lo, sub_lo + nsub) of its
@@ -1394,7 +1384,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
     // scans round by round, so that every round's subsequences are contiguous
     std::vector<Round> rounds(nrounds);
     std::vector<int> huff_l, dc_l, dcr_l, acr_l, acrs_l;
-    int acr_cap = 0;  // blocks of the masks and records: the most any round needs
+    int acr_max = 0;  // blocks of the masks and records: the most any round needs
     for (int r = 0; r < nrounds; r++) {
         Round& R = rounds[r];
         R.sub_lo = (int)subs.size();
@@ -1498,7 +1488,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
         put(dcr_l, &R.dcr_off, &R.ndcr);
         put(acr_l, &R.acr_off, &R.nacr);
         put(acrs_l, &R.acrs_off, &R.nacrs);
-        acr_cap = std::max(acr_cap, R.acr_total);
+        acr_max = std::max(acr_max, R.acr_total);
     }
     const int nscan = (int)scans.size();
     int max_passes = 1;
@@ -1510,7 +1500,7 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
                  o_sub = align_up(o_seg + sizeof(DevSeg) * segs.size(), 256),
                  o_list = align_up(o_sub + sizeof(DevSub) * subs.size(), 256),
                  o_raw = align_up(o_list + sizeof(int) * lists.size(), 256), total = o_raw + raw_total;
-    DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total));
+    DECODE_CK(ws->host.grow(total));
     DECODE_CK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
     memcpy(ws->host + o_img, imgs.data(), sizeof(DevImage) * m);
     memcpy(ws->host + o_scan, scans.data(), sizeof(DevScan) * nscan);
@@ -1530,19 +1520,19 @@ int jpeg_decode(JpegWorkspace* ws, int n, const uint8_t* const* jpeg, const int6
             }
     }
     const size_t nsub = std::max<size_t>(1, subs.size());
-    DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total));
-    DECODE_CK(grow(&ws->unst, &ws->unst_cap, (size_t)unst_total));
-    DECODE_CK(grow(&ws->st[0], &ws->st_cap[0], nsub));
-    DECODE_CK(grow(&ws->st[1], &ws->st_cap[1], nsub));
-    DECODE_CK(grow(&ws->base, &ws->base_cap, nsub));
-    DECODE_CK(grow(&ws->coef, &ws->coef_cap, (size_t)coef_blocks * 64));
-    DECODE_CK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
-    if (acr_cap) {
-        DECODE_CK(grow(&ws->acr_mask, &ws->acr_mask_cap, (size_t)acr_cap));
-        DECODE_CK(grow(&ws->acr_rec, &ws->acr_rec_cap, (size_t)acr_cap));
+    DECODE_CK(ws->dev_in.grow(total));
+    DECODE_CK(ws->unst.grow((size_t)unst_total));
+    DECODE_CK(ws->st[0].grow(nsub));
+    DECODE_CK(ws->st[1].grow(nsub));
+    DECODE_CK(ws->base.grow(nsub));
+    DECODE_CK(ws->coef.grow((size_t)coef_blocks * 64));
+    DECODE_CK(ws->planes.grow((size_t)plane_total));
+    if (acr_max) {
+        DECODE_CK(ws->acr_mask.grow((size_t)acr_max));
+        DECODE_CK(ws->acr_rec.grow((size_t)acr_max));
     }
-    DECODE_CK(grow(&ws->small, &ws->small_cap, (size_t)m + max_passes + PASS_GROUP));
-    DECODE_CK(grow_pinned(&ws->small_host, &ws->small_host_cap, (size_t)m + PASS_GROUP));
+    DECODE_CK(ws->small.grow((size_t)m + max_passes + PASS_GROUP));
+    DECODE_CK(ws->small_host.grow((size_t)m + PASS_GROUP));
     const DevImage* d_img = (const DevImage*)(ws->dev_in + o_img);
     const DevScan* d_scan = (const DevScan*)(ws->dev_in + o_scan);
     const DevHuff* d_huff = (const DevHuff*)(ws->dev_in + o_huff);

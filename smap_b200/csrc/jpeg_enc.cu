@@ -627,53 +627,28 @@ std::vector<uint8_t> jpeg_header(int q, int h, int w) {
 }  // namespace
 
 struct JpegEncWorkspace {
-    uint8_t* host = nullptr;  // staging: descriptors and tables
-    size_t host_cap = 0;
-    uint8_t* dev_in = nullptr;
-    size_t dev_in_cap = 0;
-    double* scales_host = nullptr;
-    size_t scales_host_cap = 0;
-    EncTotals* tot = nullptr;
-    size_t tot_cap = 0;
-    EncTotals* tot_host = nullptr;
-    size_t tot_host_cap = 0;
-    uint8_t* planes = nullptr;
-    size_t planes_cap = 0;
-    int* labels = nullptr;
-    size_t labels_cap = 0;
-    int16_t* coef = nullptr;
-    size_t coef_cap = 0;
-    uint32_t* counts = nullptr;  // bits, then 0xFF bytes, per block
-    size_t counts_cap = 0;
-    unsigned long long* off = nullptr;  // [nblk + 1] bit offsets
-    size_t off_cap = 0;
-    unsigned long long* ffoff = nullptr;  // [nblk + 1] 0xFF counts before each block
-    size_t ffoff_cap = 0;
-    unsigned long long* tiles = nullptr;
-    size_t tiles_cap = 0;
-    PanelSeg* segs = nullptr;  // [n][PANEL_ELEMS] (3D panel)
-    size_t segs_cap = 0;
-    uint32_t* words = nullptr;
-    size_t words_cap = 0;
-    uint8_t* out = nullptr;
-    size_t out_cap = 0;
-    uint8_t* result = nullptr;  // pinned: the streams of the last call, back to back
-    size_t result_cap = 0;
+    PinnedBuffer<uint8_t> host;  // staging: descriptors and tables
+    DeviceBuffer<uint8_t> dev_in;
+    PinnedBuffer<double> scales_host;
+    DeviceBuffer<EncTotals> tot;
+    PinnedBuffer<EncTotals> tot_host;
+    DeviceBuffer<uint8_t> planes;
+    DeviceBuffer<int> labels;
+    DeviceBuffer<int16_t> coef;
+    DeviceBuffer<uint32_t> counts;  // bits, then 0xFF bytes, per block
+    DeviceBuffer<unsigned long long> off;  // [nblk + 1] bit offsets
+    DeviceBuffer<unsigned long long> ffoff;  // [nblk + 1] 0xFF counts before each block
+    DeviceBuffer<unsigned long long> tiles;
+    DeviceBuffer<PanelSeg> segs;  // [n][PANEL_ELEMS] (3D panel)
+    DeviceBuffer<uint32_t> words;
+    DeviceBuffer<uint8_t> out;
+    PinnedBuffer<uint8_t> result;  // the streams of the last call, back to back
     std::vector<int64_t> res_off, res_len;
 };
 
 JpegEncWorkspace* jpeg_enc_workspace_create() { return new JpegEncWorkspace(); }
 
-void jpeg_enc_workspace_destroy(JpegEncWorkspace* ws) {
-    if (!ws) return;
-    void* pinned[] = {ws->host, ws->scales_host, ws->tot_host, ws->result};
-    for (void* p : pinned)
-        if (p) cudaFreeHost(p);
-    void* dev[] = {ws->dev_in, ws->tot, ws->planes, ws->labels, ws->coef, ws->counts, ws->off, ws->ffoff, ws->tiles, ws->segs, ws->words, ws->out};
-    for (void* p : dev)
-        if (p) cudaFree(p);
-    delete ws;
-}
+void jpeg_enc_workspace_destroy(JpegEncWorkspace* ws) { delete ws; }
 
 const uint8_t* jpeg_enc_result(const JpegEncWorkspace* ws, int i, int64_t* nbytes) {
     if (!ws || i < 0 || i >= (int)ws->res_off.size()) return nullptr;
@@ -685,7 +660,7 @@ const uint8_t* jpeg_enc_result(const JpegEncWorkspace* ws, int i, int64_t* nbyte
 static int scan_counts(JpegEncWorkspace* ws, const uint32_t* in, long long n, unsigned long long* out, cudaStream_t st,
                        std::string* err) {
     const long long tiles = std::max(1ll, (n + SCAN_TILE - 1) / SCAN_TILE);
-    DECODE_CK(grow(&ws->tiles, &ws->tiles_cap, (size_t)tiles));
+    DECODE_CK(ws->tiles.grow((size_t)tiles));
     scan_reduce_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(in, n, ws->tiles);
     scan_tiles_kernel<<<1, SCAN_THREADS, 0, st>>>(ws->tiles, tiles, out + n);
     scan_apply_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(in, n, ws->tiles, out);
@@ -732,15 +707,10 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
             return -1;
         }
     }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    DECODE_CK(cudaStreamIsCapturing(st, &cap));
-    if (cap != cudaStreamCaptureStatusNone) {
-        *err = "smapb_encode_jpeg: not capturable (it synchronises and may grow its workspace)";
-        return -1;
-    }
+    if (int rc = refuse_capture("smapb_encode_jpeg", st, err)) return rc;
     if (n == 0) return 0;
     if (records) {  // the letterbox of each frame, from its scale row
-        DECODE_CK(grow_pinned(&ws->scales_host, &ws->scales_host_cap, (size_t)n * SMAPB_SCALE_LEN));
+        DECODE_CK(ws->scales_host.grow((size_t)n * SMAPB_SCALE_LEN));
         DECODE_CK(cudaMemcpyAsync(ws->scales_host, scales, sizeof(double) * n * SMAPB_SCALE_LEN, cudaMemcpyDeviceToHost, st));
     }
     DECODE_CK(cudaStreamSynchronize(st));  // the scales, and the workspace the previous call may still use
@@ -792,24 +762,24 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
     }
     const size_t o_tab = align_up(sizeof(EncImg) * n, 256), o_pan = align_up(o_tab + sizeof(EncTables), 256);
     const size_t total_in = o_pan + sizeof(PanelImg) * panels.size();
-    DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total_in));
+    DECODE_CK(ws->host.grow(total_in));
     memcpy(ws->host, imgs.data(), sizeof(EncImg) * n);
     memcpy(ws->host + o_tab, &T, sizeof(T));
     if (view3d) {
         memcpy(ws->host + o_pan, panels.data(), sizeof(PanelImg) * n);
-        DECODE_CK(grow(&ws->segs, &ws->segs_cap, (size_t)n * PANEL_ELEMS));
+        DECODE_CK(ws->segs.grow((size_t)n * PANEL_ELEMS));
     }
-    DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total_in));
-    DECODE_CK(grow(&ws->planes, &ws->planes_cap, (size_t)plane_total));
-    DECODE_CK(grow(&ws->coef, &ws->coef_cap, (size_t)nblk * 64));
-    DECODE_CK(grow(&ws->counts, &ws->counts_cap, (size_t)nblk));
-    DECODE_CK(grow(&ws->off, &ws->off_cap, (size_t)nblk + 1));
-    DECODE_CK(grow(&ws->ffoff, &ws->ffoff_cap, (size_t)nblk + 1));
-    DECODE_CK(grow(&ws->words, &ws->words_cap, (size_t)word_total));
-    DECODE_CK(grow(&ws->tot, &ws->tot_cap, (size_t)n));
-    DECODE_CK(grow_pinned(&ws->tot_host, &ws->tot_host_cap, (size_t)n));
-    if (label_total) DECODE_CK(grow(&ws->labels, &ws->labels_cap, (size_t)label_total));
-    const EncImg* d_img = (const EncImg*)ws->dev_in;
+    DECODE_CK(ws->dev_in.grow(total_in));
+    DECODE_CK(ws->planes.grow((size_t)plane_total));
+    DECODE_CK(ws->coef.grow((size_t)nblk * 64));
+    DECODE_CK(ws->counts.grow((size_t)nblk));
+    DECODE_CK(ws->off.grow((size_t)nblk + 1));
+    DECODE_CK(ws->ffoff.grow((size_t)nblk + 1));
+    DECODE_CK(ws->words.grow((size_t)word_total));
+    DECODE_CK(ws->tot.grow((size_t)n));
+    DECODE_CK(ws->tot_host.grow((size_t)n));
+    if (label_total) DECODE_CK(ws->labels.grow((size_t)label_total));
+    const EncImg* d_img = (const EncImg*)ws->dev_in.get();
     const EncTables* d_tab = (const EncTables*)(ws->dev_in + o_tab);
     DECODE_CK(cudaMemcpyAsync(ws->dev_in, ws->host, total_in, cudaMemcpyHostToDevice, st));
     int max_mcus = 0;
@@ -851,8 +821,8 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         }
         total_out = t.out0 + t.stuffed + 2;
     }
-    DECODE_CK(grow(&ws->out, &ws->out_cap, (size_t)total_out));
-    DECODE_CK(grow_pinned(&ws->result, &ws->result_cap, (size_t)total_out));
+    DECODE_CK(ws->out.grow((size_t)total_out));
+    DECODE_CK(ws->result.grow((size_t)total_out));
     scatter_kernel<<<bgrid, 256, 0, st>>>(d_img, n, nblk, ws->off, ws->ffoff, ws->words, ws->tot, ws->out);
     DECODE_CK(cudaGetLastError());
     ++*launches;

@@ -476,10 +476,7 @@ int upload_conv_layer(smapb_handle* h, ConvLayer& L, int taps, const std::vector
             }
     std::vector<float> bias(L.Cout_pad, 0.f);
     for (int co = 0; co < L.Cout; co++) bias[co] = bf[co];
-    if (!L.w_dev) {
-        if (dev_alloc(h, &L.w_dev, host.size())) return -10;
-        if (dev_alloc(h, &L.bias_dev, bias.size())) return -10;
-    }
+    if (dev_alloc(h, L.w_dev, host.size()) || dev_alloc(h, L.bias_dev, bias.size())) return -10;
     CK(cudaMemcpy(L.w_dev, host.data(), host.size() * 2, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(L.bias_dev, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice));
     return 0;
@@ -524,13 +521,13 @@ struct PlanBuilder {
     }
 
     void* alloc(size_t bytes, const char* what) {
-        void* p = nullptr;
-        if (cudaMalloc(&p, bytes) != cudaSuccess) {
+        DeviceBuffer<uint8_t> b;
+        if (b.grow(bytes) != cudaSuccess) {
             rc = fail(h, -10, std::string("cudaMalloc failed for ") + what);
             return nullptr;
         }
-        plan->allocs.push_back(p);
-        return p;
+        plan->allocs.push_back(std::move(b));
+        return plan->allocs.back().get();
     }
     Act new_act(int N, int H, int W, int C) {
         Act a;
@@ -632,26 +629,6 @@ std::string debug_op_desc(const smapb_handle* h, const Op& op, const std::map<co
 
 namespace smapb {
 
-void free_plan(Plan* plan) {
-    for (void* p : plan->allocs) cudaFree(p);
-    for (Op& op : plan->ops)
-        if (op.ev) cudaEventDestroy(op.ev);
-    plan->allocs.clear();
-    plan->ops.clear();
-}
-
-void free_layers(smapb_handle* h) {
-    for (auto& kv : h->layers) {
-        cudaFree(kv.second.w_dev);
-        cudaFree(kv.second.bias_dev);
-    }
-    h->layers.clear();
-    cudaFree(h->stem_tc.w_dev);
-    cudaFree(h->stem_tc.bias_dev);
-    h->stem_tc.w_dev = nullptr;
-    h->stem_tc.bias_dev = nullptr;
-}
-
 int build_plan(smapb_handle* h, int B, Plan** out_plan) {
     auto it = h->plans.find(B);
     if (it != h->plans.end()) {
@@ -671,10 +648,7 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan) {
         bool tc = h->stem_tc_ok != 0 && !(getenv("SMAPB_STEM") && !strcmp(getenv("SMAPB_STEM"), "cuda"));
         if (tc) {
             const Act s2d = pb.new_act(B, H / 2, W / 2 + 3, 16);  // storage [plane][B][H/2][W/2+3][16]
-            if (pb.rc) {
-                free_plan(plan.get());
-                return pb.rc;
-            }
+            if (pb.rc) return pb.rc;
             Op oc;
             oc.kind = OP_CONV;
             int rc2 = setup_stem_conv(h, s2d.ptr, s2d.plane(), B, H / 2, W / 2, stem, &oc.cp, &oc.block_n, &oc.flops);
@@ -795,10 +769,7 @@ int build_plan(smapb_handle* h, int B, Plan** out_plan) {
         }
         x = cross;
     }
-    if (pb.rc) {
-        free_plan(plan.get());
-        return pb.rc;
-    }
+    if (pb.rc) return pb.rc;
     {
         Op op;
         op.kind = OP_HEADMERGE;
@@ -920,9 +891,9 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
     h->eager_runs.clear();
     if (new_planes != h->planes || !h->plans.empty()) {
         cudaDeviceSynchronize();
-        for (auto& kv : h->plans) free_plan(kv.second.get());
         h->plans.clear();
-        free_layers(h);
+        h->layers.clear();
+        h->stem_tc = ConvLayer();
     }
     set_precision(h, precision);
     // unit names: every "<name>.conv.weight" key
@@ -935,7 +906,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
     }
     if (units.empty()) return fail(h, -40, "no weights loaded");
     struct Folded {
-        ConvLayer L;  // the unit's geometry
+        ConvGeom L;
         std::vector<float> w, b;
     };
     std::map<std::string, Folded> folded;  // units the loops below build other layers from
@@ -956,10 +927,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
                     for (int ky = 0; ky < 7; ky++)
                         for (int kx = 0; kx < 7; kx++)
                             w2[((ky * 7 + kx) * 3 + ci) * 64 + co] = wf[((co * 3 + ci) * 7 + ky) * 7 + kx];
-            if (!h->stem_w) {
-                if (dev_alloc(h, &h->stem_w, w2.size())) return -10;
-                if (dev_alloc(h, &h->stem_b, 64)) return -10;
-            }
+            if (dev_alloc(h, h->stem_w, w2.size()) || dev_alloc(h, h->stem_b, 64)) return -10;
             CK(cudaMemcpy(h->stem_w, w2.data(), w2.size() * 4, cudaMemcpyHostToDevice));
             CK(cudaMemcpy(h->stem_b, bf.data(), 64 * 4, cudaMemcpyHostToDevice));
             // tensor-core stem: 4 taps (ky-blocks ay) of 64 k = ax*16 + (by*2+bx)*3 + c; ky = 2*ay+by-1, kx = 2*ax+bx-1
@@ -1023,8 +991,8 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
         const std::string base = n3.substr(0, pos), nds = base + ".0.downsample";
         auto ids = folded.find(nds);
         if (ids == folded.end()) return fail(h, -40, "missing downsample unit for " + n3);
-        const ConvLayer& L3 = kv.second.L;
-        const ConvLayer& Lds = ids->second.L;
+        const ConvGeom& L3 = kv.second.L;
+        const ConvGeom& Lds = ids->second.L;
         ConvLayer& F = h->layers[base + ".0.fused_conv3_downsample"];
         F.name = base + ".0.fused_conv3_downsample";
         F.Cin = L3.Cin;
@@ -1047,7 +1015,7 @@ int smapb_finalize_weights(smapb_handle* h, int precision) {
     for (auto& kv : folded) {
         const std::string& nm = kv.first;
         if (nm.find("res_d_conv2") == std::string::npos && nm.find("res_rd_conv2") == std::string::npos) continue;
-        const ConvLayer& L0 = kv.second.L;
+        const ConvGeom& L0 = kv.second.L;
         if (L0.k != 3) continue;
         ConvLayer& E = h->layers[nm + ".tapexp"];
         E.name = nm + ".tapexp";
@@ -1138,18 +1106,16 @@ int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int 
     int rc = build_plan(h, B, &plan);
     if (rc) return rc;
     CK(cudaDeviceSynchronize());
-    unsigned long long* d = nullptr;
-    CK(cudaMalloc((void**)&d, 8));
+    DeviceBuffer<unsigned long long> d;
+    CK(d.grow(1));
     std::map<const void*, int> dump_idx;  // output tensor -> dump index (the numbering of smapb_debug_dump)
     int n_dumped = 0;
     for (const Op& op : plan->ops) {
         long long bytes = 0;
         const void* out = dumped_output(h, op, &bytes);
         if (!out) continue;
-        if (!dump_idx.emplace(out, n_dumped++).second) {
-            cudaFree(d);
+        if (!dump_idx.emplace(out, n_dumped++).second)
             return fail(h, -2, "smapb_debug_checksums: two ops share an output tensor (" + op.name + ")");
-        }
     }
     int n = 0;
     for (const Op& op : plan->ops) {
@@ -1164,7 +1130,6 @@ int smapb_debug_checksums(smapb_handle* h, int B, unsigned long long* sums, int 
         if (desc) snprintf(desc + (size_t)n * desc_stride, desc_stride, "%s", debug_op_desc(h, op, dump_idx).c_str());
         n++;
     }
-    cudaFree(d);
     return n;
 }
 
@@ -1209,8 +1174,12 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
     if (in2_src && (stride2 < 1 || H2 < 1 || W2 < 1 || (H2 - 1) / stride2 + 1 != Ho || (W2 - 1) / stride2 + 1 != Wo))
         return fail(h, -1, "smapb_conv_test: in2 does not give the output geometry under stride2");
-    const int save_terms = h->nterms, save_planes = h->planes;
-    const bool save_f16 = h->f16;
+    struct RestorePrecision {  // the handle's precision, put back on every return
+        smapb_handle* h;
+        int nterms, planes;
+        bool f16;
+        ~RestorePrecision() { h->nterms = nterms, h->planes = planes, h->f16 = f16; }
+    } restore{h, h->nterms, h->planes, h->f16};
     set_precision(h, precision);
     int rc = 0;
     ConvLayer L;
@@ -1218,30 +1187,10 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     L.Cin = Cin, L.Cout = Cout, L.Cout_pad = pad32(Cout), L.k = k, L.stride = stride, L.pad = pad;
     L.Cin2 = Cin2, L.stride2 = stride2;
     std::vector<float> wh((size_t)Cout * (Cin + Cin2) * k * k), bh(Cout);
-    std::vector<void*> tmp;
-    auto cleanup = [&]() {
-        for (void* p : tmp) cudaFree(p);
-        cudaFree(L.w_dev);
-        cudaFree(L.bias_dev);
-        h->nterms = save_terms;
-        h->planes = save_planes;
-        h->f16 = save_f16;
-    };
-#define CKT(call)                                                                         \
-    do {                                                                                  \
-        cudaError_t e_ = (call);                                                          \
-        if (e_ != cudaSuccess) {                                                          \
-            cleanup();                                                                    \
-            return fail(h, -10, std::string(#call) + ": " + cudaGetErrorString(e_));      \
-        }                                                                                 \
-    } while (0)
-    CKT(cudaMemcpy(wh.data(), w, wh.size() * 4, cudaMemcpyDeviceToHost));
-    CKT(cudaMemcpy(bh.data(), bias, bh.size() * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(wh.data(), w, wh.size() * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(bh.data(), bias, bh.size() * 4, cudaMemcpyDeviceToHost));
     rc = upload_conv_layer(h, L, k * k, wh, bh);
-    if (rc) {
-        cleanup();
-        return rc;
-    }
+    if (rc) return rc;
     Act in, out, in2, up;
     ActF32 out32;
     in.N = B, in.H = H, in.W = W, in.C = Cin;
@@ -1250,33 +1199,31 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     up.N = B, up.H = Ho / 2, up.W = Wo / 2, up.C = Cout;
     out32.N = B, out32.H = Ho, out32.W = Wo, out32.C = L.Cout_pad;
     ConvIO io{&in, relu};
-    void* p = nullptr;
+    DeviceBuffer<__nv_bfloat16> in_buf, in2_buf, out_buf, extra_buf[4];
+    DeviceBuffer<float> y32;  // the fp32 output: the conv's own (out_f32), or its split output converted
     // the operands in the precision's activation planes, converted as the plan converts fp32 tensors (an empty tensor,
     // an in2 with Cin2 = 0 or an up of a 1-pixel output, is left unallocated: setup_conv refuses it)
-    auto planes_of = [&](const float* src, Act& a) -> cudaError_t {
+    auto planes_of = [&](const float* src, Act& a, DeviceBuffer<__nv_bfloat16>& buf) -> cudaError_t {
         if (a.plane() == 0) return cudaSuccess;
-        cudaError_t e = cudaMalloc(&p, (size_t)a.plane() * 2 * h->planes);
+        cudaError_t e = buf.grow((size_t)a.plane() * h->planes);
         if (e != cudaSuccess) return e;
-        tmp.push_back(p);
-        a.ptr = (__nv_bfloat16*)p;
+        a.ptr = buf;
         return launch_f32_to_split(src, a.ptr, a.plane(), a.plane(), h->planes, st, h->f16);
     };
-    CKT(planes_of(x, in));
+    CK(planes_of(x, in, in_buf));
     if (out_f32) {
-        CKT(cudaMalloc(&p, (size_t)out.plane() * 4));
-        tmp.push_back(p);
-        out32.ptr = (float*)p;
-        CKT(cudaMemset(p, 0, (size_t)out.plane() * 4));
+        CK(y32.grow((size_t)out.plane()));
+        out32.ptr = y32;
+        CK(cudaMemset(y32, 0, (size_t)out.plane() * 4));
         io.out_f32 = &out32;
     } else {
-        CKT(cudaMalloc(&p, (size_t)out.plane() * 2 * h->planes));
-        tmp.push_back(p);
-        out.ptr = (__nv_bfloat16*)p;
-        CKT(cudaMemset(p, 0, (size_t)out.plane() * 2 * h->planes));  // TMA stores are invisible to initcheck
+        CK(out_buf.grow((size_t)out.plane() * h->planes));
+        out.ptr = out_buf;
+        CK(cudaMemset(out_buf, 0, (size_t)out.plane() * 2 * h->planes));  // TMA stores are invisible to initcheck
         io.out = &out;
     }
     if (in2_src) {
-        CKT(planes_of(in2_src, in2));
+        CK(planes_of(in2_src, in2, in2_buf));
         io.in2 = &in2;
     }
     const float* extra_src[4] = {res, post1, post2, up_src};
@@ -1284,21 +1231,15 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     const Act** extra_role[4] = {&io.res, &io.post1, &io.post2, &io.up};
     for (int e = 0; e < 4; e++) {
         if (!extra_src[e]) continue;
-        if (L.Cout_pad != Cout) {
-            cleanup();
-            return fail(h, -1, "conv_test: residual/post/up operands require Cout % 32 == 0");
-        }
-        CKT(planes_of(extra_src[e], extra_act[e]));
+        if (L.Cout_pad != Cout) return fail(h, -1, "conv_test: residual/post/up operands require Cout % 32 == 0");
+        CK(planes_of(extra_src[e], extra_act[e], extra_buf[e]));
         *extra_role[e] = &extra_act[e];
     }
     ConvParams cp;
     int bn = 0;
     rc = choose_tile(h, L, io, false, &bn);
     if (!rc) rc = setup_conv(h, L, io, bn, &cp);
-    if (rc) {
-        cleanup();
-        return rc;
-    }
+    if (rc) return rc;
     if (launch) {
         launch[0] = bn;
         launch[1] = 1 << cp.tw_log2;
@@ -1308,23 +1249,18 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
-    long long* dbg_dev = nullptr;
+    DeviceBuffer<long long> dbg_dev, tl_dev;
     if (getenv("SMAPB_ROLES")) {
-        CKT(cudaMalloc((void**)&dbg_dev, 16 * sizeof(long long)));
-        tmp.push_back(dbg_dev);
-        CKT(cudaMemset(dbg_dev, 0, 16 * sizeof(long long)));
+        CK(dbg_dev.grow(16));
+        CK(cudaMemset(dbg_dev, 0, 16 * sizeof(long long)));
         cp.dbg = dbg_dev;
     }
-    long long* tl_dev = nullptr;
-    if (getenv("SMAPB_TIMELINE")) {
-        CKT(cudaMalloc((void**)&tl_dev, 16 * sizeof(long long)));
-        tmp.push_back(tl_dev);
-    }
-    CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));  // warm-up + result
+    if (getenv("SMAPB_TIMELINE")) CK(tl_dev.grow(16));
+    CK(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));  // warm-up + result
     cp.sat = nullptr;  // the saturation counter counts the result launch; the time-line and timed re-runs leave it alone
     if (dbg_dev) {
         long long d[16];
-        CKT(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(d, dbg_dev, sizeof d, cudaMemcpyDeviceToHost));
         const double n = d[ConvDbg::CTAS] > 0 ? (double)d[ConvDbg::CTAS] : 1.0;
         fprintf(stderr, "[roles] bn%d units%d kb%d | mean cycles per CTA: total %.0f | producer wait-empty %.0f", bn,
                 cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, d[ConvDbg::TOTAL] / n,
@@ -1339,33 +1275,31 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
         cp.dbg = nullptr;
     }
     if (tl_dev) {  // time line of CTA 0 of one warm launch (cycles since kernel entry)
-        CKT(cudaMemset(tl_dev, 0, 16 * sizeof(long long)));
+        CK(cudaMemset(tl_dev, 0, 16 * sizeof(long long)));
         cp.dbg_tl = tl_dev;
-        CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
+        CK(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
         cp.dbg_tl = nullptr;
         long long t[16];
-        CKT(cudaMemcpy(t, tl_dev, sizeof t, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(t, tl_dev, sizeof t, cudaMemcpyDeviceToHost));
         fprintf(stderr, "[timeline] bn%d units%d kb%d | set-up %lld | first operands %lld | last main loop end %lld | epilogue done "
                 "%lld | exit %lld\n", bn, cp.total_tiles, cp.kh * cp.kw * cp.kchunks + cp.kchunks2, t[1] - t[0], t[2] - t[0],
                 t[3] - t[0], t[13] - t[0], t[15] - t[0]);
     }
     const int reps = ms_out ? 5 : 0;
     cudaEventRecord(e0, st);
-    for (int i = 0; i < reps; i++) CKT(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
+    for (int i = 0; i < reps; i++) CK(launch_conv(cp, bn, h->nterms, h->f16, h->sm_count, st));
     cudaEventRecord(e1, st);
     h->launches += 1 + reps;
     // convert (split outputs) + de-pad
-    float* ytmp = out32.ptr;
     if (!out_f32) {
-        CKT(cudaMalloc((void**)&ytmp, (size_t)out.plane() * 4));
-        tmp.push_back(ytmp);
-        split_to_f32_kernel<<<(unsigned)((out.plane() + 255) / 256), 256, 0, st>>>(out.ptr, out.plane(), h->planes, ytmp,
+        CK(y32.grow((size_t)out.plane()));
+        split_to_f32_kernel<<<(unsigned)((out.plane() + 255) / 256), 256, 0, st>>>(out.ptr, out.plane(), h->planes, y32,
                                                                                    out.plane(), h->f16);
-        CKT(cudaGetLastError());
+        CK(cudaGetLastError());
     }
-    CKT(cudaMemcpy2DAsync(y, (size_t)Cout * 4, ytmp, (size_t)L.Cout_pad * 4, (size_t)Cout * 4, (size_t)B * Ho * Wo,
+    CK(cudaMemcpy2DAsync(y, (size_t)Cout * 4, y32, (size_t)L.Cout_pad * 4, (size_t)Cout * 4, (size_t)B * Ho * Wo,
                           cudaMemcpyDeviceToDevice, st));
-    CKT(cudaStreamSynchronize(st));
+    CK(cudaStreamSynchronize(st));
     if (ms_out) {
         float ms = 0;
         cudaEventElapsedTime(&ms, e0, e1);
@@ -1373,9 +1307,7 @@ int smapb_conv_test(smapb_handle* h, const float* x, const float* w, const float
     }
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
-    cleanup();
     return 0;
-#undef CKT
 }
 
 #pragma GCC visibility pop

@@ -846,36 +846,25 @@ __global__ void __launch_bounds__(256) colour_kernel(const DevPng* __restrict__ 
 }  // namespace
 
 // staging: descriptors and IDAT regions; small: stats[4] | status[m] | nblk[m] | adler[m]
-struct PngWorkspace : DecodeBuffers {
-    uint8_t* stream = nullptr;
-    size_t stream_cap = 0;
-    unsigned long long* cand = nullptr;
-    size_t cand_cap = 0;
-    CountResult* res = nullptr;
-    size_t res_cap = 0;
-    unsigned long long* hkey = nullptr;
-    size_t hkey_cap = 0;
-    int* hval = nullptr;
-    size_t hval_cap = 0;
-    DevBlock* blocks = nullptr;
-    size_t blocks_cap = 0;
-    uint16_t* marks = nullptr;
-    size_t marks_cap = 0;
-    uint8_t* raw = nullptr;
-    size_t raw_cap = 0;
+struct PngWorkspace {
+    PinnedBuffer<uint8_t> host;
+    DeviceBuffer<uint8_t> dev_in;
+    DeviceBuffer<int> small;
+    PinnedBuffer<int> small_host;
+    DeviceBuffer<uint8_t> stream;
+    DeviceBuffer<unsigned long long> cand;
+    DeviceBuffer<CountResult> res;
+    DeviceBuffer<unsigned long long> hkey;
+    DeviceBuffer<int> hval;
+    DeviceBuffer<DevBlock> blocks;
+    DeviceBuffer<uint16_t> marks;
+    DeviceBuffer<uint8_t> raw;
     int64_t stats[4] = {0, 0, 0, 0};
 };
 
 PngWorkspace* png_workspace_create() { return new PngWorkspace(); }
 
-void png_workspace_destroy(PngWorkspace* ws) {
-    if (!ws) return;
-    free_decode_buffers(ws);
-    void* d[] = {ws->stream, ws->cand, ws->res, ws->hkey, ws->hval, ws->blocks, ws->marks, ws->raw};
-    for (void* p : d)
-        if (p) cudaFree(p);
-    delete ws;
-}
+void png_workspace_destroy(PngWorkspace* ws) { delete ws; }
 
 void png_last_stats(const PngWorkspace* ws, int64_t out[4]) {
     for (int i = 0; i < 4; i++) out[i] = ws ? ws->stats[i] : 0;
@@ -946,23 +935,23 @@ int png_decode(PngWorkspace* ws, int n, const uint8_t* const* png, const int64_t
     // staging layout: images | chunks | IDAT regions
     const size_t o_img = 0, o_chunk = align_up(sizeof(DevPng) * m, 256), o_in = align_up(o_chunk + sizeof(DevChunk) * chunks.size(), 256),
                  total = o_in + in_total;
-    DECODE_CK(grow_pinned(&ws->host, &ws->host_cap, total));
+    DECODE_CK(ws->host.grow(total));
     DECODE_CK(cudaStreamSynchronize(st));  // the staging area and the workspace may still be in use by the previous call
     memcpy(ws->host + o_img, imgs.data(), sizeof(DevPng) * m);
     memcpy(ws->host + o_chunk, chunks.data(), sizeof(DevChunk) * chunks.size());
     for (int k = 0; k < m; k++) memcpy(ws->host + o_in + in_off[k], png[idx[k]] + H[idx[k]].idat.front(), in_len[k]);
     const size_t nsmall = 4 + 3 * (size_t)m;
-    DECODE_CK(grow(&ws->dev_in, &ws->dev_in_cap, total));
-    DECODE_CK(grow(&ws->stream, &ws->stream_cap, (size_t)z_total));
-    DECODE_CK(grow(&ws->cand, &ws->cand_cap, (size_t)cand_cap));
-    DECODE_CK(grow(&ws->res, &ws->res_cap, (size_t)cand_cap));
-    DECODE_CK(grow(&ws->hkey, &ws->hkey_cap, (size_t)hsize));
-    DECODE_CK(grow(&ws->hval, &ws->hval_cap, (size_t)hsize));
-    DECODE_CK(grow(&ws->blocks, &ws->blocks_cap, (size_t)blk_total));
-    DECODE_CK(grow(&ws->marks, &ws->marks_cap, (size_t)raw_total));
-    DECODE_CK(grow(&ws->raw, &ws->raw_cap, (size_t)raw_total));
-    DECODE_CK(grow(&ws->small, &ws->small_cap, nsmall));
-    DECODE_CK(grow_pinned(&ws->small_host, &ws->small_host_cap, nsmall));
+    DECODE_CK(ws->dev_in.grow(total));
+    DECODE_CK(ws->stream.grow((size_t)z_total));
+    DECODE_CK(ws->cand.grow((size_t)cand_cap));
+    DECODE_CK(ws->res.grow((size_t)cand_cap));
+    DECODE_CK(ws->hkey.grow((size_t)hsize));
+    DECODE_CK(ws->hval.grow((size_t)hsize));
+    DECODE_CK(ws->blocks.grow((size_t)blk_total));
+    DECODE_CK(ws->marks.grow((size_t)raw_total));
+    DECODE_CK(ws->raw.grow((size_t)raw_total));
+    DECODE_CK(ws->small.grow(nsmall));
+    DECODE_CK(ws->small_host.grow(nsmall));
     const DevPng* d_img = (const DevPng*)(ws->dev_in + o_img);
     const DevChunk* d_chunk = (const DevChunk*)(ws->dev_in + o_chunk);
     const uint8_t* d_in = ws->dev_in + o_in;
