@@ -271,6 +271,31 @@ int smapb_encode_jpeg_ex(smapb_handle* h, int n, const uint8_t* const* bgr_dev, 
 /* Stream i of the last smapb_encode_jpeg(_ex): *data = its first byte, *nbytes (may be NULL) its size.  -1 for i out of range. */
 int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes);
 
+/* Encodes n uint8 BGR frames into the bytes cv2.imencode(".png", frame) writes (libpng 1.6 with zlib 1.2.11, no
+ * parameters), lossless.  Frames, records_dev, scales_dev and flags (0 or SMAPB_ENCODE_VIEW3D) are as for
+ * smapb_encode_jpeg_ex, side limits included: the file shows exactly the composite that call encodes.  The file:
+ *   1. the signature, then IHDR (W, H, bit depth 8, colour type 2, compression, filter and interlace 0), no other
+ *      ancillary chunk;
+ *   2. scanlines in RGB order, each a filter byte 1 (Sub) and x[i] - x[i-3] mod 256 (the first pixel minus 0); when
+ *      W = 1 every row is filter byte 0 (None) and the pixels as they are;
+ *   3. the n = H (1 + 3 W) scanline bytes deflated as zlib's deflateInit2(level 1, Z_DEFLATED, wbits, memLevel 8, Z_RLE)
+ *      does over the whole stream: wbits = 15 except when n <= 16384, where half = 16384 is halved and wbits decremented
+ *      while n + 262 <= half; blocks of 16383 symbols, the last one empty when the symbol count is a multiple of 16383,
+ *      each stored, fixed or dynamic as zlib's _tr_flush_block chooses (stored only while the block's bytes are in the
+ *      window); then the Adler-32;
+ *   4. when n <= 16384, libpng's rewrite of the zlib header: cinfo = CMF >> 4 and half = 1 << (cinfo + 7); if n <= half,
+ *      half is halved and cinfo decremented while cinfo > 0 and n <= half; FLG's check bits are recomputed;
+ *   5. the zlib stream cut into IDAT chunks of exactly 8192 bytes and a shorter last one, each with its CRC-32; IEND.
+ * nbytes_host[i] receives each file's size; smapb_encoded_png gives its bytes, in a pinned buffer the handle owns, valid
+ * until the next smapb_encode_png on the handle that is not refused.  Each phase is one launch for the whole batch,
+ * whatever the frames' sizes and content; the workspace grows on demand; the call synchronises `stream`, so it cannot be
+ * captured into a CUDA graph.  -1 for bad arguments (a frame's sides, a scale row that does not describe its frame: the
+ * frame named), and a refused call changes no state of the handle (smapb_last_error aside). */
+int smapb_encode_png(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w,
+                     const smapb_record* records_dev, const double* scales_dev, int flags, int64_t* nbytes_host, void* stream);
+/* File i of the last smapb_encode_png: *data = its first byte, *nbytes (may be NULL) its size.  -1 for i out of range. */
+int smapb_encoded_png(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes);
+
 /* ---- multi-GPU: frames are sharded over ranks, ONE exchange step per batch --------------------------------------- */
 /* The reference's inference path is single-GPU (exps/stage3_root2/test.py:198 calls get_test_loader with num_gpu=1);
  * its data loader's rank split (lib/utils/dataloader.py:80-85: contiguous blocks of frames per rank) is the sharding

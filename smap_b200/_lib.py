@@ -22,7 +22,7 @@ EXPORTS = [
     "smapb_infer_device_gather", "smapb_submit_host_gather", "smapb_set_tile_table", "smapb_get_tile_table",
     "smapb_lift3d_gt", "smapb_infer_device_gather_async", "smapb_gather_sync", "smapb_saturation_count",
     "smapb_jpeg_info", "smapb_decode_jpeg", "smapb_jpeg_info_ex", "smapb_decode_jpeg_ex", "smapb_png_info", "smapb_decode_png",
-    "smapb_encode_jpeg", "smapb_encoded_jpeg", "smapb_encode_jpeg_ex",
+    "smapb_encode_jpeg", "smapb_encoded_jpeg", "smapb_encode_jpeg_ex", "smapb_encode_png", "smapb_encoded_png",
 ]
 
 _lib = None
@@ -97,6 +97,8 @@ def load():
     lib.smapb_encode_jpeg_ex.argtypes = [vp, i32, c.POINTER(vp), c.POINTER(i32), c.POINTER(i32), i32, vp, vp, i32, c.POINTER(i64),
                                          vp]
     lib.smapb_encoded_jpeg.argtypes = [vp, i32, c.POINTER(c.POINTER(c.c_uint8)), c.POINTER(i64)]
+    lib.smapb_encode_png.argtypes = [vp, i32, c.POINTER(vp), c.POINTER(i32), c.POINTER(i32), vp, vp, i32, c.POINTER(i64), vp]
+    lib.smapb_encoded_png.argtypes = [vp, i32, c.POINTER(c.POINTER(c.c_uint8)), c.POINTER(i64)]
     lib.smapb_png_inflate_stats.argtypes = [vp, c.POINTER(i64)]  # include/smap_b200_debug.h
     lib.smapb_set_tile_table.argtypes = [c.c_char_p]
     lib.smapb_get_tile_table.argtypes = [c.c_char_p, i32]

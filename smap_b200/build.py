@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsmap_b200.so")
-SOURCES = ["engine.cu", "plan.cu", "assoc.cu", "elementwise.cu", "refine.cu", "preprocess.cu", "jpeg.cu", "png.cu", "jpeg_enc.cu", "view3d.cu", "json_out.cpp"]
+SOURCES = ["engine.cu", "plan.cu", "assoc.cu", "elementwise.cu", "refine.cu", "preprocess.cu", "jpeg.cu", "png.cu", "jpeg_enc.cu", "png_enc.cu", "overlay.cu", "view3d.cu", "json_out.cpp"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 

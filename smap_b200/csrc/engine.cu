@@ -414,6 +414,21 @@ int smapb_encoded_jpeg(const smapb_handle* h, int i, const uint8_t** data, int64
     return *data ? 0 : -1;
 }
 
+int smapb_encode_png(smapb_handle* h, int n, const uint8_t* const* bgr_dev, const int* img_h, const int* img_w,
+                     const smapb_record* records_dev, const double* scales_dev, int flags, int64_t* nbytes_host, void* stream) {
+    if (!h) return -1;
+    cudaSetDevice(h->device);
+    if (!h->png_enc) h->png_enc.reset(smapb::png_enc_workspace_create());
+    return smapb::png_encode(h->png_enc.get(), n, bgr_dev, img_h, img_w, records_dev, scales_dev, flags, nbytes_host,
+                             (cudaStream_t)stream, &h->launches, &h->err);
+}
+
+int smapb_encoded_png(const smapb_handle* h, int i, const uint8_t** data, int64_t* nbytes) {
+    if (!h || !data) return -1;
+    *data = smapb::png_enc_result(h->png_enc.get(), i, nbytes);
+    return *data ? 0 : -1;
+}
+
 int smapb_png_inflate_stats(const smapb_handle* h, int64_t* counts4) {
     if (!h || !counts4) return -1;
     smapb::png_last_stats(h->png.get(), counts4);

@@ -17,6 +17,7 @@
 #include "decode_host.h"
 #include "jpeg.h"
 #include "jpeg_enc.h"
+#include "png_enc.h"
 #include "png.h"
 #include "preprocess.h"
 #include "refine.h"
@@ -173,12 +174,13 @@ struct smapb_handle {
     };
     std::map<std::pair<int, int>, PreEntry> pre_cache;
     smapb::DeviceBuffer<uint8_t> pre_stage;
-    // JPEG decoding (smapb_decode_jpeg), PNG decoding (smapb_decode_png) and JPEG encoding (smapb_encode_jpeg), created on
-    // first use
+    // JPEG decoding (smapb_decode_jpeg), PNG decoding (smapb_decode_png), JPEG encoding (smapb_encode_jpeg) and PNG
+    // encoding (smapb_encode_png), created on first use
     std::unique_ptr<smapb::JpegWorkspace, void (*)(smapb::JpegWorkspace*)> jpeg{nullptr, smapb::jpeg_workspace_destroy};
     std::unique_ptr<smapb::PngWorkspace, void (*)(smapb::PngWorkspace*)> png{nullptr, smapb::png_workspace_destroy};
     std::unique_ptr<smapb::JpegEncWorkspace, void (*)(smapb::JpegEncWorkspace*)> jpeg_enc{nullptr,
                                                                                           smapb::jpeg_enc_workspace_destroy};
+    std::unique_ptr<smapb::PngEncWorkspace, void (*)(smapb::PngEncWorkspace*)> png_enc{nullptr, smapb::png_enc_workspace_destroy};
     // RefineNet (optional post-processing step, SURVEY 8(f) f2)
     std::map<std::string, std::vector<float>> refine_raw;
     smapb::DeviceBuffer<float> refine_buf;  // folded, transposed weights + biases of the five layers

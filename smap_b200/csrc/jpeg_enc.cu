@@ -2,8 +2,7 @@
 // defaults: 4:2:0, standard Huffman tables, no restart interval), restated on the CPU by oracle/jpeg_encode_numpy.py.
 //
 // One launch per phase for the whole batch (frames of any sizes):
-//   overlay   (records only) one CTA per skeleton element walks a band around it and atomicMax-es its paint rank into
-//             a per-pixel label plane, so the painter's order comes out whatever order the elements run in;
+//   overlay   (records only) the composite stage's label planes (overlay.cu, view3d.cu);
 //   colour    one thread per chroma sample: its 2x2 pixels (labelled ones replaced by their element's colour), fixed-point
 //             RGB -> YCbCr, the four luma samples and the biased 2x2 chroma means, edge-replicated to the MCU grid;
 //   fdct      one thread per block: level shift, accurate-integer FDCT, quantisation, zigzag int16 coefficients; luma
@@ -25,24 +24,14 @@
 
 #include "decode_host.h"
 #include "jpeg_enc.h"
-#include "paint.cuh"
-#include "preprocess.h"
-#include "view3d.h"
+#include "overlay.cuh"
+#include "scan.cuh"
 
 namespace smapb {
 
 namespace {
 
-constexpr int NELEM = SMAPB_NL + SMAPB_NJ;  // 14 limbs then 15 joints per person: paint rank person * 29 + element + 1
 constexpr int BLOCK_BITS_MAX = 22 + 63 * 26;  // the longest DC token + 63 tokens of run 0 / size 10 (jpeg_encode_numpy)
-constexpr int SCAN_THREADS = 1024, SCAN_ITEMS = 4, SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
-
-// BGR limb colours per person (cycling), and the joint colour (include/smap_b200.h, smapb_encode_jpeg)
-__constant__ uint8_t kPalette[6][3] = {{0, 0, 255}, {0, 255, 0}, {255, 0, 0}, {0, 255, 255}, {0, 0, 0}, {255, 0, 255}};
-__constant__ uint8_t kJoint[3] = {255, 255, 255};
-// the 3D panel's background and fit-box colour
-__constant__ uint8_t kWhite[3] = {255, 255, 255};
-__constant__ uint8_t kGrey[3] = {160, 160, 160};
 
 const int kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
                          41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
@@ -85,18 +74,11 @@ struct EncTables {
 };
 
 struct EncImg {
-    const uint8_t* src;  // BGR [h][fw][3]
-    const smapb_record* rec;  // NULL: no overlay
-    int h, w, mx, my, bw, bh;  // the encoded image's size, MCU columns / rows, luma block columns / rows
-    int fw;  // the frame's width: w, or w - h with the 3D panel in columns fw..w-1
-    int r, R;  // limb half-width and joint radius (overlay)
-    int pad_l, pad_t;  // letterbox of the net input (make_resize_plan)
-    double scale;
+    int h, w, mx, my, bw, bh;  // the encoded image's size (its Composite's), MCU columns / rows, luma block columns / rows
     long long blk0;  // first block in the batch's block order
     long long plane0;  // Y plane [16 my][16 mx], then Cb and Cr [8 my][8 mx]
     long long word0;  // first word of the image's bit buffer
     long long bound_bits;  // blocks * BLOCK_BITS_MAX
-    long long label0;  // first label of the image's plane [h][w] (overlay only; the panel's labels from column fw)
 };
 
 // per-image results of the totals kernel
@@ -114,62 +96,15 @@ __device__ __forceinline__ int find_image(const EncImg* im, int n, long long g) 
     return lo;
 }
 
-// ---- overlay ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool joint_xy(const EncImg& I, const float* pj, long long* x, long long* y) {
-    if (!(pj[3] > 0.f) || !isfinite(pj[0]) || !isfinite(pj[1])) return false;
-    const double fx = rint(((double)pj[0] - I.pad_l) / I.scale), fy = rint(((double)pj[1] - I.pad_t) / I.scale);
-    *x = (long long)fmin(fmax(fx, (double)-COORD_MAX), (double)COORD_MAX);
-    *y = (long long)fmin(fmax(fy, (double)-COORD_MAX), (double)COORD_MAX);
-    return true;
-}
-
-__global__ void __launch_bounds__(256) overlay_kernel(const EncImg* __restrict__ imgs, int* __restrict__ labels) {
-    const EncImg& I = imgs[blockIdx.y];
-    if (!I.rec) return;
-    const int p = blockIdx.x / NELEM, e = blockIdx.x % NELEM;
-    if (p >= I.rec->count) return;
-    const float* P = &I.rec->pred2d[p][0][0];
-    long long ax, ay, bx, by, rad;
-    if (e < SMAPB_NL) {
-        if (!joint_xy(I, P + 4 * kPairs[e][0], &ax, &ay) || !joint_xy(I, P + 4 * kPairs[e][1], &bx, &by)) return;
-        rad = I.r;
-    } else {
-        if (!joint_xy(I, P + 4 * (e - SMAPB_NL), &ax, &ay)) return;
-        bx = ax, by = ay, rad = I.R;
-    }
-    // the frame's columns only: with a 3D panel the label plane is as wide as the composite
-    paint_band(labels + I.label0, I.w, I.fw, I.h, ax, ay, bx, by, rad, p * NELEM + e + 1);
-}
-
-// ---- colour ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void load_pixel(const EncImg& I, const int* __restrict__ labels, int x, int y, int* b, int* g, int* r) {
-    const size_t i = (size_t)y * I.w + x;
-    const uint8_t* c = nullptr;
-    if (x >= I.fw) {  // the 3D panel: white, or its element's colour (view3d.h)
-        const int l = labels[I.label0 + i];
-        c = l == 0 ? kWhite : (l & 7) == PANEL_GREY ? kGrey : kPalette[l & 7];
-    } else {
-        const uint8_t* s = I.src + ((size_t)y * I.fw + x) * 3;
-        *b = s[0], *g = s[1], *r = s[2];
-        if (I.rec) {
-            const int l = labels[I.label0 + i];
-            if (l > 0) {
-                const int e = (l - 1) % NELEM, p = (l - 1) / NELEM;
-                c = e < SMAPB_NL ? kPalette[p % 6] : kJoint;
-            }
-        }
-    }
-    if (c) *b = c[0], *g = c[1], *r = c[2];
-}
-
 // libjpeg-turbo's RGB -> YCbCr: 16-bit fixed point, Cb and Cr rounded with 1/2 - epsilon
 __device__ __forceinline__ int ycc_y(int r, int g, int b) { return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16; }
 __device__ __forceinline__ int ycc_cb(int r, int g, int b) { return (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16; }
 __device__ __forceinline__ int ycc_cr(int r, int g, int b) { return (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16; }
 
-__global__ void __launch_bounds__(256) colour_kernel(const EncImg* __restrict__ imgs, const int* __restrict__ labels,
-                                                     uint8_t* __restrict__ planes) {
+__global__ void __launch_bounds__(256) colour_kernel(const EncImg* __restrict__ imgs, const Composite* __restrict__ comps,
+                                                     const int* __restrict__ labels, uint8_t* __restrict__ planes) {
     const EncImg& I = imgs[blockIdx.y];
+    const Composite& P = comps[blockIdx.y];
     const int cw = 8 * I.mx;
     const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= (long long)cw * 8 * I.my) return;
@@ -186,9 +121,9 @@ __global__ void __launch_bounds__(256) colour_kernel(const EncImg* __restrict__ 
         for (int dx = 0; dx < 2; dx++) {
             const int x = min(2 * cx + dx, I.w - 1);
             int b, g, r;
-            load_pixel(I, labels, x, min(2 * cy + dy, I.h - 1), &b, &g, &r);
+            load_pixel(P, labels, x, min(2 * cy + dy, I.h - 1), &b, &g, &r);
             Y[(size_t)(2 * cy + dy) * yw + 2 * cx + dx] = (uint8_t)ycc_y(r, g, b);
-            if (cys != cy) load_pixel(I, labels, x, min(2 * cys + dy, I.h - 1), &b, &g, &r);
+            if (cys != cy) load_pixel(P, labels, x, min(2 * cys + dy, I.h - 1), &b, &g, &r);
             cb += ycc_cb(r, g, b);
             cr += ycc_cr(r, g, b);
         }
@@ -382,80 +317,6 @@ __global__ void __launch_bounds__(128) bits_kernel(const EncImg* __restrict__ im
     bits[g] = total;
 }
 
-// ---- exclusive scan (uint32 items -> uint64 offsets, the grand total after the last) ------------------------------
-__device__ __forceinline__ unsigned long long block_exclusive(unsigned long long v, unsigned long long* total) {
-    __shared__ unsigned long long warp_sums[SCAN_THREADS / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    unsigned long long x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sums[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-        unsigned long long s = lane < SCAN_THREADS / 32 ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < SCAN_THREADS / 32) warp_sums[lane] = s;
-    }
-    __syncthreads();
-    const unsigned long long before = (wid ? warp_sums[wid - 1] : 0) + x - v;
-    *total = warp_sums[SCAN_THREADS / 32 - 1];
-    __syncthreads();
-    return before;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) scan_reduce_kernel(const uint32_t* __restrict__ in, long long n,
-                                                                   unsigned long long* __restrict__ tile_sums) {
-    const long long base = (long long)blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-    unsigned long long s = 0;
-#pragma unroll
-    for (int i = 0; i < SCAN_ITEMS; i++)
-        if (base + i < n) s += in[base + i];
-    unsigned long long total;
-    block_exclusive(s, &total);
-    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) scan_tiles_kernel(unsigned long long* __restrict__ tile_sums, long long ntiles,
-                                                                  unsigned long long* __restrict__ grand) {
-    unsigned long long carry = 0;
-    for (long long b = 0; b < ntiles; b += SCAN_THREADS) {
-        const long long i = b + threadIdx.x;
-        const unsigned long long v = i < ntiles ? tile_sums[i] : 0;
-        unsigned long long total;
-        const unsigned long long ex = block_exclusive(v, &total);
-        if (i < ntiles) tile_sums[i] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) *grand = carry;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) scan_apply_kernel(const uint32_t* __restrict__ in, long long n,
-                                                                  const unsigned long long* __restrict__ tile_sums,
-                                                                  unsigned long long* __restrict__ out) {
-    const long long base = (long long)blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-    uint32_t v[SCAN_ITEMS];
-    unsigned long long s = 0;
-#pragma unroll
-    for (int i = 0; i < SCAN_ITEMS; i++) {
-        v[i] = base + i < n ? in[base + i] : 0;
-        s += v[i];
-    }
-    unsigned long long total;
-    unsigned long long run = tile_sums[blockIdx.x] + block_exclusive(s, &total);
-#pragma unroll
-    for (int i = 0; i < SCAN_ITEMS; i++) {
-        if (base + i < n) out[base + i] = run;
-        run += v[i];
-    }
-}
-
 // ---- packing and stuffing ------------------------------------------------------------------------------------------
 // a block's bit range inside its image: [b0, b1); the last block's range ends at the image's total
 struct BitRange {
@@ -629,17 +490,15 @@ std::vector<uint8_t> jpeg_header(int q, int h, int w) {
 struct JpegEncWorkspace {
     PinnedBuffer<uint8_t> host;  // staging: descriptors and tables
     DeviceBuffer<uint8_t> dev_in;
-    PinnedBuffer<double> scales_host;
+    CompositeStage comp;
     DeviceBuffer<EncTotals> tot;
     PinnedBuffer<EncTotals> tot_host;
     DeviceBuffer<uint8_t> planes;
-    DeviceBuffer<int> labels;
     DeviceBuffer<int16_t> coef;
     DeviceBuffer<uint32_t> counts;  // bits, then 0xFF bytes, per block
     DeviceBuffer<unsigned long long> off;  // [nblk + 1] bit offsets
     DeviceBuffer<unsigned long long> ffoff;  // [nblk + 1] 0xFF counts before each block
     DeviceBuffer<unsigned long long> tiles;
-    DeviceBuffer<PanelSeg> segs;  // [n][PANEL_ELEMS] (3D panel)
     DeviceBuffer<uint32_t> words;
     DeviceBuffer<uint8_t> out;
     PinnedBuffer<uint8_t> result;  // the streams of the last call, back to back
@@ -656,73 +515,32 @@ const uint8_t* jpeg_enc_result(const JpegEncWorkspace* ws, int i, int64_t* nbyte
     return ws->result + ws->res_off[i];
 }
 
-// exclusive scan of in[0..n) into out[0..n], out[n] = the sum; 3 launches
-static int scan_counts(JpegEncWorkspace* ws, const uint32_t* in, long long n, unsigned long long* out, cudaStream_t st,
-                       std::string* err) {
-    const long long tiles = std::max(1ll, (n + SCAN_TILE - 1) / SCAN_TILE);
-    DECODE_CK(ws->tiles.grow((size_t)tiles));
-    scan_reduce_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(in, n, ws->tiles);
-    scan_tiles_kernel<<<1, SCAN_THREADS, 0, st>>>(ws->tiles, tiles, out + n);
-    scan_apply_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(in, n, ws->tiles, out);
-    DECODE_CK(cudaGetLastError());
-    return 0;
-}
-
 int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const int* img_h, const int* img_w, int quality,
                 const smapb_record* records, const double* scales, int flags, int64_t* nbytes, cudaStream_t st,
                 int64_t* launches, std::string* err) {
     ws->res_off.clear();
     ws->res_len.clear();
-    if (n < 0 || (n > 0 && (!bgr || !img_h || !img_w || !nbytes)) || (records && !scales)) {
+    if (int rc = composite_args("smapb_encode_jpeg", "smapb_encode_jpeg_ex", n, bgr, img_h, img_w, records, scales, flags, err))
+        return rc;
+    if (n > 0 && !nbytes) {
         *err = "smapb_encode_jpeg: null argument";
-        return -1;
-    }
-    if (flags & ~SMAPB_ENCODE_VIEW3D) {
-        *err = "smapb_encode_jpeg_ex: unknown flags " + std::to_string(flags);
-        return -1;
-    }
-    const bool view3d = flags & SMAPB_ENCODE_VIEW3D;
-    if (view3d && !records) {
-        *err = "smapb_encode_jpeg_ex: SMAPB_ENCODE_VIEW3D needs records";
         return -1;
     }
     if (quality < 1 || quality > 100) {
         *err = "smapb_encode_jpeg: quality " + std::to_string(quality) + " outside 1..100";
         return -1;
     }
-    for (int i = 0; i < n; i++) {
-        if (!bgr[i]) {
-            *err = "smapb_encode_jpeg: null frame " + std::to_string(i);
-            return -1;
-        }
-        if (img_h[i] < 1 || img_h[i] > 16384 || img_w[i] < 1 || img_w[i] > 16384) {
-            *err = "smapb_encode_jpeg: frame " + std::to_string(i) + " is " + std::to_string(img_w[i]) + "x" +
-                   std::to_string(img_h[i]) + " (sides must be 1..16384)";
-            return -1;
-        }
-        if (view3d && img_w[i] + img_h[i] > 16384) {
-            *err = "smapb_encode_jpeg_ex: frame " + std::to_string(i) + " is " + std::to_string(img_w[i]) + "x" +
-                   std::to_string(img_h[i]) + ": with its 3D panel it would be " + std::to_string(img_w[i] + img_h[i]) +
-                   " wide (sides must be 1..16384)";
-            return -1;
-        }
-    }
+    if (int rc = composite_frames("smapb_encode_jpeg", "smapb_encode_jpeg_ex", n, bgr, img_h, img_w, flags, err)) return rc;
     if (int rc = refuse_capture("smapb_encode_jpeg", st, err)) return rc;
     if (n == 0) return 0;
-    if (records) {  // the letterbox of each frame, from its scale row
-        DECODE_CK(ws->scales_host.grow((size_t)n * SMAPB_SCALE_LEN));
-        DECODE_CK(cudaMemcpyAsync(ws->scales_host, scales, sizeof(double) * n * SMAPB_SCALE_LEN, cudaMemcpyDeviceToHost, st));
-    }
-    DECODE_CK(cudaStreamSynchronize(st));  // the scales, and the workspace the previous call may still use
+    CompositeStage& cs = ws->comp;
+    if (int rc = composite_plan(&cs, "smapb_encode_jpeg", n, bgr, img_h, img_w, records, scales, flags, st, err)) return rc;
     std::vector<EncImg> imgs(n);
-    std::vector<PanelImg> panels(view3d ? n : 0);
-    long long nblk = 0, plane_total = 0, word_total = 0, label_total = 0;
+    long long nblk = 0, plane_total = 0, word_total = 0;
     for (int i = 0; i < n; i++) {
         EncImg& I = imgs[i];
         memset(&I, 0, sizeof(I));
-        I.src = bgr[i];
-        I.h = img_h[i], I.fw = img_w[i];
-        I.w = view3d ? I.fw + I.h : I.fw;
+        I.h = cs.imgs[i].h, I.w = cs.imgs[i].w;
         I.mx = (I.w + 15) / 16, I.my = (I.h + 15) / 16, I.bw = (I.w + 7) / 8, I.bh = (I.h + 7) / 8;
         I.blk0 = nblk;
         const long long nb = 6ll * I.mx * I.my;
@@ -732,23 +550,6 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         I.bound_bits = nb * BLOCK_BITS_MAX;
         I.word0 = word_total;
         word_total += (I.bound_bits + 31) / 32 + 1;
-        I.label0 = -1;
-        if (records) {
-            const double* row = ws->scales_host + (size_t)i * SMAPB_SCALE_LEN;
-            ResizePlan P;
-            if (row[1] != I.fw || row[2] != I.h || !make_resize_plan(I.fw, I.h, (int)row[3], (int)row[4], &P)) {
-                *err = "smapb_encode_jpeg: the scale row of frame " + std::to_string(i) + " does not describe a " +
-                       std::to_string(I.fw) + "x" + std::to_string(I.h) + " frame";
-                return -1;
-            }
-            I.rec = records + i;
-            I.scale = row[0], I.pad_l = P.pad_l, I.pad_t = P.pad_t;
-            const int m = std::min(I.fw, I.h);
-            I.r = std::max(1, m / 400), I.R = std::max(2, m / 200);
-            I.label0 = label_total;
-            label_total += (long long)I.w * I.h;
-            if (view3d) panels[i] = PanelImg{I.rec, I.h, I.w, I.label0 + I.fw};
-        }
     }
     EncTables T;
     memset(&T, 0, sizeof(T));
@@ -760,15 +561,14 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
         huff_codes(kDcBits[t], dcv, T.dc_code[t], T.dc_len[t]);
         huff_codes(kAcBits[t], kAcVals[t], T.ac_code[t], T.ac_len[t]);
     }
-    const size_t o_tab = align_up(sizeof(EncImg) * n, 256), o_pan = align_up(o_tab + sizeof(EncTables), 256);
-    const size_t total_in = o_pan + sizeof(PanelImg) * panels.size();
+    const size_t o_tab = align_up(sizeof(EncImg) * n, 256), o_comp = align_up(o_tab + sizeof(EncTables), 256);
+    const size_t o_pan = align_up(o_comp + sizeof(Composite) * n, 256);
+    const size_t total_in = o_pan + sizeof(PanelImg) * cs.panels.size();
     DECODE_CK(ws->host.grow(total_in));
     memcpy(ws->host, imgs.data(), sizeof(EncImg) * n);
     memcpy(ws->host + o_tab, &T, sizeof(T));
-    if (view3d) {
-        memcpy(ws->host + o_pan, panels.data(), sizeof(PanelImg) * n);
-        DECODE_CK(ws->segs.grow((size_t)n * PANEL_ELEMS));
-    }
+    memcpy(ws->host + o_comp, cs.imgs.data(), sizeof(Composite) * n);
+    if (!cs.panels.empty()) memcpy(ws->host + o_pan, cs.panels.data(), sizeof(PanelImg) * n);
     DECODE_CK(ws->dev_in.grow(total_in));
     DECODE_CK(ws->planes.grow((size_t)plane_total));
     DECODE_CK(ws->coef.grow((size_t)nblk * 64));
@@ -778,32 +578,24 @@ int jpeg_encode(JpegEncWorkspace* ws, int n, const uint8_t* const* bgr, const in
     DECODE_CK(ws->words.grow((size_t)word_total));
     DECODE_CK(ws->tot.grow((size_t)n));
     DECODE_CK(ws->tot_host.grow((size_t)n));
-    if (label_total) DECODE_CK(ws->labels.grow((size_t)label_total));
     const EncImg* d_img = (const EncImg*)ws->dev_in.get();
     const EncTables* d_tab = (const EncTables*)(ws->dev_in + o_tab);
+    const Composite* d_comp = (const Composite*)(ws->dev_in + o_comp);
     DECODE_CK(cudaMemcpyAsync(ws->dev_in, ws->host, total_in, cudaMemcpyHostToDevice, st));
     int max_mcus = 0;
     for (const EncImg& I : imgs) max_mcus = std::max(max_mcus, I.mx * I.my);
-    if (label_total) {
-        DECODE_CK(cudaMemsetAsync(ws->labels, 0, sizeof(int) * label_total, st));
-        overlay_kernel<<<dim3(SMAPB_MAXP * NELEM, n), 256, 0, st>>>(d_img, ws->labels);
-        ++*launches;
-        if (view3d) {
-            panel_launch((const PanelImg*)(ws->dev_in + o_pan), n, ws->segs, ws->labels, st);
-            *launches += 2;
-        }
-    }
+    if (int rc = composite_launch(&cs, d_comp, (const PanelImg*)(ws->dev_in + o_pan), n, st, launches, err)) return rc;
     const unsigned fgrid = (unsigned)((nblk + 127) / 128), bgrid = (unsigned)((nblk + 255) / 256);
-    colour_kernel<<<dim3((unsigned)((64ll * max_mcus + 255) / 256), n), 256, 0, st>>>(d_img, ws->labels, ws->planes);
+    colour_kernel<<<dim3((unsigned)((64ll * max_mcus + 255) / 256), n), 256, 0, st>>>(d_img, d_comp, cs.labels, ws->planes);
     fdct_kernel<<<fgrid, 128, 0, st>>>(d_img, n, nblk, d_tab, ws->planes, ws->coef);
     bits_kernel<<<fgrid, 128, 0, st>>>(d_img, n, nblk, d_tab, ws->coef, ws->counts);
     DECODE_CK(cudaGetLastError());
-    if (int rc = scan_counts(ws, ws->counts, nblk, ws->off, st, err)) return rc;
+    if (int rc = exclusive_scan(&ws->tiles, ws->counts, nblk, ws->off, st, err)) return rc;
     zero_kernel<<<bgrid, 256, 0, st>>>(d_img, n, nblk, ws->off, ws->words);
     pack_kernel<<<fgrid, 128, 0, st>>>(d_img, n, nblk, d_tab, ws->coef, ws->off, ws->words);
     ff_kernel<<<bgrid, 256, 0, st>>>(d_img, n, nblk, ws->off, ws->words, ws->counts);
     DECODE_CK(cudaGetLastError());
-    if (int rc = scan_counts(ws, ws->counts, nblk, ws->ffoff, st, err)) return rc;
+    if (int rc = exclusive_scan(&ws->tiles, ws->counts, nblk, ws->ffoff, st, err)) return rc;
     const std::vector<uint8_t> hdr0 = jpeg_header(quality, 1, 1);
     const long long L = (long long)hdr0.size();
     totals_kernel<<<1, 1, 0, st>>>(d_img, n, nblk, ws->off, ws->ffoff, L, ws->tot);

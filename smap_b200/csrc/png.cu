@@ -41,6 +41,7 @@
 #include <vector>
 
 #include "../../include/smap_b200.h"
+#include "checksum.cuh"
 #include "decode_host.h"
 #include "orient.h"
 #include "png.h"
@@ -89,22 +90,6 @@ enum { ST_CAND = 0, ST_ONCHAIN = 1, ST_CONFIRMED = 2, ST_SERIAL = 3 };
 
 // ---- host chunk walk -------------------------------------------------------------------------------------------------
 inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
-
-uint32_t crc32_host(const uint8_t* p, int64_t n) {
-    static uint32_t T[256];
-    static bool init = false;
-    if (!init) {
-        for (uint32_t i = 0; i < 256; i++) {
-            uint32_t c = i;
-            for (int k = 0; k < 8; k++) c = c & 1 ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-            T[i] = c;
-        }
-        init = true;
-    }
-    uint32_t c = 0xFFFFFFFFu;
-    for (int64_t i = 0; i < n; i++) c = T[(c ^ p[i]) & 255] ^ (c >> 8);
-    return ~c;
-}
 
 struct PngHeader {
     int w = 0, h = 0, depth = 0, ctype = 0, interlace = 0, orientation = 1, out_h = 0, out_w = 0, npal = 0, wsize = 0;
@@ -459,31 +444,6 @@ __device__ bool stored_block(const uint32_t* __restrict__ words, uint32_t zbits,
 __device__ __forceinline__ void set_status(int* status, int img, int s) { atomicCAS(&status[img], SMAPB_JPEG_OK, s); }
 
 // ---- 1. gather + IDAT CRCs -------------------------------------------------------------------------------------------
-__device__ uint32_t multmodp(uint32_t a, uint32_t b) {  // a * b modulo the CRC-32 polynomial (reflected bit order)
-    uint32_t m = 1u << 31, p = 0;
-    for (;;) {
-        if (a & m) {
-            p ^= b;
-            if ((a & (m - 1)) == 0) break;
-        }
-        m >>= 1;
-        b = b & 1 ? (b >> 1) ^ 0xEDB88320u : b >> 1;
-    }
-    return p;
-}
-
-// x^(8 n) mod P from the table x2n[k] = x^(2^k) mod P
-__device__ uint32_t x8nmodp(const uint32_t* x2n, uint64_t n) {
-    uint32_t p = 1u << 31;  // x^0
-    int k = 3;
-    while (n) {
-        if (n & 1) p = multmodp(x2n[k & 31], p);
-        n >>= 1;
-        k++;
-    }
-    return p;
-}
-
 constexpr int GATHER_THREADS = 512;
 
 __global__ void __launch_bounds__(GATHER_THREADS) gather_kernel(const DevPng* __restrict__ imgs, const DevChunk* __restrict__ chunks,
@@ -492,17 +452,7 @@ __global__ void __launch_bounds__(GATHER_THREADS) gather_kernel(const DevPng* __
     __shared__ uint32_t T[256], x2n[32], red[GATHER_THREADS / 32];
     const DevPng& I = imgs[blockIdx.x];
     const int tid = threadIdx.x;
-    for (int i = tid; i < 256; i += blockDim.x) {
-        uint32_t c = i;
-        for (int k = 0; k < 8; k++) c = c & 1 ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-        T[i] = c;
-    }
-    if (tid == 0) {
-        uint32_t p = 1u << 30;  // x^1
-        x2n[0] = p;
-        for (int k = 1; k < 32; k++) x2n[k] = p = multmodp(p, p);
-    }
-    __syncthreads();
+    crc_tables(T, x2n);
     uint8_t* zs = stream + I.zoff;
     const int64_t zlen = I.zbits / 8;
     for (int i = tid; i < 16; i += blockDim.x) zs[zlen + i] = 0;
@@ -510,19 +460,16 @@ __global__ void __launch_bounds__(GATHER_THREADS) gather_kernel(const DevPng* __
         const DevChunk C = chunks[I.chunk0 + c];
         const uint8_t* src = in + C.src;
         for (uint32_t j = tid; j < C.len; j += blockDim.x) zs[C.dst + j] = src[4 + j];
-        // CRC over type + payload: thread slices from a zero register, each shifted by the bytes after it
-        const uint64_t L = 4ull + C.len, S = (L + blockDim.x - 1) / blockDim.x;
-        const uint64_t a = min(L, tid * S), b = min(L, a + S);
-        uint32_t r = 0;
-        for (uint64_t j = a; j < b; j++) r = T[(r ^ src[j]) & 255] ^ (r >> 8);
-        if (a < b && b < L) r = multmodp(x8nmodp(x2n, L - b), r);
+        // CRC over type + payload
+        const uint64_t L = 4ull + C.len;
+        uint32_t r = crc_slice(T, x2n, L, [&](uint64_t j) { return src[j]; });
         for (int o = 16; o; o >>= 1) r ^= __shfl_xor_sync(0xffffffffu, r, o);
         if ((tid & 31) == 0) red[tid >> 5] = r;
         __syncthreads();
         if (tid == 0) {
-            uint32_t t = multmodp(x8nmodp(x2n, L), 0xFFFFFFFFu);
+            uint32_t t = 0;
             for (int w = 0; w < (int)(blockDim.x / 32); w++) t ^= red[w];
-            if (~t != C.crc) set_status(status, blockIdx.x, SMAPB_JPEG_CORRUPT);
+            if (crc_finish(x2n, L, t) != C.crc) set_status(status, blockIdx.x, SMAPB_JPEG_CORRUPT);
         }
         __syncthreads();
     }
@@ -698,7 +645,6 @@ __global__ void __launch_bounds__(64) write_kernel(const DevPng* __restrict__ im
 
 // ---- 6. resolve + Adler-32 -------------------------------------------------------------------------------------------
 constexpr int RESOLVE_THREADS = 1024;
-constexpr uint32_t ADLER_MOD = 65521;
 
 __global__ void __launch_bounds__(RESOLVE_THREADS) resolve_kernel(const DevPng* __restrict__ imgs, const DevBlock* __restrict__ blocks,
                                                                   const int* __restrict__ nblk, const uint16_t* __restrict__ marks,

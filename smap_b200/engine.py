@@ -274,21 +274,48 @@ class Engine:
         encoded with its skeletons drawn over it (smapb_encode_jpeg, include/smap_b200.h).  view3d (records required):
         each H x W frame is encoded as an H x (W + H) composite, the drawn frame and an H x H panel of its 3D skeletons
         (smapb_encode_jpeg_ex with SMAPB_ENCODE_VIEW3D; oracle/view3d_numpy.py).  The frames are not modified."""
+        a = self._encode_args("encode_jpeg", frames, records, scales, view3d)
+        if a is None:
+            return []
+        n, ptrs, hs, ws, rec, sc, sizes = a
+        if view3d:
+            self._check(self.lib.smapb_encode_jpeg_ex(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), ENCODE_VIEW3D,
+                                                      sizes, self._st()), "smapb_encode_jpeg_ex")
+        else:
+            self._check(self.lib.smapb_encode_jpeg(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), sizes,
+                                                   self._st()), "smapb_encode_jpeg")
+        return self._encoded(self.lib.smapb_encoded_jpeg, "smapb_encoded_jpeg", sizes)
+
+    def encode_png(self, frames, records=None, scales=None, view3d=False):
+        """As encode_jpeg, but lossless: per frame (or composite) what cv2.imencode(".png", frame) writes
+        (smapb_encode_png, include/smap_b200.h; oracle/png_encode_numpy.py)."""
+        a = self._encode_args("encode_png", frames, records, scales, view3d)
+        if a is None:
+            return []
+        n, ptrs, hs, ws, rec, sc, sizes = a
+        self._check(self.lib.smapb_encode_png(self._h, n, ptrs, hs, ws, _ptr(rec), _ptr(sc), ENCODE_VIEW3D if view3d else 0,
+                                              sizes, self._st()), "smapb_encode_png")
+        return self._encoded(self.lib.smapb_encoded_png, "smapb_encoded_png", sizes)
+
+    def _encode_args(self, name, frames, records, scales, view3d):
+        """The encoders' arguments: frames uploaded, records and scales checked -> (n, frame pointers, heights, widths,
+        records, scales, sizes), or None for no frames.  The device copies live as long as the returned tuple."""
         n = len(frames)
         if view3d and records is None:
-            raise ValueError("encode_jpeg: view3d needs records and scales")
+            raise ValueError("%s: view3d needs records and scales" % name)
         if n == 0:
-            return []
+            return None
         if (records is None) != (scales is None):
-            raise ValueError("encode_jpeg: records and scales go together")
+            raise ValueError("%s: records and scales go together" % name)
         dev = []
         for f in frames:
             if not torch.is_tensor(f):
                 f = torch.from_numpy(np.ascontiguousarray(f))
             if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                raise ValueError("encode_jpeg: uint8 BGR [H,W,3] frames expected")
+                raise ValueError("%s: uint8 BGR [H,W,3] frames expected" % name)
             dev.append(f.to(self.device).contiguous())
         ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in dev])
+        ptrs._frames = dev  # keeps the device copies alive with the pointer array
         hs = (ctypes.c_int * n)(*[f.shape[0] for f in dev])
         ws = (ctypes.c_int * n)(*[f.shape[1] for f in dev])
         rec = sc = None
@@ -296,18 +323,14 @@ class Engine:
             rec = records.to(self.device).contiguous()
             sc = torch.as_tensor(scales, dtype=torch.float64).to(self.device).contiguous()
             if rec.dtype != torch.uint8 or tuple(rec.shape) != (n, RECORD_BYTES) or tuple(sc.shape) != (n, SCALE_LEN):
-                raise ValueError("encode_jpeg: records uint8 [n, %d] and scales float64 [n, %d] expected" % (RECORD_BYTES, SCALE_LEN))
-        sizes = (ctypes.c_int64 * n)()
-        if view3d:
-            self._check(self.lib.smapb_encode_jpeg_ex(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), ENCODE_VIEW3D,
-                                                      sizes, self._st()), "smapb_encode_jpeg_ex")
-        else:
-            self._check(self.lib.smapb_encode_jpeg(self._h, n, ptrs, hs, ws, int(quality), _ptr(rec), _ptr(sc), sizes,
-                                                   self._st()), "smapb_encode_jpeg")
+                raise ValueError("%s: records uint8 [n, %d] and scales float64 [n, %d] expected" % (name, RECORD_BYTES, SCALE_LEN))
+        return n, ptrs, hs, ws, rec, sc, (ctypes.c_int64 * n)()
+
+    def _encoded(self, get, name, sizes):
         out = []
-        for i in range(n):
+        for i in range(len(sizes)):
             p = ctypes.POINTER(ctypes.c_uint8)()
-            self._check(self.lib.smapb_encoded_jpeg(self._h, i, ctypes.byref(p), None), "smapb_encoded_jpeg")
+            self._check(get(self._h, i, ctypes.byref(p), None), name)
             out.append(ctypes.string_at(p, sizes[i]))
         return out
 

@@ -3,7 +3,7 @@ path: images on disk -> result JSON.
 
     python -m smap_b200.run_inference -p SMAP.pth [-rp RefineNet.pth] --dataset_path DIR --batch_size 8 --do_flip 1 \
         [--json_name SUFFIX] [--output_dir OUT] [--dataset_name CMU] [--precision {bf16x3,fp16,bf16}] [--jpeg_colour 1]
-        [--vis_dir DIR [--vis_quality 95] [--vis_3d 1]]
+        [--vis_dir DIR [--vis_format {jpg,png}] [--vis_quality 95] [--vis_3d 1]]
 
 Same flags and the same output file name / schema as the reference ('{OUT}/stage3_root2_run_inference_{data_mode}_{suffix}.json',
 test.py:147-152).  Differences, both deliberate: images are visited in sorted path order unless --glob_order 1 (the
@@ -58,12 +58,13 @@ def image_name(path, dataset_path):
     return path.rstrip().replace(dataset_path, "").lstrip("/")
 
 
-def vis_names(paths, dataset_path):
+def vis_names(paths, dataset_path, ext=".jpg"):
     """-> per image the relative path of its annotated frame under --vis_dir: its image name with the extension replaced
-    by .jpg.  Raises ValueError naming both inputs when two images would write the same file (a.png and a.jpg)."""
+    by ext (".jpg", or ".png" with --vis_format png).  Raises ValueError naming both inputs when two images would write
+    the same file (a.png and a.jpg)."""
     names, seen = [], {}
     for p in paths:
-        name = osp.splitext(image_name(p, dataset_path))[0] + ".jpg"
+        name = osp.splitext(image_name(p, dataset_path))[0] + ext
         if name in seen:
             raise ValueError("--vis_dir: %s and %s would both be written to %s" % (seen[name], p, name))
         seen[name] = p
@@ -74,10 +75,11 @@ def vis_names(paths, dataset_path):
 VIEW3D_MAX_WIDTH = 16384  # the encoder's largest side: a frame of w + h over it has no room for its 3D panel
 
 
-def write_vis(eng, vis_dir, quality, names, frames, records, scales, view3d=False):
-    """Encodes the frames with their skeletons drawn (Engine.encode_jpeg on the device records and scale rows) and writes
-    them to vis_dir/names[i], creating subdirectories.  view3d: each frame with the panel of its 3D skeletons on its right;
-    a frame too wide for that composite raises ValueError naming it."""
+def write_vis(eng, vis_dir, quality, names, frames, records, scales, view3d=False, fmt="jpg"):
+    """Encodes the frames with their skeletons drawn (Engine.encode_jpeg at quality on the device records and scale rows,
+    or with fmt "png" Engine.encode_png, lossless) and writes them to vis_dir/names[i], creating subdirectories.
+    view3d: each frame with the panel of its 3D skeletons on its right; a frame too wide for that composite raises
+    ValueError naming it."""
     kw = {}
     if view3d:
         for name, f in zip(names, frames):
@@ -85,7 +87,11 @@ def write_vis(eng, vis_dir, quality, names, frames, records, scales, view3d=Fals
                 raise ValueError("--vis_3d: %s is %dx%d, so its composite would be %d pixels wide (at most %d)"
                                  % (name, f.shape[1], f.shape[0], f.shape[0] + f.shape[1], VIEW3D_MAX_WIDTH))
         kw = dict(view3d=True)
-    for name, data in zip(names, eng.encode_jpeg(frames, quality, records, scales, **kw)):
+    if fmt == "png":
+        files = eng.encode_png(frames, records, scales, **kw)
+    else:
+        files = eng.encode_jpeg(frames, quality, records, scales, **kw)
+    for name, data in zip(names, files):
         path = osp.join(vis_dir, name)
         os.makedirs(osp.dirname(path) or ".", exist_ok=True)
         with open(path, "wb") as f:
@@ -150,7 +156,7 @@ def _load_weights(eng, smap_state_dict, refine_state_dict, precision):
 
 def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False, dataset_name="CMU",
         device=0, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3", stats=None, jpeg_colour=False,
-        vis_dir=None, vis_quality=95, vis_3d=False):
+        vis_dir=None, vis_quality=95, vis_3d=False, vis_format="jpg"):
     """-> number of images processed.  imread(path) -> uint8 BGR [H,W,3], used for every file; by default .jpg/.jpeg
     and .png files are decoded on the GPU (Engine.decode_jpeg, then Engine.decode_jpeg_ex for the progressive and
     multi-scan JPEGs decode_jpeg leaves, and Engine.decode_png; byte-identical to cv2.imread) and the
@@ -158,12 +164,13 @@ def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batc
     YCCK and RGB JPEGs and every integral sampling are decoded on the GPU too (Engine.decode_jpeg_ex(colour=True));
     off by default, so those files keep going to cv2.imread.  precision: one of engine.PRECISIONS.  stats (a dict,
     optional) receives "saturation": the fp16 clamp count.  vis_dir: also write every image with its skeletons drawn,
-    JPEG-encoded at vis_quality on the GPU (write_vis), to vis_dir/<image name with a .jpg extension>; vis_3d: with the
-    panel of its 3D skeletons on the right of each frame."""
+    JPEG-encoded at vis_quality on the GPU (write_vis), to vis_dir/<image name with a .jpg extension>, or with vis_format
+    "png" PNG-encoded (lossless) to vis_dir/<image name with a .png extension>; vis_3d: with the panel of its 3D skeletons
+    on the right of each frame."""
     if precision not in PRECISIONS:
         raise ValueError("unknown precision %r (choose from %s)" % (precision, ", ".join(PRECISIONS)))
     paths = list_images(dataset_path, glob_order)
-    names = vis_names(paths, dataset_path) if vis_dir else None
+    names = vis_names(paths, dataset_path, _vis_ext(vis_format)) if vis_dir else None
     eng = Engine(device, max_batch=batch_size, in_h=in_h, in_w=in_w)
     try:
         _load_weights(eng, smap_state_dict, refine_state_dict, precision)
@@ -179,7 +186,7 @@ def run(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batc
                 torch.cuda.current_stream().synchronize()
                 w.append(host[:len(chunk)], [image_name(p, dataset_path) for p in chunk])
                 if vis_dir:
-                    write_vis(eng, vis_dir, vis_quality, names[lo:lo + batch_size], frames, rec, scales, vis_3d)
+                    write_vis(eng, vis_dir, vis_quality, names[lo:lo + batch_size], frames, rec, scales, vis_3d, vis_format)
         if stats is not None:
             stats["saturation"] = eng.saturation_count()
         return len(paths)
@@ -310,7 +317,7 @@ class _GatherSteps:
 
 def run_distributed(smap_state_dict, dataset_path, output_file, refine_state_dict=None, batch_size=8, do_flip=False,
                     dataset_name="CMU", device=None, in_h=512, in_w=832, imread=None, glob_order=False, precision="bf16x3",
-                    stats=None, jpeg_colour=False, vis_dir=None, vis_quality=95, vis_3d=False):
+                    stats=None, jpeg_colour=False, vis_dir=None, vis_quality=95, vis_3d=False, vis_format="jpg"):
     """run() on every rank of torch.distributed's default group (gloo), with the same arguments; batch_size frames per
     rank and step, device None = LOCAL_RANK.  Rank 0 lists the images and alone writes output_file, byte-identical to
     run()'s; with vis_dir every rank writes the annotated frames of its own shard.  -> number of images;
@@ -343,10 +350,10 @@ def run_distributed(smap_state_dict, dataset_path, output_file, refine_state_dic
         paths = box[0]
         vis = None
         if vis_dir:
-            names = vis_names(paths, dataset_path)  # the same list on every rank: all of them refuse a collision
+            names = vis_names(paths, dataset_path, _vis_ext(vis_format))  # the same list on every rank: all refuse a collision
 
             def vis(indices, frames, records, scales):
-                write_vis(eng, vis_dir, vis_quality, [names[i] for i in indices], frames, records, scales, vis_3d)
+                write_vis(eng, vis_dir, vis_quality, [names[i] for i in indices], frames, records, scales, vis_3d, vis_format)
         steps = _GatherSteps(eng, frame_reader(eng, imread, jpeg_colour), paths, bool(do_flip), vis)
         saturation = drive(len(paths), batch_size, steps,
                            lambda rec, frames: writer.append(rec, [image_name(paths[i], dataset_path) for i in frames]))
@@ -389,7 +396,11 @@ def main(argv=None):
                          "GPU instead of with cv2.imread")
     ap.add_argument("--vis_dir", default="", help="also write every image with its skeletons drawn, JPEG-encoded on the GPU, "
                                                   "to VIS_DIR/<image name with a .jpg extension>")
-    ap.add_argument("--vis_quality", type=int, default=95, help="JPEG quality of --vis_dir, 1..100 (cv2's default 95)")
+    ap.add_argument("--vis_format", default="jpg", choices=["jpg", "png"],
+                    help="file format of --vis_dir: jpg (default) or png (lossless, cv2.imencode's bytes), both encoded "
+                         "on the GPU; the files are named <image name>.<format>")
+    ap.add_argument("--vis_quality", type=int, default=95,
+                    help="JPEG quality of --vis_dir, 1..100 (cv2's default 95); JPEG only, --vis_format png ignores it")
     ap.add_argument("--vis_3d", type=int, default=0, choices=[0, 1],
                     help="1: put a panel with the 3D skeletons (pred_3d, seen as lib/visualize/vis.py shows them) on the "
                          "right of every --vis_dir frame")
@@ -398,6 +409,8 @@ def main(argv=None):
         ap.error("--vis_quality must be in 1..100")
     if a.vis_3d and not a.vis_dir:
         ap.error("--vis_3d needs --vis_dir")
+    if a.vis_format != "jpg" and not a.vis_dir:
+        ap.error("--vis_format needs --vis_dir")
     if "WORLD_SIZE" in os.environ:
         return _main_distributed(a)
     try:
@@ -415,12 +428,20 @@ def main(argv=None):
 
 
 def _vis_kwargs(a):
-    """--vis_dir / --vis_quality / --vis_3d as run()'s keyword arguments; none without --vis_dir, and vis_3d only when
-    set, so that run is called as before without them."""
+    """--vis_dir / --vis_quality / --vis_3d / --vis_format as run()'s keyword arguments; none without --vis_dir, and
+    vis_3d and vis_format only when they differ from the default, so that run is called as before without them."""
     kw = dict(vis_dir=a.vis_dir, vis_quality=a.vis_quality) if a.vis_dir else {}
     if a.vis_3d:
         kw["vis_3d"] = True
+    if a.vis_format != "jpg":
+        kw["vis_format"] = a.vis_format
     return kw
+
+
+def _vis_ext(vis_format):
+    if vis_format not in ("jpg", "png"):
+        raise ValueError("vis_format must be jpg or png, not %r" % (vis_format,))
+    return "." + vis_format
 
 
 def _load_checkpoints(a):
